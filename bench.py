@@ -4,19 +4,23 @@
 Headline workload (BASELINE.json configs[1]): GpuIndexFlatL2, N=10M, d=128, nq=10k, k=100, synthetic fp32.
 A "step" = one search() of all nq queries over the whole database.
 
-  python bench.py --gpus 1 --steps K --warmup W            # this framework (tcgen05 Flat path)
+  python bench.py --gpus 1 --steps K --warmup W            # this framework (tensor-core Flat path)
   python bench.py --impl reference --gpus 1 --steps K ...   # reference CPU IndexFlatL2 (oracle/_ref)
   torchrun --nproc-per-node N bench.py --gpus N ...         # database sharded over N GPUs
                                                             # (IndexShards semantics, NCCL all-gather merge)
 
 One JSON line on stdout (rank 0).  `value` = QPS with inputs resident in HBM; `e2e` = QPS through
 the public API with host (pinned) buffers, H2D/D2H inside the timed region; `roofline` = algorithmic
-FLOPs of the step / device time inside the tcgen05 kernel, vs the measured bf16 GEMM peak;
+FLOPs of the step / device time inside the wgmma kernel, vs the measured bf16 GEMM peak;
 `parity_check` = the step's result compared (outside the timed region) with an unsharded exact answer
 and with the reference CPU library; `workloads.ivfpq` (N=1 only) = BASELINE configs[3] (IVFPQ N=100M)
 with its own roofline (scan kernel, HBM), e2e, CPU IndexIVFPQ baseline on the CLONED index and
 recall@1/10/100 for CPU and GPU; `workloads.ivfpq_synthetic` = the same on contrib/datasets.py's
 SyntheticDataset distribution, where IVF/PQ recall is meaningful.
+
+--dump-outputs DIR writes the last timed step's result (distances.npy float32 [nq, k], labels.npy float64
+[nq, k]) so that two builds can be compared output for output: the inputs are seeded and identical from run
+to run.
 """
 import argparse
 import ctypes
@@ -55,11 +59,12 @@ def peaks():
             return j, "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA's H100 SXM data sheet (700 W): dense BF16, HBM3 -- upper bounds, not measured rates
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data-sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe).  nvidia-smi
+    """nvidia-smi clocks / throttle reasons during the timed region.  nvidia-smi
     needs ~0.5 s to produce its first line, so it is started before the warm-up; samples are time-stamped
     on arrival and only those inside [mark_begin, mark_end] (the timed region) are used -- widened to the
     warm-up steps of the same workload if the timed region is shorter than one sampling period."""
@@ -135,6 +140,17 @@ class ClockSampler:
                 "samples": len(sm), "power_w_max": float(max(power)), "window": window}
 
 
+def gpu_identity(gpu_index=0):
+    """name, power limit and max SM clock of the card: an absolute number is only meaningful with these"""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(gpu_index), "--query-gpu=name,power.limit,clocks.max.sm",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+        name, plim, smax = [x.strip() for x in r.stdout.strip().split(",")[:3]]
+        return {"name": name, "power_limit_w": float(plim), "sm_max_mhz": float(smax)}
+    except Exception as e:
+        return {"error": str(e)[:100]}
+
+
 def gen_rows(torch, device, r0, r1, d, n_total=None, seed0=1234):
     """rows [r0, r1) of the synthetic database: uniform [0,1) fp32, chunk c seeded with seed0 + c"""
     n_total = N_TOTAL if n_total is None else n_total
@@ -194,9 +210,9 @@ def _blas_sample_queries(nq, d):
 
 
 def ref_thread_sweep(ref, xb, xq, k, cores):
-    """Best thread count for the reference's BLAS + OpenMP path on this host.  This image's OpenBLAS is
-    a pthreads build whose pool oversubscribes badly next to OpenMP when handed every CPU of a large
-    host (round 1: 96 threads were 12x slower than 16), so the count is measured, not assumed."""
+    """Best thread count for the reference's BLAS + OpenMP path on this host.  A pthreads OpenBLAS build
+    oversubscribes badly next to OpenMP when handed every CPU of a large host, so the count is measured,
+    not assumed."""
     cand = sorted({t for t in (2, 4, 8, 12, 16, 24, 32, 48, 64, cores) if 1 <= t <= cores})
     rows = min(xb.shape[0], 100_000)
     idx = ref.IndexFlat(xb.shape[1], 1)
@@ -216,7 +232,7 @@ def ref_thread_sweep(ref, xb, xq, k, cores):
     return best, {str(t): round(v, 4) for t, v in res.items()}
 
 
-def cpu_flat_reference(xb_host, xq_host, k, step_budget_s, steps, warmup, total_budget_s):
+def cpu_flat_reference(xb_host, xq_host, k, step_budget_s, steps, warmup):
     """Times faiss::IndexFlatL2 (oracle/_ref) on a bounded sample: the first ns queries (BLAS path) against a
     leading slice of the rows sized so one step fits `step_budget_s`.  Returns (qps_full, info): qps_full is
     the sample's rate scaled to the full N (exhaustive search is linear in the rows scanned);
@@ -241,8 +257,8 @@ def cpu_flat_reference(xb_host, xq_host, k, step_budget_s, steps, warmup, total_
     nrows = min(nrows, nfull)
     idx = ref.IndexFlat(d, 1)
     idx.add(xb_host[:nrows])
+    # every requested step is timed: the row slice above bounds the time of one step, not their number
     ts = []
-    t_begin = time.time()
     D = I = None
     for i in range(warmup + steps):
         t0 = time.time()
@@ -250,8 +266,6 @@ def cpu_flat_reference(xb_host, xq_host, k, step_budget_s, steps, warmup, total_
         dt = time.time() - t0
         if i >= warmup:
             ts.append(dt)
-        if time.time() - t_begin > total_budget_s and ts:
-            break
     t_meas = float(np.mean(ts))
     scale = nfull / float(nrows)
     qps = ns / (t_meas * scale)
@@ -284,7 +298,7 @@ def flat_config(world):
     return {"workload": "GpuIndexFlatL2 N=%d d=%d nq=%d k=%d (BASELINE configs[1])" % (N_TOTAL, DIM, NQ, K),
             "N": N_TOTAL, "d": DIM, "nq": NQ, "k": K,
             "parallelism": "IndexShards x%d (contiguous row shards, all-gather top-k merge)" % world if world > 1 else "single GPU",
-            "l2_note": "inputs larger than L2 (database %.1f GB fp32 + %.1f GB fp16 copy per step vs 126 MB L2)" % (
+            "l2_note": "inputs larger than L2 (database %.1f GB fp32 + %.1f GB fp16 copy per step vs 50 MB L2)" % (
                 N_TOTAL * DIM * 4 / 1e9 / world, N_TOTAL * DIM * 2 / 1e9 / world)}
 
 
@@ -302,7 +316,7 @@ def reference_arm(args, torch):
     total = float(os.environ.get("BENCH_REF_BUDGET_S", 150.0))
     step_budget = max(1.0, total / (steps + warmup))
     if ref.available():
-        qps, info, _ = cpu_flat_reference(xb, xq, K, step_budget, steps, warmup, total * 1.5)
+        qps, info, _ = cpu_flat_reference(xb, xq, K, step_budget, steps, warmup)
     else:
         qps, info = cpu_flat_port(xb, xq, K)
     out = {"impl": "reference", "metric": METRIC, "value": qps, "unit": UNIT,
@@ -498,16 +512,8 @@ def ivfpq_workload(torch, fb, res, device, name, N, d, nlist, M, nprobe, nq, k, 
     gpu_I = I[:n_gt].cpu().numpy()
     gpu_D = D[:n_gt].cpu().numpy()
     pk, src = peaks()
-    roof = {"bound": "hbm", "unit": "GB/s", "peak": float(pk["hbm_gbs"]), "peak_source": src + " copy bandwidth (MEASURED_PEAKS.json)",
+    roof = {"bound": "hbm", "unit": "GB/s", "peak": float(pk["hbm_gbs"]), "peak_source": src + " HBM bandwidth",
             "traffic": None, "kernel": "ivfpq_scan_interleaved_kernel", "algorithmic_bytes_per_step": alg_bytes, "vectors_scanned_per_step": scanned}
-    tpath = os.path.join(ROOT, "profiles", "ivfpq_scan_traffic.json")
-    if name == "ivfpq" and N == 100_000_000 and os.path.exists(tpath):
-        try:
-            tj = json.load(open(tpath))
-            roof["traffic"] = tj["dram_bytes_per_launch"]
-            roof["traffic_source"] = tj["source"]
-        except Exception:
-            pass
     if kn.value:
         kms_step = kms.value / steps
         roof.update({"achieved": alg_bytes / (kms_step * 1e-3) / 1e9, "kernel_ms_per_step": kms_step, "kernel_share_of_step": kms_step / ms,
@@ -518,7 +524,7 @@ def ivfpq_workload(torch, fb, res, device, name, N, d, nlist, M, nprobe, nq, k, 
            "config": {"workload": "GpuIndexIVFPQ N=%d d=%d nlist=%d M=%d nbits=8 nprobe=%d nq=%d k=%d" % (N, d, nlist, M, nprobe, nq, k),
                       "data": "uniform [0,1) fp32 (seeded chunks)" if kind == "uniform" else "SyntheticDataset (contrib/datasets.py:84-105, seed 1338)",
                       "list_len_mean": float(lens.mean()), "list_len_max": int(lens.max()), "train_s": round(t_train, 2), "add_s": round(t_add, 2),
-                      "add_vec_per_s": N / t_add, "l2_note": "codes scanned per step %.1f GB vs 126 MB L2" % (alg_bytes / 1e9)},
+                      "add_vec_per_s": N / t_add, "l2_note": "codes scanned per step %.1f GB vs 50 MB L2" % (alg_bytes / 1e9)},
            "e2e": {"value": nq / (e2e_ms * 1e-3), "unit": UNIT, "ms_per_step": e2e_ms, "h2d_bytes_per_step": nq * d * 4, "d2h_bytes_per_step": nq * k * 12},
            "gpu_launches": int(launches), "roofline": roof,
            "recall": {"queries": n_gt, "ground_truth": "exact fp32 k-NN (exact SIMT Flat kernel, chunked over the database)", "gpu": _recalls(gpu_I, gt)}}
@@ -602,6 +608,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-ivfpq", action="store_true", help="skip the IVFPQ workloads (configs[3] + SyntheticDataset)")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's distances and labels as DIR/<name>.npy")
     args = ap.parse_args()
     steps, warmup = max(1, args.steps), max(0, args.warmup)
 
@@ -703,6 +710,10 @@ def main():
     sampler.mark_end()
     ms = e0.elapsed_time(e1) / steps
     launches = fb.lib.faiss_b200_launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "distances.npy"), D.cpu().numpy().astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "labels.npy"), I.cpu().numpy().astype(np.float64))  # ids < 2^53: exact
     tc_ms = ctypes.c_double()
     tc_n = ctypes.c_int()
     fb.lib.faiss_b200_kernel_timing_collect(b"flat_tc", ctypes.byref(tc_ms), ctypes.byref(tc_n))
@@ -741,19 +752,9 @@ def main():
         tc_ms_step = tc_ms.value / steps if tc_n.value else None
         peak_tf = float(pk.get("bf16_tflops_sustained", pk.get("bf16_tflops")))
         roof = {"bound": "tensor", "unit": "TFLOP/s", "peak": peak_tf, "traffic": None,
-                "peak_source": "%s bf16 GEMM peak (sustained; kernel timed inside a multi-step loop), MEASURED_PEAKS.json" % pk_src,
-                "kernel": "flat_tc_kernel (tcgen05 fp16 scoring + fused top-k filter), %d launches/step" % (tc_n.value // steps if tc_n.value else 0),
+                "peak_source": "%s bf16 GEMM peak" % pk_src,
+                "kernel": "flat_tc_kernel (wgmma fp16 scoring + fused top-k filter), %d launches/step" % (tc_n.value // steps if tc_n.value else 0),
                 "algorithmic_flops_per_step": flops_step}
-        # DRAM bytes per launch of this kernel, from the committed `ncu --set full` capture of this same
-        # workload (profiles/flat_tc_traffic.json, written by scripts/ncu_traffic.py); single GPU only
-        tpath = os.path.join(ROOT, "profiles", "flat_tc_traffic.json")
-        if world == 1 and N_TOTAL == 10_000_000 and os.path.exists(tpath):
-            try:
-                tj = json.load(open(tpath))
-                roof["traffic"] = tj["dram_bytes_per_launch"]
-                roof["traffic_source"] = tj["source"]
-            except Exception:
-                pass
         if tc_ms_step:
             roof["achieved"] = flops_step / (tc_ms_step * 1e-3) / 1e12
             roof["frac"] = roof["achieved"] / peak_tf
@@ -765,7 +766,7 @@ def main():
         out = {"metric": METRIC, "value": NQ / (ms * 1e-3), "unit": UNIT,
                "n_gpus": world, "steps": steps, "warmup": max(warmup, 3), "ms_per_step": ms, "higher_is_better": True,
                "scaling": "strong", "vs_baseline": None, "dtype": "f16 mma (fp32 accumulate) + f32 exact re-rank", "data": "synthetic",
-               "config": flat_config(world), "clocks": clocks,
+               "config": flat_config(world), "clocks": clocks, "gpu": gpu_identity(local_rank),
                "e2e": {"value": NQ / (e2e_ms * 1e-3), "unit": UNIT, "ms_per_step": e2e_ms,
                        "h2d_bytes_per_step": NQ * DIM * 4, "d2h_bytes_per_step": NQ * K * 12},
                "gpu_launches": int(launches), "roofline": roof,
@@ -790,7 +791,7 @@ def main():
 
                 xb_host = index.copyTo()
                 if ref.available():
-                    qps, cinfo, _ = cpu_flat_reference(xb_host, xq_pin.numpy(), K, step_budget_s=6.0, steps=2, warmup=1, total_budget_s=30.0)
+                    qps, cinfo, _ = cpu_flat_reference(xb_host, xq_pin.numpy(), K, step_budget_s=6.0, steps=2, warmup=1)
                 else:
                     qps, cinfo = cpu_flat_port(xb_host, xq_pin.numpy(), K)
                 del xb_host
@@ -806,14 +807,14 @@ def main():
             wl = {}
             try:
                 n_pq = int(os.environ.get("BENCH_IVFPQ_N", 100_000_000))
-                wl["ivfpq"] = ivfpq_workload(torch, fb, res, device, "ivfpq", n_pq, 128, 4096, 32, 32, NQ, K, min(steps, 10), warmup,
+                wl["ivfpq"] = ivfpq_workload(torch, fb, res, device, "ivfpq", n_pq, 128, 4096, 32, 32, NQ, K, steps, warmup,
                                              ("uniform", None), n_gt=1000, cpu_queries=1000)
             except Exception as e:
                 wl["ivfpq"] = {"error": str(e)[:300]}
             try:
                 n_syn = int(os.environ.get("BENCH_SYNTH_N", 2_000_000))
                 xt, xbs, xqs = synthetic_dataset(128, 200_000, n_syn, NQ)
-                wl["ivfpq_synthetic"] = ivfpq_workload(torch, fb, res, device, "ivfpq_synthetic", n_syn, 128, 1024, 32, 32, NQ, K, min(steps, 10), warmup,
+                wl["ivfpq_synthetic"] = ivfpq_workload(torch, fb, res, device, "ivfpq_synthetic", n_syn, 128, 1024, 32, 32, NQ, K, steps, warmup,
                                                        ("arrays", (xt, xbs, xqs)), n_gt=1000, cpu_queries=1000)
             except Exception as e:
                 wl["ivfpq_synthetic"] = {"error": str(e)[:300]}

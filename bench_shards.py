@@ -6,7 +6,7 @@ one node (IndexShards semantics), coarse quantiser trained by sharded k-means.
       bench_shards.py --gpus N [--ntotal 1000000000 --d 96 --nlist 65536 --m 32 --nprobe 32]
 
 One process per GPU.  Per rank: its contiguous slice of the database and of the training set.
-  * train: `faiss_b200.kmeans_sharded` (C++, faiss_b200_kmeans_sharded) -- Flat k=1 assignment on the tcgen05
+  * train: `faiss_b200.kmeans_sharded` (C++, faiss_b200_kmeans_sharded) -- Flat k=1 assignment on the wgmma
     streaming path against the replicated centroid table, deterministic local partial sums, ONE packed NCCL
     all-reduce per iteration (k*d sums | k counts | objective); PQ codebooks trained on rank 0's residuals and broadcast.
   * add: device-side assign -> residual -> PQ encode -> append, shard-local ids.
@@ -106,7 +106,7 @@ def main():
     torch.cuda.synchronize()
     dist.barrier()
     tt = time.time()
-    # C++ sharded k-means behind the C ABI: local tcgen05 k=1 assignment (streaming mode), deterministic local
+    # C++ sharded k-means behind the C ABI: local wgmma k=1 assignment (streaming mode), deterministic local
     # partial sums, ONE packed ncclAllReduce per iteration on the library's own communicator
     cent_np, objs, kstats = fb.kmeans_sharded(res, xt, nlist, niter=args.niter, seed=1234, device=local_rank)
     cent = torch.from_numpy(cent_np).to(dev)

@@ -1,4 +1,4 @@
-"""faiss_b200 -- B200-native (sm_100a) similarity search behind the Faiss GPU plugin surface.
+"""faiss_b200 -- H100-native (sm_90a) similarity search behind the Faiss GPU plugin surface.
 
 Python mirror of the reference's index classes over the C ABI of ``libfaiss_b200.so``
 (``include/faiss_b200_c.h``).  Same class / method names and argument meaning as
@@ -812,7 +812,7 @@ def topk_merge(res, D_in, I_in, k, metric=METRIC_L2, id_offsets=None, device=0):
 
 
 def flat_tc_scores_debug(res, Q16, Y16, device=0):
-    """Raw tcgen05 fp16 score matrix [nq, roundup(N,128)] (unit-test seam)."""
+    """Raw tensor-core fp16 score matrix [nq, roundup(N,256)] (unit-test seam)."""
     import torch
 
     nq, dpad = Q16.shape

@@ -226,7 +226,7 @@ faiss::Index* index_cpu_to_b200(B200Resources* res, int device, const faiss::Ind
         return new B200IndexIVFPQ(res, pq, device);
     if (auto* fl = dynamic_cast<const faiss::IndexIVFFlat*>(index))
         return new B200IndexIVFFlat(res, fl, device);
-    FAISS_THROW_MSG("index_cpu_to_b200: this type of index is not on the B200 path (Flat, IVFFlat, IVFPQ are)");
+    FAISS_THROW_MSG("index_cpu_to_b200: this type of index is not on the faiss_b200 path (Flat, IVFFlat, IVFPQ are)");
 }
 
 faiss::Index* index_b200_to_cpu(const faiss::Index* index) {

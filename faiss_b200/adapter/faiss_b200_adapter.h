@@ -3,7 +3,7 @@
 // Each class derives from faiss::Index (faiss/Index.h:101-435) and forwards to the C ABI of libfaiss_b200.so
 // (include/faiss_b200_c.h), so everything in Faiss that drives a `faiss::Index&` -- faiss::Clustering::train
 // (faiss/Clustering.cpp:254-356), faiss::IndexShards / ThreadedIndex (faiss/IndexShards.cpp:197-264),
-// ProductQuantizer::assign_index, IndexIVF's quantizer slot -- runs on the B200 kernels without a change at
+// ProductQuantizer::assign_index, IndexIVF's quantizer slot -- runs on the faiss_b200 kernels without a change at
 // the call site.  index_cpu_to_b200 / index_b200_to_cpu are the cloner pair of faiss/gpu/GpuCloner.cpp:124-255
 // (copyFrom / copyTo of GpuIndexFlat.cu:105-176, GpuIndexIVFFlat.cu:89-150, GpuIndexIVFPQ.cu:105-217; inverted
 // lists are moved in the CPU ArrayInvertedLists byte format, so copyTo(copyFrom(x)) is byte-identical).

@@ -1,6 +1,6 @@
-"""Build libfaiss_b200.so in-tree with nvcc for sm_100a (no JIT cache, no torch extension).
+"""Build libfaiss_b200.so in-tree with nvcc for sm_90a (no JIT cache, no torch extension).
 
-Usage: python -m faiss_b200.build [-j N] [--force]
+Usage: python faiss_b200/build.py [-j N] [--force]
 Objects go to faiss_b200/csrc/_obj/, the library to faiss_b200/libfaiss_b200.so.
 """
 import os
@@ -15,7 +15,7 @@ LIB = os.path.join(HERE, "libfaiss_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "--expt-relaxed-constexpr", "-I" + os.path.join(HERE, "..", "include"), "-I" + SRC,
 ]
@@ -62,7 +62,7 @@ def build(jobs=None, force=False, verbose=True):
 
     if todo:
         if verbose:
-            print("[faiss_b200.build] compiling %d file(s) for sm_100a" % len(todo), flush=True)
+            print("[faiss_b200.build] compiling %d file(s) for sm_90a" % len(todo), flush=True)
         with ThreadPoolExecutor(max_workers=jobs or min(8, os.cpu_count() or 4)) as ex:
             list(ex.map(cc, todo))
     if todo or not os.path.exists(LIB):

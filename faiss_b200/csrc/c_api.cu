@@ -64,7 +64,7 @@ const char* faiss_get_last_error(void) {
     return g_last_error.c_str();
 }
 const char* faiss_b200_version(void) {
-    return "faiss_b200 0.1 (sm_100a)";
+    return "faiss_b200 0.1 (sm_90a)";
 }
 
 // ---------------------------------------------------------------- resources

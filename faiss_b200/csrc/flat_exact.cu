@@ -4,7 +4,7 @@
 // cuBLAS SGEMM -> materialised fp32 tile in HBM -> l2SelectMinK -> second-level blockSelect.
 // Here one kernel computes a [TQ x TN] distance tile in registers and feeds it straight into
 // per-query shared-memory top-k lists (select.cuh); distances never reach HBM.  A database split
-// (gridDim.y) fills the 148 SMs when nq is small; partial lists are merged by runMergeTopK.
+// (gridDim.y) fills the 132 SMs when nq is small; partial lists are merged by runMergeTopK.
 //
 // Arithmetic: direct form, accumulated strictly in dimension order with FMA:
 //   L2: acc = fma(q_i - y_i, q_i - y_i, acc)     IP: acc = fma(q_i, y_i, acc)

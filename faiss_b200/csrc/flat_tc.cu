@@ -1,4 +1,4 @@
-// faiss_b200 -- Flat L2/IP k-NN on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), sm_100a only.
+// faiss_b200 -- Flat L2/IP k-NN on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 // Replaces, for the Flat path, the reference chain
 //   runDistance<float> (faiss/gpu/impl/Distance.cu:121-405) = cuBLAS SGEMM -> fp32 tile in HBM ->
@@ -6,15 +6,15 @@
 //
 // Design (see DESIGN.md "Flat"):
 //   * Scoring.  score(q,y) = q.y - ||y||^2/2 (L2; maximise) or q.y (IP).  q and y are rounded to
-//     fp16 after a power-of-two scaling; the dot product runs on tcgen05.mma (kind::f16, fp32
-//     accumulate in TMEM).  |approx - exact| <= eps_q, a rigorous bound from the fp16 rounding
+//     fp16 after a power-of-two scaling; the dot product runs on wgmma.mma_async (fp16 inputs,
+//     fp32 accumulate in registers).  |approx - exact| <= eps_q, a rigorous bound from the fp16 rounding
 //     model (10 mantissa bits) and the fp32 accumulation.
-//   * Fused filter (flat_tc_kernel.cuh).  A persistent warp-specialised kernel: warp 0 = TMA producer
-//     (two query tiles once per work unit, 256-row database tiles through an mbarrier ring), warp 1 =
-//     single-thread MMA issuer (128x256xK tiles, two TMEM accumulators = the unit's two query tiles),
-//     16 epilogue warps: each thread owns ONE query row (a TMEM lane) and 64 of a tile's 256 columns,
-//     pulls 32 columns at a time with tcgen05.ld, folds the RAW accumulators with an FMNMX3 tree and
-//     compares one bound per chunk against the query's threshold held in a register -- the fp16 copy
+//   * Fused filter (flat_tc_kernel.cuh).  A persistent warp-specialised kernel: one TMA producer warp
+//     (the unit's 128-query tile once per work unit, 256-row database tiles through an mbarrier ring) and
+//     two consumer warpgroups that each run 64x256xK wgmma tiles into register accumulators and filter
+//     them in place: each thread holds two query rows and 64 of a tile's 256 columns of each, folds the
+//     RAW accumulators with a max tree and compares one bound per 32 of them against the query's
+//     threshold held in a register -- the fp16 copy
 //     is stored sorted by norm, so the tile's maximum bias bounds every row's bias tightly.  Scores
 //     never reach HBM; only the rare survivors are appended (plain stores, no atomics) to a
 //     thread-private candidate segment.
@@ -196,7 +196,7 @@ __global__ void tc_prepare_queries_kernel(
     if (lane_id() == 0) {
         float qn = sqrtf(acc) * 1.0001f;
         // |approx score - score implied by the exact kernel's fp32 distance| <= c1*|q||y| + c2*(|q|+|y|)^2
-        // (see DESIGN.md, error model): c1 = fp16 input rounding + TMEM accumulation of q.y, c2 = fp32
+        // (see DESIGN.md, error model): c1 = fp16 input rounding + fp32 accumulation of q.y, c2 = fp32
         // rounding of the bias (norms), of the final FMA and of the exact kernel's own sum (d terms)
         const float qy = qn + yMaxNorm;
         eps[row] = c1 * qn * yMaxNorm + c2 * qy * qy;
@@ -252,8 +252,8 @@ __global__ void tc_select_kernel(
     __syncwarp();
     w.thr = w.q.threshold();
     int overflow = 0;
-    const int pair = q / kPairM, prow = q % kPairM; // row within the unit's 256 query rows
-    const int qPairs = (nq + kPairM - 1) / kPairM;
+    const int pair = q / kUnitM, prow = q % kUnitM; // row within the unit's 128 query rows
+    const int qPairs = (nq + kUnitM - 1) / kUnitM;
     // segment counts are fetched 32 at a time (one per lane): the loop over a query's slices x parts
     // segments would otherwise serialise one L2 round trip per segment, and most segments are empty
     const int nseg = slices * parts;
@@ -263,7 +263,7 @@ __global__ void tc_select_kernel(
         int myCount = 0;
         if (si < nseg) {
             const int s = si / parts, h = si - s * parts;
-            mySeg = ((long long)(s * qPairs + pair) * kPairM + prow) * parts + h;
+            mySeg = ((long long)(s * qPairs + pair) * kUnitM + prow) * parts + h;
             myCount = candCount[mySeg];
         }
         unsigned pending = __ballot_sync(kFullMask, myCount > 0);
@@ -388,8 +388,8 @@ __global__ void __launch_bounds__(kSelWarps * 32) tc_select_bisect_kernel(
     // (2) this round's candidates.  32 segments at a time: a warp scan of their counts gives every lane the offset
     // of ITS segment, then the lanes copy their segments in parallel (one memory round trip per batch of 32
     // segments instead of one per segment -- the gather is latency-bound, not bandwidth-bound).
-    const int pair = q / kPairM, prow = q % kPairM;
-    const int qPairs = (nq + kPairM - 1) / kPairM;
+    const int pair = q / kUnitM, prow = q % kUnitM;
+    const int qPairs = (nq + kUnitM - 1) / kUnitM;
     const int nseg = slices * parts;
     for (int s0 = 0; s0 < nseg; s0 += 32) {
         const int si = s0 + lane;
@@ -397,7 +397,7 @@ __global__ void __launch_bounds__(kSelWarps * 32) tc_select_bisect_kernel(
         int myCount = 0;
         if (si < nseg) {
             const int s = si / parts, h = si - s * parts;
-            mySeg = ((long long)(s * qPairs + pair) * kPairM + prow) * parts + h;
+            mySeg = ((long long)(s * qPairs + pair) * kUnitM + prow) * parts + h;
             myCount = candCount[mySeg];
             if (myCount > cap) {
                 overflow = 1;
@@ -635,15 +635,15 @@ __global__ void tc_argmin_finish_kernel(
     const int q = blockIdx.x * (blockDim.x >> 5) + warp;
     if (q >= nq)
         return;
-    const int pair = q / kPairM, prow = q % kPairM;
-    const int qPairs = (nq + kPairM - 1) / kPairM;
+    const int pair = q / kUnitM, prow = q % kUnitM;
+    const int qPairs = (nq + kUnitM - 1) / kUnitM;
     const int nseg = slices * parts;
     // pass 1: maximum approximate score
     float m = -CUDART_INF_F;
     int overflow = 0;
     for (int si = 0; si < nseg; si++) {
         const int s = si / parts, h = si - s * parts;
-        const long long seg = ((long long)(s * qPairs + pair) * kPairM + prow) * parts + h;
+        const long long seg = ((long long)(s * qPairs + pair) * kUnitM + prow) * parts + h;
         int c = candCount[seg];
         if (c > cap) {
             overflow = 1;
@@ -663,7 +663,7 @@ __global__ void tc_argmin_finish_kernel(
     const float* qp = Q + (int64_t)q * d;
     for (int si = 0; si < nseg; si++) {
         const int s = si / parts, h = si - s * parts;
-        const long long seg = ((long long)(s * qPairs + pair) * kPairM + prow) * parts + h;
+        const long long seg = ((long long)(s * qPairs + pair) * kUnitM + prow) * parts + h;
         const int c = min(candCount[seg], cap);
         const uint2* sp = cand + seg * cap;
         for (int e0 = 0; e0 < c; e0 += 32) {
@@ -812,43 +812,29 @@ struct SmemPlan {
     int ksplit; // ring stages hold single K-blocks (see flat_tc_kernel)
 };
 
-constexpr int kMaxKB = 4; // d <= 256: two query tiles (32 KB per K-block) + at least three 32 KB K-block stages in 227 KB
+constexpr int kMaxKB = 4; // d <= 256: the query tile (16 KB per K-block) + at least three 32 KB K-block stages in 227 KB
 
+// d <= 128: whole-tile stages (64 KB at d = 128: three of them); beyond, K-block stages (see flat_tc_kernel)
 SmemPlan planSmem(int KB) {
-    const size_t qtiles = (size_t)2 * KB * kTileM * kKBlock * 2;
-    const size_t fixed = 1024 /*align slack*/ + 512 /*barriers*/ + qtiles;
-    if (KB <= 2) {
-        const size_t stage = (size_t)KB * kTileN * kKBlock * 2;
-        const size_t budget = 220 * 1024;
-        int ys = (int)std::min<size_t>(kMaxYStages, (budget - fixed) / stage);
-        return {ys, fixed + ys * stage, 0};
-    }
     FB_THROW_IF_NOT_MSG(KB <= kMaxKB, "dimension too large for the tensor-core Flat kernel");
-    const size_t stage = (size_t)kTileN * kKBlock * 2;
+    const int ksplit = KB > 2 ? 1 : 0;
+    const size_t qtile = (size_t)KB * kTileM * kKBlock * 2;
+    const size_t fixed = 1024 /*align slack*/ + 512 /*barriers*/ + qtile;
+    const size_t stage = (size_t)(ksplit ? 1 : KB) * kTileN * kKBlock * 2;
     const size_t budget = 226 * 1024; // 232448 B is the opt-in limit per CTA
     int ys = (int)std::min<size_t>(kMaxYStages, (budget - fixed) / stage);
     FB_THROW_IF_NOT(ys >= 3);
-    return {ys, fixed + ys * stage, 1};
-}
-
-// column parts per tile = epilogue warps / 4 (FB200_TC_PARTS: tuning knob, 2 or 4)
-int tcParts() {
-    static const int parts = getenv("FB200_TC_PARTS") ? atoi(getenv("FB200_TC_PARTS")) : 4;
-    return parts == 2 ? 2 : 4;
+    return {ys, fixed + ys * stage, ksplit};
 }
 
 template <bool DUMP>
 void launchTc(const CUtensorMap& mq, const CUtensorMap& my, const TcParams& p, int grid, size_t smem, cudaStream_t stream, bool self = false) {
-    // FB200_TC_DEBUG_SKIP=1 (timing experiments only): skip the filter, keep the TMEM loads
-    static const bool dbg = getenv("FB200_TC_DEBUG_SKIP") && atoi(getenv("FB200_TC_DEBUG_SKIP")) != 0;
-    const int parts = tcParts();
-    auto kern = parts == 2 ? (dbg ? flat_tc_kernel<DUMP, 1, 2> : flat_tc_kernel<DUMP, 0, 2>)
-                           : (dbg ? flat_tc_kernel<DUMP, 1, 4> : flat_tc_kernel<DUMP, 0, 4>);
+    auto kern = flat_tc_kernel<DUMP>;
     if (self && !DUMP) // k = 1 streaming mode (self-tightening thresholds)
-        kern = parts == 2 ? flat_tc_kernel<false, 0, 2, true> : flat_tc_kernel<false, 0, 4, true>;
+        kern = flat_tc_kernel<false, true>;
     CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTiming::begin("flat_tc", stream);
-    kern<<<grid, tcThreads(parts), smem, stream>>>(mq, my, p);
+    kern<<<grid, kTcThreads, smem, stream>>>(mq, my, p);
     KernelTiming::end("flat_tc", stream);
     CUDA_CHECK_LAST();
 }
@@ -935,11 +921,11 @@ void runFlatTcScoresDebug(
     SmemPlan sp = planSmem(KB);
     CUtensorMap my = makeTileMap(Y16, n, dpad, kTileN, sp.ksplit);
     const int64_t numTiles = ceil_div(n, kTileN);
-    const int64_t qPairs = ceil_div(nq, kPairM);
-    // the kernel reads whole 256-row query pairs: zero-padded private copy
+    const int64_t qPairs = ceil_div(nq, kUnitM);
+    // the kernel reads whole 128-row query tiles: zero-padded private copy
     __half* qpad = nullptr;
-    CUDA_VERIFY(cudaMallocAsync(&qpad, sizeof(__half) * qPairs * kPairM * dpad, stream));
-    CUDA_VERIFY(cudaMemsetAsync(qpad, 0, sizeof(__half) * qPairs * kPairM * dpad, stream));
+    CUDA_VERIFY(cudaMallocAsync(&qpad, sizeof(__half) * qPairs * kUnitM * dpad, stream));
+    CUDA_VERIFY(cudaMemsetAsync(qpad, 0, sizeof(__half) * qPairs * kUnitM * dpad, stream));
     CUDA_VERIFY(cudaMemcpyAsync(qpad, Q16, sizeof(__half) * nq * dpad, cudaMemcpyDeviceToDevice, stream));
     // scale (1.0) for the debug run; the dump path never reads biases
     float* one = nullptr;
@@ -950,7 +936,7 @@ void runFlatTcScoresDebug(
     p.slices = 1;
     p.qPairs = (int)qPairs;
     p.numUnits = (int)qPairs;
-    CUtensorMap mq = makeTileMap(qpad, qPairs * kPairM, dpad, kTileM);
+    CUtensorMap mq = makeTileMap(qpad, qPairs * kUnitM, dpad, kTileM);
     p.tileBegin = 0;
     p.tileEnd = (int)numTiles;
     p.tilesPerSlice = (int)numTiles;
@@ -1046,23 +1032,23 @@ void runFlatTcSearch(
     if (useBisect)
         r0Tiles = std::min(r0Tiles, std::max(2, kSelCap * 3 / 4 / kTileN));
     // queries per pass: bounds the candidate arena, whose largest user is the all-pass round 0
-    // (512 KB per query pair and tile) -- 16384 queries at k = 100, up to 131072 for small k
+    // (2 KB per query and tile) -- 16384 queries at k = 100, up to 131072 for small k
     // k = 1 (k-means assignment, the coarse quantiser of an add): streaming mode -- one pass over all tiles with
     // self-tightening per-thread thresholds (flat_tc_kernel SELF) and a fused select + exact re-rank
     // (tc_argmin_finish_kernel); no rounds, no all-pass first round, no per-query sorted lists.
     static const bool noStream = getenv("FB200_TC_NO_STREAM") && atoi(getenv("FB200_TC_NO_STREAM")) != 0;
     const bool streaming = k == 1 && !shard && !noStream;
-    // streaming: a batch is a whole number of waves of the persistent grid (one 256-query unit per CTA and wave)
+    // streaming: a batch is a whole number of waves of the persistent grid (one 128-query unit per CTA and wave)
     // (large k: the all-pass round covers 40 k rows, so the floor drops to keep the arena near 1 GiB)
     const int64_t kQFloor = r0Tiles > 64 ? 2048 : 16384;
-    const int64_t kQBatch = streaming ? (int64_t)sms * kPairM * 4
-                                      : std::min<int64_t>(131072, std::max<int64_t>(kQFloor, (int64_t)kPairM * 1024 / r0Tiles));
+    const int64_t kQBatch = streaming ? (int64_t)sms * kUnitM * 4
+                                      : std::min<int64_t>(131072, std::max<int64_t>(kQFloor, (int64_t)262144 / r0Tiles));
     for (int64_t qb = 0; qb < nqAll; qb += kQBatch) {
         const int64_t nq = std::min(kQBatch, nqAll - qb);
         const float* Qb = Q + qb * d;
-        const int64_t qPairs = ceil_div(nq, kPairM);
+        const int64_t qPairs = ceil_div(nq, kUnitM);
 
-        auto q16 = res->temp(device, sizeof(__half) * qPairs * kPairM * dpad);
+        auto q16 = res->temp(device, sizeof(__half) * qPairs * kUnitM * dpad);
         auto scal = res->temp(device, sizeof(float) * 4); // [absmax, qScale, inv, -]
         auto eps = res->temp(device, sizeof(float) * nq);
         auto thr = res->temp(device, sizeof(float) * nq);
@@ -1072,7 +1058,7 @@ void runFlatTcSearch(
 
         CUDA_VERIFY(cudaMemsetAsync(scal.data, 0, sizeof(float) * 4, stream));
         CUDA_VERIFY(cudaMemsetAsync(flags.data, 0, sizeof(int) * (nq + 1), stream));
-        CUDA_VERIFY(cudaMemsetAsync(q16.data, 0, sizeof(__half) * qPairs * kPairM * dpad, stream));
+        CUDA_VERIFY(cudaMemsetAsync(q16.data, 0, sizeof(__half) * qPairs * kUnitM * dpad, stream));
         float* sc = scal.as<float>();
         runAbsMax(Qb, nq * d, sc + 0, stream);
         tc_query_scale_kernel<<<1, 1, 0, stream>>>(sc + 0, yScale, sc + 1, sc + 2);
@@ -1091,7 +1077,7 @@ void runFlatTcSearch(
         struct Round {
             int begin, end, slices, tilesPerSlice, cap;
         };
-        const int parts = tcParts();
+        const int parts = kParts;
         std::vector<Round> rounds;
         {
             int64_t seen = 0;
@@ -1143,8 +1129,8 @@ void runFlatTcSearch(
         size_t arenaBytes = 0, countBytes = 0;
         for (auto& r : rounds) {
             size_t units = (size_t)qPairs * r.slices;
-            arenaBytes = std::max(arenaBytes, units * tcSegsPerUnit(parts) * (size_t)r.cap * sizeof(uint2));
-            countBytes = std::max(countBytes, units * tcSegsPerUnit(parts) * sizeof(int));
+            arenaBytes = std::max(arenaBytes, units * kSegsPerUnit * (size_t)r.cap * sizeof(uint2));
+            countBytes = std::max(countBytes, units * kSegsPerUnit * sizeof(int));
         }
         auto arena = res->temp(device, arenaBytes);
         auto counts = res->temp(device, countBytes);
@@ -1161,7 +1147,7 @@ void runFlatTcSearch(
             p.slices = r.slices;
             p.qPairs = (int)qPairs;
             p.numUnits = (int)(qPairs * r.slices);
-            CUtensorMap mapQ = makeTileMap(q16.as<__half>(), qPairs * kPairM, dpad, kTileM);
+            CUtensorMap mapQ = makeTileMap(q16.as<__half>(), qPairs * kUnitM, dpad, kTileM);
             p.tileBegin = (int)std::min<int64_t>(r.begin, T); // schedule laid out over the largest shard: clamp to ours
             p.tileEnd = (int)std::min<int64_t>(r.end, T);
             p.tilesPerSlice = r.tilesPerSlice;
@@ -1187,7 +1173,7 @@ void runFlatTcSearch(
             if (p.tileBegin < p.tileEnd) {
                 launchTc<false>(mapQ, mapY, p, std::min(p.numUnits, sms), sp.bytes, stream, streaming);
             } else { // this shard has no tiles in this round of the common schedule: no candidates
-                CUDA_VERIFY(cudaMemsetAsync(counts.data, 0, (size_t)p.numUnits * tcSegsPerUnit(parts) * sizeof(int), stream));
+                CUDA_VERIFY(cudaMemsetAsync(counts.data, 0, (size_t)p.numUnits * kSegsPerUnit * sizeof(int), stream));
             }
             if (streaming) { // select + exact re-rank fused: one warp per query
                 const int fw = 8;
@@ -1249,8 +1235,6 @@ void runFlatTcSearch(
 
         // ---- exact re-rank
         if (!streaming) {
-            // (staging the 32 candidate rows of a step through shared memory with coalesced loads was
-            // measured slower on B200: 0.91 ms vs 0.72 ms per 10k queries -- the per-lane row walk wins)
             const int rrWarps = (int)std::max<size_t>(1, std::min<size_t>(8, (48 * 1024) / SmemTopK<int>::bytes(KL, 64)));
             const size_t rrSmem = SmemTopK<int>::bytes(KL, 64) * rrWarps;
             float* oD = outD + qb * k;

@@ -1,23 +1,20 @@
-// faiss_b200 -- the tcgen05 Flat scoring + filter kernel (included by flat_tc.cu).
+// faiss_b200 -- the wgmma Flat scoring + filter kernel (included by flat_tc.cu).
 //
-// Shape decisions, each backed by a measurement on B200 (profiles/r01_ubench_tcgen05.txt):
-//   * tcgen05.commit costs MMA throughput: 128x128x16 MMAs with a commit every 8 instructions run
-//     at ~0.95 PFLOP/s, 128x256x16 at ~1.46 (SS) -- so the database tile is N = 256 rows and one
-//     commit pair covers 1024 cycles of tensor work.
-//   * L2 -> SM bandwidth (~8 TB/s chip-wide) caps a one-query-tile CTA at ~1.1 PFLOP/s for d = 128:
-//     a work unit therefore covers TWO query tiles (256 queries); every database tile that lands in
-//     shared memory feeds two MMA groups (accumulators h = 0, 1 -> the two 256-column halves of TMEM).
-//   * tcgen05.ld is not a limit (~770 B/cycle/SM measured), so fp32 accumulators are drained in full.
+// Roles in one persistent CTA (2 consumer warpgroups + 1 producer warp = 288 threads, one CTA per SM):
+//   warps 0-7 : two consumer warpgroups.  A work unit is one 128-query tile; warpgroup g owns its query rows
+//               64 g .. 64 g + 63.  For every database tile it issues wgmma.m64n256k16 (fp16 operands straight
+//               from the 128B-swizzled shared-memory stages, fp32 accumulators in registers: 128 per thread),
+//               waits for them, hands the stage back and filters its own accumulator fragment (below).  A
+//               warpgroup's own MMAs and filter do not overlap; the two warpgroups share the ring without
+//               synchronising with each other, so one's tensor work can overlap the other's filter.  Survivors (rare) are appended with plain stores to a thread-private candidate segment;
+//               scores never reach HBM.
+//   warp 8    : TMA producer -- the unit's query tile once, then database tiles (256 rows x dpad fp16,
+//               128B-swizzled K-major) through an mbarrier ring.
+// Nine warps put three on one scheduler, which caps a thread at 168 registers: the 128 accumulators plus the filter
+// state fit without spills.
 //
-// Roles in one persistent CTA (64 + 128 * PARTS threads, one CTA per SM):
-//   warp 0   : TMA producer -- the unit's two query tiles once, then database tiles (256 rows x dpad
-//              fp16, 128B-swizzled K-major) through an mbarrier ring
-//   warp 1   : single-thread tcgen05.mma issuer (SS mode, M=128 N=256 K=16, fp32 accumulate in TMEM)
-//   warps 2+ : epilogue, 4 * PARTS warps.  A thread owns one TMEM lane = one query row of each of the
-//              unit's two query tiles, and 256 / PARTS of a tile's columns.  It drains its slice of an
-//              accumulator with tcgen05.ld (32 or 64 columns at a time), hands the accumulator back to
-//              the MMA warp after its last load, and filters (below).  Survivors (rare) are
-//              appended with plain stores to a thread-private candidate segment; scores never reach HBM.
+// A thread's fragment holds two query rows (r and r + 8) and, of each, the 64 columns 8 j + 2 (lane % 4) + {0, 1}:
+// the four lanes of a quad split a row's 256 columns, which is why a query row has kParts = 4 candidate segments.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -28,28 +25,21 @@
 namespace fb200 {
 namespace tc {
 
-constexpr int kTileM = 128;       // queries per MMA tile (TMEM lanes)
-constexpr int kPairM = 256;       // queries per work unit (two MMA tiles)
-constexpr int kTileN = 256;       // database rows per tile (TMEM columns per accumulator)
+constexpr int kTileM = 128;       // queries per work unit (the query tile)
+constexpr int kUnitM = kTileM;
+constexpr int kWgM = 64;          // query rows per consumer warpgroup (wgmma M)
+constexpr int kTileN = 256;       // database rows per tile (wgmma N)
 constexpr int kKBlock = 64;       // fp16 elements per 128-byte swizzle row
-// PARTS = column parts of a tile filtered by different warps: 4 * PARTS epilogue warps (a warp may only
-// touch its own TMEM lane quarter), 64 + 128 * PARTS threads per CTA.  With PARTS = 4 two schedulers
-// hold 5 warps, which caps a thread at 96 registers: the filter then works on 32-column chunks.
-// (Measured on B200, N=10M d=128 nq=10k: PARTS=2 / 64-column blocks 23.6 ms per step in this kernel,
-// PARTS=4 / 32-column chunks 20.9 ms, PARTS=4 / 64-column blocks with setmaxnreg 112 registers 23.2 ms.)
-constexpr int kMaxParts = 4;
+constexpr int kParts = 4;         // column parts of a tile per query row (lanes of a quad)
+constexpr int kConsumerWarps = 8; // two warpgroups
+constexpr int kTcThreads = 32 * kConsumerWarps + 32;
 constexpr int kMaxYStages = 6;
-__host__ __device__ constexpr int tcThreads(int parts) {
-    return 64 + 128 * parts; // TMA warp, MMA warp, 4 * parts epilogue warps
-}
-__host__ __device__ constexpr int tcSegsPerUnit(int parts) {
-    return kPairM * parts; // 256 query rows x column parts
-}
+constexpr int kSegsPerUnit = kUnitM * kParts;
 
 struct TcParams {
     int numUnits;
     int slices;
-    int qPairs;         // unit u = slice * qPairs + pair: neighbouring CTAs stream the SAME database tiles (L2 reuse)
+    int qPairs;         // number of query units; unit u = slice * qPairs + qunit: neighbouring CTAs stream the SAME database tiles (L2 reuse)
     int tileBegin;      // permuted position range of this round
     int tileEnd;
     int tilesPerSlice;
@@ -76,20 +66,25 @@ __device__ __forceinline__ int perm_tile(const TcParams& p, int pos) {
     return (int)(((unsigned long long)pos * p.permA + p.permB) % p.numTiles);
 }
 
-// Filter of one query row against a run of columns (database rows).
+// column of element e of a 32-element chunk, relative to the chunk's first column (fragment layout above)
+__device__ __forceinline__ int chunk_col(int e) {
+    return 8 * (e >> 1) + (e & 1);
+}
+
+// Filter of one query row against 32 of its columns (database rows).
 //
 // The exact test is  score = fma(acc, inv, bias[row]) > thr.  The database tiles hold rows SORTED BY
 // NORM, so the biases of a tile are nearly equal and  bound = fma(max acc, inv, max bias of the tile)
 // is a tight upper bound of every score in a group (inv > 0 and rounding are monotonic: no false
-// negatives, bit for bit).  The fast path is therefore a pure FMNMX3 tree over raw accumulators --
+// negatives, bit for bit).  The fast path is therefore a pure max tree over raw accumulators --
 // no bias loads, no per-element FMA -- plus one FMA per 32 columns; the rare group whose bound beats
 // the threshold evaluates the exact test with biases read through L1/L2.
 template <bool DUMP, bool SELF>
 __device__ __forceinline__ void epi_filter32(
         const TcParams& p,
-        const uint32_t (&r)[32],
+        const float (&r)[32],
         int q,
-        long long colBase, // global (sorted) row index of column 0 of this chunk
+        long long colBase, // global (sorted) row index of element 0 of this chunk
         float inv,
         float& thr,  // SELF: tightened in place (running maximum minus the slack)
         float slack, // SELF: 2 * eps of this query
@@ -102,7 +97,7 @@ __device__ __forceinline__ void epi_filter32(
             float* dst = p.dump + (long long)q * p.dumpLd + colBase;
 #pragma unroll
             for (int j = 0; j < 32; j++)
-                dst[j] = __uint_as_float(r[j]);
+                dst[chunk_col(j)] = r[j];
         }
         return;
     }
@@ -110,11 +105,11 @@ __device__ __forceinline__ void epi_filter32(
 #pragma unroll
     for (int g = 0; g < 4; g++) {
         const int o = 8 * g;
-        const float a = ptx::max3(__uint_as_float(r[o + 0]), __uint_as_float(r[o + 1]), __uint_as_float(r[o + 2]));
-        const float c = ptx::max3(__uint_as_float(r[o + 3]), __uint_as_float(r[o + 4]), __uint_as_float(r[o + 5]));
-        mg[g] = ptx::max3(a, c, fmaxf(__uint_as_float(r[o + 6]), __uint_as_float(r[o + 7])));
+        const float a = fmaxf(fmaxf(r[o + 0], r[o + 1]), fmaxf(r[o + 2], r[o + 3]));
+        const float c = fmaxf(fmaxf(r[o + 4], r[o + 5]), fmaxf(r[o + 6], r[o + 7]));
+        mg[g] = fmaxf(a, c);
     }
-    const float m = ptx::max3(mg[0], mg[1], fmaxf(mg[2], mg[3]));
+    const float m = fmaxf(fmaxf(mg[0], mg[1]), fmaxf(mg[2], mg[3]));
     if (SELF) {
         // the chunk's best row scores at least fma(m, inv, min bias of the tile) (monotone rounding, bias >= minb):
         // the running "best - 2 eps" threshold can be raised BEFORE any per-element work, so the slow path below
@@ -129,10 +124,10 @@ __device__ __forceinline__ void epi_filter32(
             if (fmaf(mg[g], inv, maxb) > thr) {
 #pragma unroll
                 for (int j = 8 * g; j < 8 * g + 8; j++) {
-                    const float v = fmaf(__uint_as_float(r[j]), inv, __ldg(bias + j));
+                    const float v = fmaf(r[j], inv, __ldg(bias + chunk_col(j)));
                     if (v > thr) {
                         if (cnt < p.cap)
-                            buf[cnt] = make_uint2(__float_as_uint(v), rowBase + j);
+                            buf[cnt] = make_uint2(__float_as_uint(v), rowBase + chunk_col(j));
                         cnt++;
                         if (SELF) // k = 1: nothing scoring <= v - 2 eps can be the exact argmin any more
                             thr = fmaxf(thr, nextafterf(v - slack, -CUDART_INF_F));
@@ -143,31 +138,11 @@ __device__ __forceinline__ void epi_filter32(
     }
 }
 
-// 64 columns (two 32-column register sets) in one go: more independent work per warp for the
-// two-warps-per-scheduler configuration (PARTS = 2).
-template <bool DUMP, bool SELF>
-__device__ __forceinline__ void epi_filter64(
-        const TcParams& p,
-        const uint32_t (&r0)[32],
-        const uint32_t (&r1)[32],
-        int q,
-        long long colBase,
-        float inv,
-        float& thr,
-        float slack,
-        float maxb,
-        uint2* buf,
-        int& cnt,
-        float minb = 0.f) {
-    epi_filter32<DUMP, SELF>(p, r0, q, colBase, inv, thr, slack, maxb, buf, cnt, minb);
-    epi_filter32<DUMP, SELF>(p, r1, q, colBase + 32, inv, thr, slack, maxb, buf, cnt, minb);
-}
-
-// SELF (k = 1 streaming mode, used for k-means assignment): one pass over all tiles, every epilogue thread keeps
+// SELF (k = 1 streaming mode, used for k-means assignment): one pass over all tiles, every consumer thread keeps
 // a running "best approximate score minus 2 eps" threshold for its two queries and emits only the candidates
 // that beat it -- about ln(columns per thread) plus the near-ties of the maximum.
-template <bool DUMP, int DBG, int PARTS, bool SELF = false>
-__global__ void __launch_bounds__(tcThreads(PARTS), 1) flat_tc_kernel(
+template <bool DUMP, bool SELF = false>
+__global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
         const __grid_constant__ CUtensorMap mapQ,
         const __grid_constant__ CUtensorMap mapY,
         const TcParams p) {
@@ -175,73 +150,58 @@ __global__ void __launch_bounds__(tcThreads(PARTS), 1) flat_tc_kernel(
     // 1024-byte aligned carve-up (SWIZZLE_128B atoms need it)
     unsigned char* smem = reinterpret_cast<unsigned char*>(
             (reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
-    const int qBytes = p.KB * kTileM * kKBlock * 2;     // one query tile   (128 rows)
-    // one ring stage: a whole database tile (256 rows x dpad), or -- K-split mode, dpad > 128, where two query tiles plus
-    // whole-tile stages no longer fit 227 KB -- one 64-wide K-block of it.  K-split streams every tile once per
-    // accumulator (twice per unit): L2 -> SM traffic doubles, the roles and the epilogue stay exactly the same.
+    const int qBytes = p.KB * kTileM * kKBlock * 2; // the query tile (128 rows)
+    // one ring stage: a whole database tile (256 rows x dpad), or -- K-split mode, dpad > 128, where the query tile
+    // plus several whole-tile stages no longer fit 227 KB -- one 64-wide K-block of it
     const int stageBytes = (p.ksplit ? 1 : p.KB) * kTileN * kKBlock * 2;
-    unsigned char* sQ = smem;                            // two query tiles
-    unsigned char* sY = smem + 2 * qBytes;
+    unsigned char* sQ = smem;
+    unsigned char* sY = smem + qBytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(sY + (size_t)p.yStages * stageBytes);
     uint64_t* q_full = bars + 0;
     uint64_t* q_empty = bars + 1;
     uint64_t* y_full = bars + 2;
     uint64_t* y_empty = y_full + kMaxYStages;
-    uint64_t* t_full = y_empty + kMaxYStages; // [2] one per accumulator half
-    uint64_t* t_empty = t_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
 
-    const int warp = threadIdx.x >> 5;
+    // warp index as a provably warp-uniform value: ptxas then knows every warpgroup reaches its wgmma converged
+    // (otherwise it serialises the wgmma chain)
+    const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
-    constexpr int kEpiWarps = 4 * PARTS;
-    constexpr int kColsPerThread = kTileN / PARTS; // columns of a tile one epilogue thread filters
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kConsumerWarps && lane == 0) {
         ptx::prefetch_tensormap(&mapQ);
         ptx::prefetch_tensormap(&mapY);
         ptx::mbar_init(q_full, 1);
-        ptx::mbar_init(q_empty, 1);
+        ptx::mbar_init(q_empty, kConsumerWarps);
         for (int i = 0; i < p.yStages; i++) {
             ptx::mbar_init(&y_full[i], 1);
-            ptx::mbar_init(&y_empty[i], 1);
-        }
-        for (int i = 0; i < 2; i++) {
-            ptx::mbar_init(&t_full[i], 1);
-            ptx::mbar_init(&t_empty[i], kEpiWarps);
+            ptx::mbar_init(&y_empty[i], kConsumerWarps);
         }
         ptx::fence_barrier_init();
     }
-    if (warp == 1) {
-        ptx::tmem_alloc<512>(tmem_slot);
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == kConsumerWarps) {
         // ================================ TMA producer ================================
         if (lane == 0) {
             int ys = 0;
             uint32_t yphase = 0;
             int it = 0;
             for (int u = blockIdx.x; u < p.numUnits; u += gridDim.x, it++) {
-                const int pair = u % p.qPairs;
+                const int qunit = u % p.qPairs;
                 const int sl = u / p.qPairs;
                 ptx::mbar_wait(q_empty, (it & 1) ^ 1);
-                ptx::mbar_arrive_expect_tx(q_full, (uint32_t)(2 * qBytes));
-                ptx::tma_load_3d(sQ, &mapQ, q_full, 0, pair * kPairM, 0);
-                ptx::tma_load_3d(sQ + qBytes, &mapQ, q_full, 0, pair * kPairM + kTileM, 0);
+                ptx::mbar_arrive_expect_tx(q_full, (uint32_t)qBytes);
+                ptx::tma_load_3d(sQ, &mapQ, q_full, 0, qunit * kUnitM, 0);
                 const int pb = p.tileBegin + sl * p.tilesPerSlice;
                 const int pe = min(p.tileEnd, pb + p.tilesPerSlice);
                 for (int pp = pb; pp < pe; pp++) {
                     const int t = perm_tile(p, pp);
-                    // K-split: mapY's box is one K-block; the tile goes through the ring once per accumulator
-                    const int loads = p.ksplit ? 2 * p.KB : 1;
+                    // K-split: mapY's box is one K-block; both warpgroups consume every stage
+                    const int loads = p.ksplit ? p.KB : 1;
                     for (int l = 0; l < loads; l++) {
                         ptx::mbar_wait(&y_empty[ys], yphase ^ 1);
                         ptx::mbar_arrive_expect_tx(&y_full[ys], (uint32_t)stageBytes);
-                        ptx::tma_load_3d(sY + (size_t)ys * stageBytes, &mapY, &y_full[ys], 0, t * kTileN, p.ksplit ? l % p.KB : 0);
+                        ptx::tma_load_3d(sY + (size_t)ys * stageBytes, &mapY, &y_full[ys], 0, t * kTileN, l);
                         if (++ys == p.yStages) {
                             ys = 0;
                             yphase ^= 1;
@@ -250,186 +210,114 @@ __global__ void __launch_bounds__(tcThreads(PARTS), 1) flat_tc_kernel(
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================================ MMA issuer ================================
-        if (lane == 0) {
-            constexpr uint32_t idesc = ptx::make_idesc_f16(kTileM, kTileN);
-            int ys = 0;
-            uint32_t yphase = 0, tphase = 0;
-            int it = 0;
-            const uint32_t sQaddr = ptx::smem_u32(sQ);
-            const uint32_t sYaddr = ptx::smem_u32(sY);
-            const int qkb = kTileM * kKBlock * 2; // bytes per K-block of a query tile
-            const int ykb = kTileN * kKBlock * 2; // bytes per K-block of a database tile
-            for (int u = blockIdx.x; u < p.numUnits; u += gridDim.x, it++) {
-                const int sl = u / p.qPairs;
-                const int pb = p.tileBegin + sl * p.tilesPerSlice;
-                const int pe = min(p.tileEnd, pb + p.tilesPerSlice);
-                ptx::mbar_wait(q_full, it & 1);
-                ptx::tc_fence_after();
-                for (int pp = pb; pp < pe; pp++) {
-                    if (p.ksplit) {
-                        // one ring stage per K-block, consumed in the producer's order (h outer, kb inner)
-#pragma unroll 1
-                        for (int h = 0; h < 2; h++) {
-                            ptx::mbar_wait(&t_empty[h], tphase ^ 1);
-                            ptx::tc_fence_after();
-                            const uint32_t dcol = tmem_base + (uint32_t)h * kTileN;
-                            const uint32_t qaddr = sQaddr + (uint32_t)h * (uint32_t)qBytes;
-                            for (int kb = 0; kb < p.KB; kb++) {
-                                ptx::mbar_wait(&y_full[ys], yphase);
-                                ptx::tc_fence_after();
-                                const uint32_t yaddr = sYaddr + (uint32_t)ys * (uint32_t)stageBytes;
-                                const int k4n = min(4, p.kSteps - 4 * kb);
-                                for (int k4 = 0; k4 < k4n; k4++) {
-                                    uint64_t da = ptx::make_smem_desc_sw128(qaddr + kb * qkb + k4 * 32);
-                                    uint64_t db = ptx::make_smem_desc_sw128(yaddr + k4 * 32);
-                                    ptx::mma_f16_ss(dcol, da, db, idesc, (kb | k4) != 0 ? 1u : 0u);
-                                }
-                                ptx::mma_commit(&y_empty[ys]);
-                                if (++ys == p.yStages) {
-                                    ys = 0;
-                                    yphase ^= 1;
-                                }
-                            }
-                            ptx::mma_commit(&t_full[h]);
-                        }
-                        tphase ^= 1;
-                        continue;
-                    }
-                    ptx::mbar_wait(&y_full[ys], yphase);
-                    ptx::tc_fence_after();
-                    const uint32_t yaddr = sYaddr + (uint32_t)ys * (uint32_t)stageBytes;
-#pragma unroll 1
-                    for (int h = 0; h < 2; h++) {
-                        ptx::mbar_wait(&t_empty[h], tphase ^ 1); // epilogue drained this accumulator
-                        ptx::tc_fence_after();
-                        const uint32_t dcol = tmem_base + (uint32_t)h * kTileN;
-                        const uint32_t qaddr = sQaddr + (uint32_t)h * (uint32_t)qBytes;
-                        // (d = 96: 6 of the 8 K-steps of the padded tile -- a quarter of the tensor work is zeros otherwise)
-                        for (int ks = 0; ks < p.kSteps; ks++) {
-                            const int kb = ks >> 2, k4 = ks & 3;
-                            uint64_t da = ptx::make_smem_desc_sw128(qaddr + kb * qkb + k4 * 32);
-                            uint64_t db = ptx::make_smem_desc_sw128(yaddr + kb * ykb + k4 * 32);
-                            ptx::mma_f16_ss(dcol, da, db, idesc, ks != 0 ? 1u : 0u);
-                        }
-                        ptx::mma_commit(&t_full[h]); // accumulator ready for the epilogue
-                    }
-                    ptx::mma_commit(&y_empty[ys]); // smem stage reusable once these MMAs retire
-                    tphase ^= 1;
-                    if (++ys == p.yStages) {
-                        ys = 0;
-                        yphase ^= 1;
-                    }
-                }
-                ptx::mma_commit(q_empty); // the query tiles may be overwritten
-            }
-        }
-    } else {
-        // ================================ epilogue ================================
-        const int ew = warp - 2;
-        const int quarter = warp & 3;  // TMEM lane quarter this warp may access
-        const int half = ew >> 2;      // which column part of a tile
-        const int row = quarter * 32 + lane;
-        const float inv = *p.invScalePtr;
-        const uint32_t lane_acc = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(half * kColsPerThread);
-        uint32_t tphase = 0;
-        const int permStep = (int)(p.permA % p.numTiles);
-        for (int u = blockIdx.x; u < p.numUnits; u += gridDim.x) {
-            const int pair = u % p.qPairs;
-            const int sl = u / p.qPairs;
-            // per-thread filter state for its two queries (one per query tile of the pair)
-            const int q0 = pair * kPairM + row;
-            const int q1 = q0 + kTileM;
-            float thr0 = (!DUMP && q0 < p.nq) ? p.thr[q0] : CUDART_INF_F;
-            float thr1 = (!DUMP && q1 < p.nq) ? p.thr[q1] : CUDART_INF_F;
-            const float slack0 = (SELF && q0 < p.nq) ? 2.f * p.eps[q0] : 0.f;
-            const float slack1 = (SELF && q1 < p.nq) ? 2.f * p.eps[q1] : 0.f;
-            const long long seg0 = ((long long)u * kPairM + row) * PARTS + half;
-            const long long seg1 = ((long long)u * kPairM + kTileM + row) * PARTS + half;
-            uint2* buf0 = DUMP ? nullptr : p.cand + seg0 * p.cap;
-            uint2* buf1 = DUMP ? nullptr : p.cand + seg1 * p.cap;
-            int cnt0 = 0, cnt1 = 0;
-            const int pb = p.tileBegin + sl * p.tilesPerSlice;
-            const int pe = min(p.tileEnd, pb + p.tilesPerSlice);
-
-            // PARTS == 2: block stream per database tile (h=0: blocks 0,1), (h=1: blocks 0,1), 64 columns each
-            // (two x32 TMEM loads) filtered together for instruction-level parallelism with 2 warps per
-            // scheduler.  PARTS == 4: 4 warps per scheduler hide the latencies; 32-column chunks keep the
-            // thread under the 112-register budget of a 576-thread CTA.
-            uint32_t a0[32], a1[PARTS == 2 ? 32 : 1];
-            // tile ids follow the producer's affine permutation incrementally; the tile's bias bound is
-            // fetched one tile ahead (its L2 latency would otherwise sit on the filter's critical path)
-            int t = pb < pe ? perm_tile(p, pb) : 0;
-            float maxbNext = (!DUMP && pb < pe) ? __ldg(p.tileMaxBias + t) : 0.f;
-            float minbNext = (SELF && pb < pe) ? __ldg(p.tileMinBias + t) : 0.f;
-            for (int pp = pb; pp < pe; pp++) {
-                const long long colBase = (long long)t * kTileN + half * kColsPerThread;
-                const float maxb = maxbNext;
-                const float minb = minbNext;
-                t += permStep;
-                if (t >= (int)p.numTiles)
-                    t -= (int)p.numTiles;
-                if (!DUMP && pp + 1 < pe)
-                    maxbNext = __ldg(p.tileMaxBias + t);
-                if (SELF && pp + 1 < pe)
-                    minbNext = __ldg(p.tileMinBias + t);
-#pragma unroll 1
-                for (int h = 0; h < 2; h++) {
-                    const int q = h ? q1 : q0;
-                    float thr = h ? thr1 : thr0;
-                    const float slack = h ? slack1 : slack0;
-                    uint2* buf = h ? buf1 : buf0;
-                    int cnt = h ? cnt1 : cnt0;
-                    const uint32_t acc = lane_acc + (uint32_t)h * kTileN;
-                    ptx::mbar_wait(&t_full[h], tphase);
-                    ptx::tc_fence_after();
-#pragma unroll 1
-                    for (int blk = 0; blk < 2; blk++) {
-                        if constexpr (PARTS == 2) {
-                            ptx::tmem_ld_32x32b_x32(acc + (uint32_t)(blk * 64), a0);
-                            ptx::tmem_ld_32x32b_x32(acc + (uint32_t)(blk * 64 + 32), a1);
-                        } else {
-                            ptx::tmem_ld_32x32b_x32(acc + (uint32_t)(blk * 32), a0);
-                        }
-                        ptx::tmem_ld_wait();
-                        if (blk == 1) { // the accumulator is out of TMEM: hand it back to the MMA warp
-                            ptx::tc_fence_before();
-                            __syncwarp();
-                            if (lane == 0)
-                                ptx::mbar_arrive(&t_empty[h]);
-                        }
-                        if (DBG == 0) {
-                            if constexpr (PARTS == 2)
-                                epi_filter64<DUMP, SELF>(p, a0, a1, q, colBase + blk * 64, inv, thr, slack, maxb, buf, cnt, minb);
-                            else
-                                epi_filter32<DUMP, SELF>(p, a0, q, colBase + blk * 32, inv, thr, slack, maxb, buf, cnt, minb);
-                        }
-                    }
-                    if (h) {
-                        cnt1 = cnt;
-                        if (SELF)
-                            thr1 = thr;
-                    } else {
-                        cnt0 = cnt;
-                        if (SELF)
-                            thr0 = thr;
-                    }
-                }
-                tphase ^= 1;
-            }
-            if (!DUMP) {
-                p.candCount[seg0] = cnt0;
-                p.candCount[seg1] = cnt1;
-            }
-        }
+        return;
     }
 
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<512>(tmem_base);
+    // ================================ consumers ================================
+    const int wg = warp >> 2;
+    const int part = lane & 3;
+    const int row = wg * kWgM + (warp & 3) * 16 + (lane >> 2); // first of the thread's two rows; the second is row + 8
+    const float inv = *p.invScalePtr;
+    const uint32_t sQaddr = ptx::smem_u32(sQ) + (uint32_t)(wg * kWgM * kKBlock * 2); // this warpgroup's 64 rows
+    const uint32_t sYaddr = ptx::smem_u32(sY);
+    const int qkb = kTileM * kKBlock * 2; // bytes per K-block of the query tile
+    const int ykb = kTileN * kKBlock * 2; // bytes per K-block of a database tile
+    const int permStep = (int)(p.permA % p.numTiles);
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; i++)
+        acc[i] = 0.f;
+    int ys = 0;
+    uint32_t yphase = 0;
+    int it = 0;
+    for (int u = blockIdx.x; u < p.numUnits; u += gridDim.x, it++) {
+        const int qunit = u % p.qPairs;
+        const int sl = u / p.qPairs;
+        // per-thread filter state for its two queries
+        const int q0 = qunit * kUnitM + row;
+        const int q1 = q0 + 8;
+        float thr0 = (!DUMP && q0 < p.nq) ? p.thr[q0] : CUDART_INF_F;
+        float thr1 = (!DUMP && q1 < p.nq) ? p.thr[q1] : CUDART_INF_F;
+        const float slack0 = (SELF && q0 < p.nq) ? 2.f * p.eps[q0] : 0.f;
+        const float slack1 = (SELF && q1 < p.nq) ? 2.f * p.eps[q1] : 0.f;
+        const long long seg0 = ((long long)u * kUnitM + row) * kParts + part;
+        const long long seg1 = ((long long)u * kUnitM + row + 8) * kParts + part;
+        uint2* buf0 = DUMP ? nullptr : p.cand + seg0 * p.cap;
+        uint2* buf1 = DUMP ? nullptr : p.cand + seg1 * p.cap;
+        int cnt0 = 0, cnt1 = 0;
+        const int pb = p.tileBegin + sl * p.tilesPerSlice;
+        const int pe = min(p.tileEnd, pb + p.tilesPerSlice);
+
+        // tile ids follow the producer's affine permutation incrementally; the tile's bias bound is
+        // fetched one tile ahead (its L2 latency would otherwise sit on the filter's critical path)
+        int t = pb < pe ? perm_tile(p, pb) : 0;
+        float maxbNext = (!DUMP && pb < pe) ? __ldg(p.tileMaxBias + t) : 0.f;
+        float minbNext = (SELF && pb < pe) ? __ldg(p.tileMinBias + t) : 0.f;
+        ptx::mbar_wait(q_full, it & 1);
+        for (int pp = pb; pp < pe; pp++) {
+            const long long colBase = (long long)t * kTileN + 2 * part;
+            const float maxb = maxbNext;
+            const float minb = minbNext;
+            t += permStep;
+            if (t >= (int)p.numTiles)
+                t -= (int)p.numTiles;
+            if (!DUMP && pp + 1 < pe)
+                maxbNext = __ldg(p.tileMaxBias + t);
+            if (SELF && pp + 1 < pe)
+                minbNext = __ldg(p.tileMinBias + t);
+
+            // ---- scores of the tile: acc = Q[64 rows] . Y[256 rows]^T
+            const int stagesPerTile = p.ksplit ? p.KB : 1;
+#pragma unroll 1
+            for (int kb0 = 0; kb0 < stagesPerTile; kb0++) {
+                ptx::mbar_wait(&y_full[ys], yphase);
+                const uint32_t yaddr = sYaddr + (uint32_t)ys * (uint32_t)stageBytes;
+                // K-steps of this stage (d = 96: 6 of the 8 K-steps of the padded tile -- a quarter of the tensor
+                // work is zeros otherwise)
+                const int ks0 = p.ksplit ? 4 * kb0 : 0;
+                const int ks1 = p.ksplit ? min(p.kSteps, ks0 + 4) : p.kSteps;
+                ptx::wgmma_fence();
+#pragma unroll 1
+                for (int ks = ks0; ks < ks1; ks++) {
+                    const int kb = ks >> 2, k4 = ks & 3;
+                    const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + kb * qkb + k4 * 32);
+                    const uint64_t db = ptx::make_smem_desc_sw128(yaddr + (p.ksplit ? 0 : kb * ykb) + k4 * 32);
+                    ptx::wgmma_m64n256k16_f16_ss(acc, da, db, ks != 0 ? 1u : 0u);
+                }
+                ptx::wgmma_commit();
+                ptx::wgmma_wait_all();
+                __syncwarp();
+                if (lane == 0) // this warp's share of the stage has been read
+                    ptx::mbar_arrive(&y_empty[ys]);
+                if (++ys == p.yStages) {
+                    ys = 0;
+                    yphase ^= 1;
+                }
+            }
+
+            // ---- filter: two rows x two 32-element chunks (128 columns each)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+#pragma unroll
+                for (int c = 0; c < 2; c++) {
+                    float r[32];
+#pragma unroll
+                    for (int e = 0; e < 32; e++)
+                        r[e] = acc[4 * (16 * c + (e >> 1)) + 2 * h + (e & 1)];
+                    if (h)
+                        epi_filter32<DUMP, SELF>(p, r, q1, colBase + 128 * c, inv, thr1, slack1, maxb, buf1, cnt1, minb);
+                    else
+                        epi_filter32<DUMP, SELF>(p, r, q0, colBase + 128 * c, inv, thr0, slack0, maxb, buf0, cnt0, minb);
+                }
+            }
+        }
+        __syncwarp();
+        if (lane == 0) // the query tile may be overwritten
+            ptx::mbar_arrive(q_empty);
+        if (!DUMP) {
+            p.candCount[seg0] = cnt0;
+            p.candCount[seg1] = cnt1;
+        }
     }
 }
 

@@ -1594,9 +1594,9 @@ bool GpuIndexIVFPQ::precomputedActive_() const {
         return false;
     if (precomputedExplicit_)
         return usePrecomputed_;
-    // auto: the CPU reference's size rule, and only where it pays -- measured on B200: with long lists
-    // (N=100M / nlist=4096, 24k vectors per list) the direct LUT is faster (55.7 vs 57.7 ms per step, the
-    // build is ~2 % of the scan); with short lists (nlist=65536) the LUT build dominates the CTA
+    // auto: the CPU reference's size rule, and only with short lists: with long lists (N=100M / nlist=4096, 24k
+    // vectors per list) the LUT build is a small share of the scan and the direct LUT needs no [nlist][256][M] table
+    // reads; with short lists (nlist=65536) the LUT build dominates the CTA
     const size_t bytes = sizeof(float) * (size_t)nlist * 256 * M_;
     return bytes <= (size_t(1) << 31) && this->ntotal / nlist < 4096;
 }

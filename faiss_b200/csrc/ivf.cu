@@ -468,7 +468,7 @@ void runMergeTopKKeyspace(
 // CTAs per query: 1 when the queries alone fill the machine several times over, else the probes are
 // split so that ~8 CTAs per SM exist
 int ivfScanChunks(int device, int64_t nq, int nprobe, int* probesPerCta) {
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     const int64_t wantCtas = (int64_t)sms * 8;
     int chunks = (int)std::min<int64_t>(nprobe, std::max<int64_t>(1, ceil_div(wantCtas, nq)));

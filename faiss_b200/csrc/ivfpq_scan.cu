@@ -110,7 +110,7 @@ __device__ __forceinline__ float lds_f32(unsigned addr) {
 // Keys: L2 -> sum of LUT entries (+ ||x - c||^2 with precomputed tables); IP -> -(q.centroid) - sum.
 // kU: groups of 32 vectors per work unit (kU * 32 * M bytes of codes in flight per warp); kMinCtas: CTAs per
 // SM the register budget is set for; ROLL: rolling prefetch of the next unit (L2 pairs); SBASE: shared-window address of the dynamic shared
-// memory (0x400 on sm_100: the first KB of the window is reserved), folded into the LDS immediate so that the
+// memory (0x400 on sm_90: the first KB of the window is reserved), folded into the LDS immediate so that the
 // PRMT result IS the address; -1 = unknown (one extra IADD per lookup).
 template <int M, bool IS_L2, bool PRECOMP, typename IdT, int kWarps, int kU, int kMinCtas, bool ROLL, int SBASE>
 __global__ void __launch_bounds__(kWarps * 32, kMinCtas) ivfpq_scan_interleaved_kernel(
@@ -558,7 +558,7 @@ static void launchScanV(
     CUDA_CHECK_LAST();
 }
 
-// launch shapes (FB200_PQ_CFG selects one for A/B runs; see profiles/ for the measurements behind the default)
+// launch shapes (FB200_PQ_CFG selects one for A/B runs)
 //   0: 16 warps, 4 KB of codes in flight per warp, 2 CTAs/SM (64 registers)
 //   1: 16 warps, 2 KB per warp, 3 CTAs/SM (42 registers)      2: 32 warps, 2 KB per warp, 2 CTAs/SM (32 registers)
 static int scanConfig() {

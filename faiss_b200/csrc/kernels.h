@@ -95,7 +95,7 @@ void runCalcResidual(
 // gather rows by id (reconstruct_batch) / by range
 void runGatherRows(const void* src, const idx_t* ids, int64_t n, int d, float* out, cudaStream_t stream, int yHalf = 0);
 
-// ---------------------------------------------------------------- flat_tc.cu  (tcgen05 path)
+// ---------------------------------------------------------------- flat_tc.cu  (tensor-core path)
 struct FlatTcPlan; // opaque: tensor maps + scratch sizing for one (index, nq, k) shape
 
 // fp32 rows -> scaled fp16 rows (padded to dpad, multiple of 64) + score bias (bias = -||y||^2/2 for
@@ -134,7 +134,7 @@ struct FlatTcShard {
     int64_t maxTiles;         // max over ranks of ceil(n_r / 256): the common round schedule
 };
 
-// Full certified search: fp16 tcgen05 scoring + candidate emission + exact fp32 re-rank, with the
+// Full certified search: fp16 wgmma scoring + candidate emission + exact fp32 re-rank, with the
 // exact SIMT kernel as fallback for queries whose certificate fails.  See flat_tc.cu.
 void runFlatTcSearch(
         GpuResources* res,
@@ -284,7 +284,7 @@ void runIvfPqScan(
         idx_t* outI,
         cudaStream_t stream);
 
-// ---- "rotated, interleaved-by-32" PQ code layout (B200-native storage for M % 16 == 0, M <= 32) ----
+// ---- "rotated, interleaved-by-32" PQ code layout (native storage for M % 16 == 0, M <= 32) ----
 // List-relative vector v = 32*g + t is stored in group g; byte position j of the vector holds
 // code[(j + t) % M] and lives at  g*32*M + (j/16)*512 + t*16 + (j%16).  A warp therefore loads a
 // group with fully coalesced 128-bit loads (512 B per instruction), and at step j lane t needs the

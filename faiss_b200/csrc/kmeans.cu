@@ -219,7 +219,7 @@ void runKmeansAccumulate(
     }
     size_t smem = sizeof(float) * ((size_t)k * d + k);
     if (smem <= 64 * 1024) {
-        int64_t ppb = std::max<int64_t>(256, ceil_div(n, 148 * 4));
+        int64_t ppb = std::max<int64_t>(256, ceil_div(n, 132 * 4));
         CUDA_VERIFY(cudaFuncSetAttribute(
                 kmeans_accum_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kmeans_accum_smem_kernel<<<(unsigned)ceil_div(n, ppb), 256, smem, stream>>>(

@@ -111,7 +111,7 @@ void StackDeviceMemory::dealloc(void* p) {
 
 // ---------------------------------------------------------------- StandardGpuResources
 // default pinned size 256 MiB (faiss/gpu/StandardGpuResources.cpp:49); default temp memory: the
-// reference caps at 1.5 GiB for >8 GiB devices (:58,180-208).  A B200 carries 180 GB, and the
+// reference caps at 1.5 GiB for >8 GiB devices (:58,180-208).  An H100 carries 80 GB, and the
 // fused Flat path wants candidate arenas resident, so the default here is 4 GiB.
 StandardGpuResources::StandardGpuResources()
         : tempMemSize_(size_t(4) << 30), pinnedSize_(size_t(256) << 20) {}
@@ -197,10 +197,10 @@ void StandardGpuResources::initializeForDevice(int device) {
     DeviceScope s(device);
     cudaDeviceProp prop;
     CUDA_VERIFY(cudaGetDeviceProperties(&prop, device));
-    // this library carries sm_100a SASS only; fail loudly elsewhere
+    // this library carries sm_90a SASS only; fail loudly elsewhere
     FB_THROW_IF_NOT_FMT(
-            prop.major == 10,
-            "device %d is sm_%d%d; faiss_b200 kernels are built for sm_100a (B200) only",
+            prop.major == 9 && prop.minor == 0,
+            "device %d is sm_%d%d; faiss_b200 kernels are built for sm_90a (H100) only",
             device,
             prop.major,
             prop.minor);

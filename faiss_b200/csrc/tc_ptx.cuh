@@ -1,7 +1,7 @@
-// faiss_b200 -- thin inline-PTX wrappers for the Blackwell (sm_100a) async machinery used by the
-// tensor-core Flat kernel: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit /
-// ld / fences) and the shared-memory + instruction descriptors.  Bit layouts follow the PTX ISA
-// tcgen05 "matrix descriptor" / "instruction descriptor" tables.
+// faiss_b200 -- thin inline-PTX wrappers for the Hopper (sm_90a) async machinery used by the
+// tensor-core Flat kernel: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit /
+// wait) and the shared-memory matrix descriptor.  Bit layouts follow the PTX ISA "Matrix Descriptor
+// Format" table of the asynchronous warpgroup-level matrix instructions.
 #pragma once
 
 #include <cuda.h>
@@ -114,100 +114,66 @@ __device__ __forceinline__ void sts32(uint32_t addr, int v) {
     asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 
-// ------------------------------------------------------------------ packed fp32 math (sm_100)
-// (o0,o1) = (a0,a1) * (s,s) + (c0,c1)   -> one FFMA2
-__device__ __forceinline__ void fma2(float& o0, float& o1, float a0, float a1, float s, float c0, float c1) {
-    asm("{\n.reg .b64 ra, rs, rc, rd;\nmov.b64 ra, {%2,%3};\nmov.b64 rs, {%4,%4};\nmov.b64 rc, {%5,%6};\n"
-        "fma.rn.f32x2 rd, ra, rs, rc;\nmov.b64 {%0,%1}, rd;\n}"
-        : "=f"(o0), "=f"(o1)
-        : "f"(a0), "f"(a1), "f"(s), "f"(c0), "f"(c1));
+// ------------------------------------------------------------------ wgmma
+__device__ __forceinline__ void wgmma_fence() {
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-// 3-input max -> one FMNMX3
-__device__ __forceinline__ float max3(float a, float b, float c) {
-    float d;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-    return d;
+__device__ __forceinline__ void wgmma_commit() {
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-
-// ------------------------------------------------------------------ tcgen05
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "n"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_wait_all() {
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, fp16/bf16 inputs, fp32 accumulate
-__device__ __forceinline__ void mma_f16_ss(
-        uint32_t tmem_d,
-        uint64_t desc_a,
-        uint64_t desc_b,
-        uint32_t idesc,
-        uint32_t accumulate) {
+// D[64 x 256, registers] (+)= A[smem desc, 64 x 16] * B[smem desc, 256 x 16]^T, fp16 inputs, fp32 accumulate,
+// both operands K-major.  Fragment of D held by thread t of the warpgroup (warp w = t / 32, lane l):
+//   d[4 j + 2 h + b] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + b]   (j < 32, h, b < 2)
+__device__ __forceinline__ void wgmma_m64n256k16_f16_ss(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
             "{\n"
             ".reg .pred p;\n"
-            "setp.ne.b32 p, %4, 0;\n"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-            "}\n" ::"r"(tmem_d),
-            "l"(desc_a),
-            "l"(desc_b),
-            "r"(idesc),
-            "r"(accumulate)
-            : "memory");
-}
-// mbarrier arrive when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+            "setp.ne.b32 p, %130, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
             "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-              "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-              "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-              "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-              "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(taddr)
-            : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+            "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+            "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+            "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+            "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+            "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+            "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+            "%128, %129, p, 1, 1, 0, 0;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+              "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+              "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+              "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+              "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+              "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+              "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+              "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+              "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+            : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
 // ------------------------------------------------------------------ descriptors
 // Shared-memory matrix descriptor, K-major operand, 128-byte swizzle:
 //   rows of 128 B (64 fp16), 8-row core groups of 1024 B (stride byte offset), tile base 1024-aligned.
 //   bits [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major, set 1) | [32,46) SBO>>4
-//   | [46,48) version=1 | [61,64) layout (2 = SWIZZLE_128B)
+//   | [49,52) base offset (0: 1024-aligned atoms) | [62,64) layout (1 = SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
-}
-// Instruction descriptor for kind::f16: fp16 A/B (format 0), fp32 accumulate, both K-major.
-//   bits [4,6) c_format=1 (F32) | [7,10) a_format | [10,13) b_format | 15 a_major | 16 b_major
-//   | [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-    return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 } // namespace ptx

@@ -1,4 +1,4 @@
-/* faiss_b200 -- C ABI of the B200-native similarity-search backend.
+/* faiss_b200 -- C ABI of the H100-native (sm_90a) similarity-search backend.
  *
  * Plain C (extern "C"), opaque handles, plain pointers and sizes; no torch / C++ types.
  * Two tiers:
@@ -97,7 +97,7 @@ FB200_API int faiss_GpuIndex_setMinPagingSize(FaissGpuIndex* index, size_t size)
 FB200_API int faiss_GpuIndex_getMinPagingSize(const FaissGpuIndex* index, size_t* out_size);
 
 /* ---- GpuIndexFlat (faiss/gpu/GpuIndexFlat.h:43-217) ---- */
-/* use_tensor_cores: 1 = tcgen05 path when the shape supports it (default), 0 = exact SIMT only */
+/* use_tensor_cores: 1 = tensor-core path when the shape supports it (default), 0 = exact SIMT only */
 FB200_API int faiss_GpuIndexFlat_new(FaissGpuIndex** p_index, FaissStandardGpuResources* res, int d, FaissMetricType metric, int device, int use_tensor_cores);
 /* GpuIndexFlatConfig (faiss/gpu/GpuIndexFlat.h:26-35).  use_float16: the vectors are stored as fp16 and queries are
  * rounded to fp16 before the comparison, as FlatIndex::query does (faiss/gpu/impl/FlatIndex.cu:112-136); distances are
@@ -248,7 +248,7 @@ FB200_API int b200_l2_norms(FaissStandardGpuResources* res, int device, const fl
 FB200_API int b200_flat_search_exact(FaissStandardGpuResources* res, int device, const float* Y, idx_t N, int d, const float* Q, idx_t nq, int k, FaissMetricType metric, float* D, idx_t* I);
 /* role of merge_knn_results (faiss/utils/Heap.cpp:166-238) on the device: in [nq, nshard, k] */
 FB200_API int b200_topk_merge(FaissStandardGpuResources* res, int device, const float* D_in, const idx_t* I_in, idx_t nq, int nshard, int k_in, const idx_t* id_offsets /* device, [nshard] or NULL */, int k, FaissMetricType metric, float* D, idx_t* I);
-/* unit-test seam for the tcgen05 path: S[nq, roundup(N,128)] = Q16 . Y16^T (fp16 inputs) */
+/* unit-test seam for the tensor-core path: S[nq, roundup(N,256)] = Q16 . Y16^T (fp16 inputs) */
 FB200_API int b200_flat_tc_scores_debug(FaissStandardGpuResources* res, int device, const void* Q16, idx_t nq, const void* Y16, idx_t N, int dpad, float* S);
 /* role of IVFBase::searchCoarseQuantizer_ (faiss/gpu/impl/IVFBase.cu:509-545): nprobe nearest centroids per query */
 FB200_API int b200_ivf_coarse(FaissStandardGpuResources* res, int device, const float* centroids, idx_t nlist, int d, const float* Q, idx_t nq, int nprobe, FaissMetricType metric, float* coarse_dis, idx_t* coarse_ids);

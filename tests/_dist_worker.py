@@ -31,7 +31,7 @@ def main():
     out = {"world": world}
     rs = np.random.RandomState(123)
 
-    # ---- Flat, tensor-core path with pooled thresholds (N large enough for tcgen05), floats and integers
+    # ---- Flat, tensor-core path with pooled thresholds (N large enough for the tensor-core path), floats and integers
     N, d, nq, k = 300_000, 64, 700, 50
     xb = rs.rand(N, d).astype(np.float32)
     xq = rs.rand(nq, d).astype(np.float32)

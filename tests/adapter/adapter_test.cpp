@@ -1,5 +1,5 @@
-// Runs the REFERENCE's own drivers over the faiss_b200 adapter (needs a B200; built by faiss_b200/build.py
-// where /root/reference is available, executed by tests/test_adapter_gpu.py):
+// Runs the REFERENCE's own drivers over the faiss_b200 adapter (needs a GPU; built by tests/adapter/build_adapter.py
+// where the reference's headers are available, executed by tests/test_adapter_gpu.py):
 //   1. index_cpu_to_b200(IndexFlatL2) answers like the CPU index (integer data: identical ids and distances)
 //   2. faiss::Clustering::train(n, x, adapter) == faiss::Clustering::train(n, x, IndexFlatL2)  (faiss/Clustering.cpp:254-356)
 //   3. faiss::IndexShards over adapter sub-indexes == CPU IndexFlat                              (faiss/IndexShards.cpp:197-264)

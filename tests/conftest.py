@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (B200, sm_100a)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (H100, sm_90a)")
 
 
 def _has_gpu():

@@ -1,6 +1,6 @@
 """The compiled faiss::Index adapter (faiss_b200/adapter): built against the reference's own headers and
 CPU library, then driven by the reference's own code -- faiss::Clustering::train, faiss::IndexShards, the cloner
-pair -- on a B200 (tests/adapter/adapter_test.cpp)."""
+pair -- on the GPU (tests/adapter/adapter_test.cpp)."""
 import os
 import subprocess
 

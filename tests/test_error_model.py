@@ -1,4 +1,4 @@
-"""CPU model of the tcgen05 Flat path's rounding certificate (DESIGN.md 3.1, `tc_prepare_queries_kernel`):
+"""CPU model of the tensor-core Flat path's rounding certificate (DESIGN.md 3.1, `tc_prepare_queries_kernel`):
 fp16 inputs after power-of-two scaling, fp32 accumulation, fp32 bias, one FMA -- against the bound
 eps_q = c1*|q|*max|y| + c2*(|q| + max|y|)^2 that the kernel uses to set thresholds.  The test restates the
 arithmetic in numpy (it does not call the product) and checks, over norm ratios from 1e-3 to 1e3, that

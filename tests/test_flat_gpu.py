@@ -4,7 +4,7 @@ Model: the reference's CPU-vs-GPU differential tests (faiss/gpu/test/TestGpuInde
 compareLists in faiss/gpu/test/TestUtils.cpp:234-443), with tighter bars:
   * integer-valued inputs -> ids AND distances bit-exact vs the reference CPU result;
   * uniform floats -> distances within 1e-4 relative (north_star), ids up to fp32 near-ties;
-  * the tcgen05 path must return exactly what the exact SIMT path returns.
+  * the tensor-core path must return exactly what the exact SIMT path returns.
 """
 import ctypes
 
@@ -75,7 +75,7 @@ def test_golden_integer_regime_bit_exact(res, golden, k):
      # K-split kernel (128 < d <= 256: ring stages hold single K-blocks) and the large-k lists
      (70000, 192, 300, 100), (66000, 256, 530, 10), (50000, 130, 100, 33), (90000, 64, 300, 1024), (100000, 32, 70, 2048), (40000, 256, 64, 2048)])
 def test_tensor_core_path_equals_exact_path(res, N, d, nq, k, metric):
-    """tcgen05 scoring + certified re-rank must be indistinguishable from the exact kernel"""
+    """wgmma scoring + certified re-rank must be indistinguishable from the exact kernel"""
     import torch
 
     import faiss_b200 as fb
@@ -140,7 +140,7 @@ def test_tensor_core_adversarial_order_falls_back_correctly(res):
 
 
 def test_tcgen05_raw_scores(res):
-    """unit test of the MMA path alone: fp16 operands, fp32 accumulation in TMEM"""
+    """unit test of the MMA path alone: fp16 operands, fp32 accumulation (wgmma, register accumulators)"""
     import torch
 
     import faiss_b200 as fb
@@ -237,7 +237,7 @@ def test_memory_info_and_oom(res):
 @pytest.mark.parametrize("metric", [1, 0])
 @pytest.mark.parametrize("N,d,nq", [(4096, 128, 3000), (70000, 96, 5000), (2048, 64, 17), (300000, 32, 700), (30000, 256, 2000), (5000, 160, 300)])
 def test_streaming_argmin_equals_exact_path(res, N, d, nq, metric):
-    """k = 1 takes the streaming tcgen05 mode (self-tightening thresholds, fused select + re-rank): the k-means
+    """k = 1 takes the streaming tensor-core mode (self-tightening thresholds, fused select + re-rank): the k-means
     assignment path.  Must be indistinguishable from the exact kernel, ids and distances."""
     import torch
 
@@ -303,7 +303,7 @@ def test_bfknn_free_function(res, metric):
 def test_float16_storage(res, N, d, nq, k, tc, metric):
     """GpuIndexFlatConfig::useFloat16 (faiss/gpu/GpuIndexFlat.h:26-35; the reference's TestGpuIndexFlat Float16 cases):
     vectors and queries are rounded to fp16, distances are exact between the rounded values -- i.e. a CPU IndexFlat over
-    the rounded data.  Both paths (tcgen05 + certified re-rank, exact SIMT) must agree bit for bit."""
+    the rounded data.  Both paths (wgmma + certified re-rank, exact SIMT) must agree bit for bit."""
     import faiss_b200 as fb
 
     xb = o.float_rand(N * d, 91).reshape(N, d)

@@ -463,7 +463,7 @@ def test_index_shards_ivf_common_quantizer(res, golden):
 @pytest.mark.parametrize("M", [32, 16])
 def test_ivfpq_k2048(res, M):
     """k = 2048 (the documented GPU limit, faiss/gpu/utils/DeviceDefs.cuh:61-68) through the interleaved scan: the
-    CTA-wide list holds it (round 1 ran out of shared memory above k = 1024)"""
+    CTA-wide list holds it"""
     import faiss_b200 as fb
 
     rs = np.random.RandomState(M)
