@@ -31,9 +31,7 @@
 #include <cfloat>
 #include <cmath>
 #include <cub/cub.cuh>
-#include <cstdlib>
 #include <mutex>
-#include <string>
 #include <vector>
 
 #include "comm.h"
@@ -1021,14 +1019,12 @@ void runFlatTcSearch(
     // first round: ~40 k rows (16 tiles at k = 100).  Every score of round 0 becomes a candidate, so a
     // fixed 16 tiles would make small-k searches (k-means assignment: k = 1, millions of queries) pay 4096
     // candidates per query for nothing.
-    static const int r0Env = getenv("FB200_TC_R0") ? atoi(getenv("FB200_TC_R0")) : 0;
-    int r0Tiles = std::max(r0Env > 0 ? r0Env : std::max(1, (40 * k + kTileN - 1) / kTileN), (k + 127) / 128 * 2);
+    int r0Tiles = std::max(std::max(1, (40 * k + kTileN - 1) / kTileN), (k + 127) / 128 * 2);
     if (nShards > 1) // pooled evidence: nShards * r0Tiles tiles; a shard must still be able to vouch for kFrac rows
         r0Tiles = std::max<int>((r0Tiles + nShards - 1) / nShards, std::max(2, (2 * kFrac + kTileN - 1) / kTileN));
     // threshold selection by bisection (no sorted lists) holds kSelCap entries per query and round: the all-pass first
-    // round is sized to 3/4 of that (FB200_TC_SELECT=sort keeps the bitonic list kernel for A/B runs)
-    static const bool selSortEnv = getenv("FB200_TC_SELECT") && std::string(getenv("FB200_TC_SELECT")) == "sort";
-    const bool useBisect = LIST <= 256 && !selSortEnv;
+    // round is sized to 3/4 of that
+    const bool useBisect = LIST <= 256;
     if (useBisect)
         r0Tiles = std::min(r0Tiles, std::max(2, kSelCap * 3 / 4 / kTileN));
     // queries per pass: bounds the candidate arena, whose largest user is the all-pass round 0
@@ -1036,8 +1032,7 @@ void runFlatTcSearch(
     // k = 1 (k-means assignment, the coarse quantiser of an add): streaming mode -- one pass over all tiles with
     // self-tightening per-thread thresholds (flat_tc_kernel SELF) and a fused select + exact re-rank
     // (tc_argmin_finish_kernel); no rounds, no all-pass first round, no per-query sorted lists.
-    static const bool noStream = getenv("FB200_TC_NO_STREAM") && atoi(getenv("FB200_TC_NO_STREAM")) != 0;
-    const bool streaming = k == 1 && !shard && !noStream;
+    const bool streaming = k == 1 && !shard;
     // streaming: a batch is a whole number of waves of the persistent grid (one 128-query unit per CTA and wave)
     // (large k: the all-pass round covers 40 k rows, so the floor drops to keep the arena near 1 GiB)
     const int64_t kQFloor = r0Tiles > 64 ? 2048 : 16384;
@@ -1080,14 +1075,9 @@ void runFlatTcSearch(
         const int parts = kParts;
         std::vector<Round> rounds;
         {
+            const double g = nShards > 1 ? std::max(4.0, std::min(8.0, 2.0 * nShards)) : 4.0; // growth per round
             int64_t seen = 0;
             while (seen < Tsched) {
-                // schedule knobs (tuning only): first-round tiles, early / late growth factors
-                static const double gEarly = getenv("FB200_TC_G_EARLY") ? atof(getenv("FB200_TC_G_EARLY")) : 4.0;
-                static const double gLate = getenv("FB200_TC_G_LATE") ? atof(getenv("FB200_TC_G_LATE")) : 4.0;
-                static const int64_t lateFrom = getenv("FB200_TC_LATE_FROM") ? atol(getenv("FB200_TC_LATE_FROM")) : 8192;
-                static const double gShard = getenv("FB200_TC_G_SHARD") ? atof(getenv("FB200_TC_G_SHARD")) : 8.0;
-                const double g = nShards > 1 ? std::max(gEarly, std::min(gShard, 2.0 * nShards)) : (seen >= lateFrom ? gLate : gEarly);
                 int64_t end = seen == 0 ? std::min<int64_t>(Tsched, r0Tiles)
                                         : std::min<int64_t>(Tsched, (int64_t)(seen * g));
                 if (Tsched - end < end / 4)

@@ -12,7 +12,6 @@
 //     LUT access is bank-conflict-free by construction (lane t reads bank (t + j) % 32).
 // LUT and distances never touch HBM; the running top-k stays in shared memory (select.cuh).
 #include <cfloat>
-#include <cstdlib>
 #include <type_traits>
 
 #include "kernels.h"
@@ -27,6 +26,8 @@ int ivfScanChunks(int device, int64_t nq, int nprobe, int* probesPerCta);
 namespace {
 
 constexpr int kLutSlots = 64; // 256 B per code value
+constexpr int kScanWarps = 16;  // warps per scan CTA
+constexpr int kScanMinCtas = 2; // CTAs per SM the scan kernel's register budget is set for (64 registers)
 
 __device__ __forceinline__ int64_t interleaved_pos(int64_t v, int j, int M) {
     // byte position j of list-relative vector v
@@ -95,7 +96,7 @@ __device__ __forceinline__ float lds_f32(unsigned addr) {
     return v;
 }
 
-// One CTA = one query x one chunk of its probes, kWarps warps.
+// One CTA = one query x one chunk of its probes, kScanWarps warps.
 //
 //   * ONE top-k list per CTA (CtaTopK, select.cuh): every warp filters against the CTA-wide k-th key,
 //     survivors go to a small per-warp buffer, only the final half-merge runs under a CTA lock.  The list
@@ -108,12 +109,11 @@ __device__ __forceinline__ float lds_f32(unsigned addr) {
 //     of a list is amortised over two.  IP (and any list-independent table) needs no barrier at all.
 //   * inner loop per lookup: PRMT (code byte -> row, packed per-lane slot byte -> column) + LDS + FADD.
 // Keys: L2 -> sum of LUT entries (+ ||x - c||^2 with precomputed tables); IP -> -(q.centroid) - sum.
-// kU: groups of 32 vectors per work unit (kU * 32 * M bytes of codes in flight per warp); kMinCtas: CTAs per
-// SM the register budget is set for; ROLL: rolling prefetch of the next unit (L2 pairs); SBASE: shared-window address of the dynamic shared
-// memory (0x400 on sm_90: the first KB of the window is reserved), folded into the LDS immediate so that the
-// PRMT result IS the address; -1 = unknown (one extra IADD per lookup).
-template <int M, bool IS_L2, bool PRECOMP, typename IdT, int kWarps, int kU, int kMinCtas, bool ROLL, int SBASE>
-__global__ void __launch_bounds__(kWarps * 32, kMinCtas) ivfpq_scan_interleaved_kernel(
+// SBASE: shared-window address of the dynamic shared memory (0x400 on sm_90: the first KB of the window is
+// reserved), folded into the LDS immediate so that the PRMT result IS the address; -1 = unknown (one extra
+// IADD per lookup).
+template <int M, bool IS_L2, bool PRECOMP, typename IdT, int SBASE>
+__global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_interleaved_kernel(
         const float* __restrict__ Q,
         int d,
         const idx_t* __restrict__ probes,
@@ -132,9 +132,10 @@ __global__ void __launch_bounds__(kWarps * 32, kMinCtas) ivfpq_scan_interleaved_
         float* __restrict__ partD,
         idx_t* __restrict__ partI) {
     static_assert(!PRECOMP || IS_L2, "precomputed tables are an L2 decomposition");
-    static_assert((kWarps & (kWarps - 1)) == 0, "kWarps must be a power of two");
+    static_assert((kScanWarps & (kScanWarps - 1)) == 0, "kScanWarps must be a power of two");
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    constexpr int kThreads = kWarps * 32;
+    constexpr int kThreads = kScanWarps * 32;
+    constexpr int kU = M == 32 ? 4 : 8;      // groups of 32 vectors per work unit: 4 KB of codes in flight per warp
     constexpr int H = M / 16;                // 16-byte words per lane and group
     constexpr int kEntriesPerThread = 256 * M / kThreads;
     static_assert(256 * M % kThreads == 0, "LUT entries must divide evenly among the threads");
@@ -150,7 +151,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinCtas) ivfpq_scan_interleaved_
     idx_t* oI = partI + ((int64_t)q * gridDim.x + chunk) * k;
 
     CtaTopK<IdT> top;
-    top.init(listMem, ctl, LIST, k, kWarps);
+    top.init(listMem, ctl, LIST, k, kScanWarps);
     const unsigned sbase = (unsigned)__cvta_generic_to_shared(lut);
     if (SBASE >= 0 && sbase != (unsigned)SBASE)
         __trap(); // compiled for another shared-window base: refuse to read the wrong addresses
@@ -293,7 +294,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinCtas) ivfpq_scan_interleaved_
 
     const int pBegin = chunk * probesPerCta;
     const int pEnd = min(nprobe, pBegin + probesPerCta);
-    int base = 0; // work units dealt so far (identical in every warp): unit i belongs to warp i % kWarps
+    int base = 0; // work units dealt so far (identical in every warp): unit i belongs to warp i % kScanWarps
     if (IS_L2) {
         for (int p0 = pBegin; p0 < pEnd; p0 += 2) {
             idx_t l[2];
@@ -365,67 +366,17 @@ __global__ void __launch_bounds__(kWarps * 32, kMinCtas) ivfpq_scan_interleaved_
                 }
             }
             __syncthreads();
-            if (!ROLL) {
 #pragma unroll 1
-                for (int s = 0; s < 2; s++) {
-                    if (len[s] == 0)
-                        continue;
-                    const uint8_t* codes = arenaCodes + ls[s] * (int64_t)M;
-                    const int ngroups = (len[s] + 31) >> 5;
-                    const int units = (ngroups + kU - 1) / kU;
-                    const float add = PRECOMP ? t1s[s] : 0.f;
-                    for (int u = (warp - base) & (kWarps - 1); u < units; u += kWarps)
-                        scanUnit(s, codes, ngroups, u * kU, len[s], ls[s], add);
-                    base += units;
-                }
-            } else {
-                // Rolling prefetch: this warp's units of the pair form one stream; as soon as the lookups of a
-                // register slot are done the slot is refilled with the same slot of the warp's NEXT unit, so
-                // ~4 KB of code loads stay in flight per warp while it computes (no extra registers).
-                const int ng0 = (len[0] + 31) >> 5, ng1 = (len[1] + 31) >> 5;
-                const int un0 = (ng0 + kU - 1) / kU, un1 = (ng1 + kU - 1) / kU;
-                const uint8_t* c0 = arenaCodes + ls[0] * (int64_t)M;
-                const uint8_t* c1 = arenaCodes + ls[1] * (int64_t)M;
-                // stream position i = 0, 1, ...: global unit index gu = first + i * kWarps over [0, un0 + un1)
-                int gu = (warp - base) & (kWarps - 1);
-                const int total = un0 + un1;
-                uint4 cur[kU][H];
-                if (gu < total) {
-                    const bool in1 = gu >= un0;
-                    const uint8_t* cc = in1 ? c1 : c0;
-                    const int ng = in1 ? ng1 : ng0;
-                    const int g0 = (in1 ? gu - un0 : gu) * kU;
-#pragma unroll
-                    for (int u = 0; u < kU; u++)
-                        loadGroup(cc, min(g0 + u, ng - 1), cur[u]);
-                }
-                for (; gu < total; gu += kWarps) {
-                    const bool in1 = gu >= un0;
-                    const int ng = in1 ? ng1 : ng0;
-                    const int g0 = (in1 ? gu - un0 : gu) * kU;
-                    const int ln = in1 ? len[1] : len[0];
-                    const int64_t lsx = in1 ? ls[1] : ls[0];
-                    const float add = PRECOMP ? (in1 ? t1s[1] : t1s[0]) : 0.f;
-                    const unsigned Pbase = (t4 | (in1 ? 0x80u : 0u)) * 0x010101u;
-                    // next unit of this warp
-                    const int gn = gu + kWarps;
-                    const bool has = gn < total;
-                    const bool nin1 = gn >= un0;
-                    const uint8_t* nc = nin1 ? c1 : c0;
-                    const int nng = nin1 ? ng1 : ng0;
-                    const int ng0n = (nin1 ? gn - un0 : gn) * kU;
-                    top.refresh();
-#pragma unroll
-                    for (int u = 0; u < kU; u++) {
-                        const float sum = groupSum(cur[u], Pbase);
-                        if (has)
-                            loadGroup(nc, min(ng0n + u, nng - 1), cur[u]); // slot u is free again: refill it
-                        const int v = (g0 + u) * 32 + lane;
-                        const float key = (IS_L2 && !PRECOMP) ? sum : sum + add;
-                        top.add(g0 + u < ng && v < ln, key, (IdT)(lsx + v));
-                    }
-                }
-                base += total;
+            for (int s = 0; s < 2; s++) {
+                if (len[s] == 0)
+                    continue;
+                const uint8_t* codes = arenaCodes + ls[s] * (int64_t)M;
+                const int ngroups = (len[s] + 31) >> 5;
+                const int units = (ngroups + kU - 1) / kU;
+                const float add = PRECOMP ? t1s[s] : 0.f;
+                for (int u = (warp - base) & (kScanWarps - 1); u < units; u += kScanWarps)
+                    scanUnit(s, codes, ngroups, u * kU, len[s], ls[s], add);
+                base += units;
             }
         }
     } else {
@@ -441,7 +392,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinCtas) ivfpq_scan_interleaved_
             const int ngroups = (len + 31) >> 5;
             const int units = (ngroups + kU - 1) / kU;
             const float add = -coarseDis[(int64_t)q * nprobe + p];
-            for (int u = (warp - base) & (kWarps - 1); u < units; u += kWarps)
+            for (int u = (warp - base) & (kScanWarps - 1); u < units; u += kScanWarps)
                 scanUnit(0, codes, ngroups, u * kU, len, ls, add);
             base += units;
         }
@@ -526,49 +477,6 @@ void runIvfPqListFromInterleaved(const uint8_t* listCodes, int64_t len, int M, u
     CUDA_CHECK_LAST();
 }
 
-template <int M, bool IS_L2, bool PRECOMP, typename IdT, int kWarps, int kU, int kMinCtas, bool ROLL, int SBASE>
-static void launchScanV(
-        dim3 grid,
-        size_t smem,
-        cudaStream_t stream,
-        const float* Q,
-        int d,
-        const idx_t* probes,
-        const float* coarseDis,
-        int nprobe,
-        int probesPerCta,
-        const float* coarse,
-        const float* pqT,
-        const float* term2,
-        const int64_t* listStart,
-        const int* listLen,
-        const uint8_t* codes,
-        const idx_t* ids,
-        int k,
-        int LIST,
-        float* partD,
-        idx_t* partI) {
-    auto kern = ivfpq_scan_interleaved_kernel<M, IS_L2, PRECOMP, IdT, kWarps, kU, kMinCtas, ROLL, SBASE>;
-    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    KernelTiming::begin("ivfpq_scan", stream);
-    kern<<<grid, kWarps * 32, smem, stream>>>(
-            Q, d, probes, coarseDis, nprobe, probesPerCta, coarse, pqT, term2, listStart, listLen, codes, ids, k, LIST,
-            partD, partI);
-    KernelTiming::end("ivfpq_scan", stream);
-    CUDA_CHECK_LAST();
-}
-
-// launch shapes (FB200_PQ_CFG selects one for A/B runs)
-//   0: 16 warps, 4 KB of codes in flight per warp, 2 CTAs/SM (64 registers)
-//   1: 16 warps, 2 KB per warp, 3 CTAs/SM (42 registers)      2: 32 warps, 2 KB per warp, 2 CTAs/SM (32 registers)
-static int scanConfig() {
-    static const int cfg = getenv("FB200_PQ_CFG") ? atoi(getenv("FB200_PQ_CFG")) : 0;
-    return cfg;
-}
-static int scanWarps() {
-    return scanConfig() == 2 ? 32 : 16;
-}
-
 __global__ void smem_base_probe_kernel(unsigned* out) {
     extern __shared__ __align__(16) unsigned char probe_raw[];
     if (threadIdx.x == 0)
@@ -598,26 +506,39 @@ static int probedSmemBase(int device, cudaStream_t stream) {
     return (int)h;
 }
 
-template <int M, bool IS_L2, bool PRECOMP, typename IdT, typename... Args>
-static void launchScan(int smemBase, Args... args) {
-    constexpr int U = M == 32 ? 4 : 8; // groups per unit at 4 KB per warp
-    if (smemBase != kExpectedSmemBase) { // unknown shared-window base: generic addressing
-        launchScanV<M, IS_L2, PRECOMP, IdT, 16, U, 2, false, -1>(args...);
-        return;
-    }
-    switch (scanConfig()) {
-        case 1:
-            launchScanV<M, IS_L2, PRECOMP, IdT, 16, U / 2, 3, false, kExpectedSmemBase>(args...);
-            break;
-        case 2:
-            launchScanV<M, IS_L2, PRECOMP, IdT, 32, U / 2, 2, false, kExpectedSmemBase>(args...);
-            break;
-        case 3:
-            launchScanV<M, IS_L2, PRECOMP, IdT, 16, U, 2, true, kExpectedSmemBase>(args...);
-            break;
-        default:
-            launchScanV<M, IS_L2, PRECOMP, IdT, 16, U, 2, false, kExpectedSmemBase>(args...);
-    }
+template <int M, bool IS_L2, bool PRECOMP, typename IdT>
+static void launchScan(
+        int smemBase,
+        dim3 grid,
+        size_t smem,
+        cudaStream_t stream,
+        const float* Q,
+        int d,
+        const idx_t* probes,
+        const float* coarseDis,
+        int nprobe,
+        int probesPerCta,
+        const float* coarse,
+        const float* pqT,
+        const float* term2,
+        const int64_t* listStart,
+        const int* listLen,
+        const uint8_t* codes,
+        const idx_t* ids,
+        int k,
+        int LIST,
+        float* partD,
+        idx_t* partI) {
+    // any other shared-window base than the expected one: generic addressing
+    auto kern = smemBase == kExpectedSmemBase ? ivfpq_scan_interleaved_kernel<M, IS_L2, PRECOMP, IdT, kExpectedSmemBase>
+                                              : ivfpq_scan_interleaved_kernel<M, IS_L2, PRECOMP, IdT, -1>;
+    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    KernelTiming::begin("ivfpq_scan", stream);
+    kern<<<grid, kScanWarps * 32, smem, stream>>>(
+            Q, d, probes, coarseDis, nprobe, probesPerCta, coarse, pqT, term2, listStart, listLen, codes, ids, k, LIST,
+            partD, partI);
+    KernelTiming::end("ivfpq_scan", stream);
+    CUDA_CHECK_LAST();
 }
 
 void runIvfPqScanInterleaved(
@@ -649,7 +570,6 @@ void runIvfPqScanInterleaved(
     const int LIST = std::max(CtaTopK<int>::BUF, next_pow2(k)); // a sorted buffer (<= BUF entries) is merged into the list
     const bool wide = arenaElems >= (int64_t(1) << 31) - 1; // arena positions need 64-bit list ids
     const int smemBase = probedSmemBase(device, stream);
-    const int kScanWarps = smemBase == kExpectedSmemBase ? scanWarps() : 16;
     const size_t listBytes = wide ? CtaTopK<long long>::bytes(LIST, kScanWarps) : CtaTopK<int>::bytes(LIST, kScanWarps);
     size_t smem = sizeof(float) * 256 * kLutSlots + round_up(sizeof(float) * 2 * d, 16) + 16 + listBytes;
     FB_THROW_IF_NOT_MSG(smem <= 220 * 1024, "LUT + top-k lists do not fit shared memory");

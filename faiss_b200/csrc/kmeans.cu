@@ -3,15 +3,9 @@
 // The reference runs Lloyd's update on the CPU every iteration (compute_centroids,
 // faiss/impl/ClusteringHelpers.cpp:101-172: every OpenMP thread scans all n assignments) after
 // re-uploading the training set for the GPU assignment step.  Here the training set stays in HBM;
-// assignment is the Flat k=1 kernel and the update below is a privatised reduction:
-//   * small codebooks (k*d floats fit in shared memory, e.g. the 256 x dsub PQ codebooks): each
-//     block accumulates its slice of points into a shared-memory copy with shared atomics and
-//     flushes once with global RED;
-//   * large codebooks (IVF coarse centroids): one warp per point, lanes over dimensions, global
-//     RED.ADD.F32 (low contention: points hit k >= thousands of rows).
+// assignment is the Flat k=1 kernel and the update sorts the points by assignment, then adds each
+// centroid's points in index order, so the sums are bit-reproducible run to run.
 #include <cub/cub.cuh>
-
-#include <cstdlib>
 
 #include "kernels.h"
 #include "select.cuh"
@@ -211,12 +205,13 @@ void runKmeansAccumulate(
         cudaStream_t stream) {
     if (n == 0)
         return;
-    // FB200_KMEANS_ATOMIC=1 keeps the older atomic kernels (timing comparisons only; not order-deterministic)
-    static const bool atomicPath = getenv("FB200_KMEANS_ATOMIC") && atoi(getenv("FB200_KMEANS_ATOMIC")) != 0;
-    if (!atomicPath && n < (int64_t(1) << 31)) {
+    if (n < (int64_t(1) << 31)) {
         runKmeansAccumulateSorted(x, assign, n, d, k, sums, counts, stream);
         return;
     }
+    // n >= 2^31 exceeds the radix sort's int item count: atomic accumulation, not order-deterministic.
+    // Codebooks whose k*d floats fit in shared memory (e.g. the 256 x dsub PQ codebooks) are accumulated
+    // per block with shared atomics and flushed once; larger ones take one warp per point with global RED.
     size_t smem = sizeof(float) * ((size_t)k * d + k);
     if (smem <= 64 * 1024) {
         int64_t ppb = std::max<int64_t>(256, ceil_div(n, 132 * 4));
