@@ -4,8 +4,9 @@
 //   warps 0-7 : two consumer warpgroups.  A work unit is one 128-query tile; warpgroup g owns its query rows
 //               64 g .. 64 g + 63.  For every database tile it issues wgmma.m64n256k16 (fp16 operands straight
 //               from the 128B-swizzled shared-memory stages, fp32 accumulators in registers: 128 per thread),
-//               waits for them, hands the stage back and filters its own accumulator fragment (below).  A
-//               warpgroup's own MMAs and filter do not overlap; the two warpgroups share the ring without
+//               waits for them, hands the stage back and filters its own accumulator fragment (below).  At
+//               112 < d <= 128 the tile's MMAs run as two N = 128 halves, and the filter of the first half overlaps
+//               the MMAs of the second; otherwise a warpgroup's own MMAs and filter do not overlap.  The two warpgroups share the ring without
 //               synchronising with each other, so one's tensor work can overlap the other's filter.  Survivors (rare) are appended with plain stores to a thread-private candidate segment;
 //               scores never reach HBM.
 //   warp 8    : TMA producer -- the unit's query tile once, then database tiles (256 rows x dpad fp16,
@@ -266,40 +267,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
             if (SELF && pp + 1 < pe)
                 minbNext = __ldg(p.tileMinBias + t);
 
-            // ---- scores of the tile: acc = Q[64 rows] . Y[256 rows]^T
-            const int stagesPerTile = p.ksplit ? p.KB : 1;
-#pragma unroll 1
-            for (int kb0 = 0; kb0 < stagesPerTile; kb0++) {
-                ptx::mbar_wait(&y_full[ys], yphase);
-                const uint32_t yaddr = sYaddr + (uint32_t)ys * (uint32_t)stageBytes;
-                // K-steps of this stage (d = 96: 6 of the 8 K-steps of the padded tile -- a quarter of the tensor
-                // work is zeros otherwise)
-                const int ks0 = p.ksplit ? 4 * kb0 : 0;
-                const int ks1 = p.ksplit ? min(p.kSteps, ks0 + 4) : p.kSteps;
-                ptx::wgmma_fence();
-#pragma unroll 1
-                for (int ks = ks0; ks < ks1; ks++) {
-                    const int kb = ks >> 2, k4 = ks & 3;
-                    const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + kb * qkb + k4 * 32);
-                    const uint64_t db = ptx::make_smem_desc_sw128(yaddr + (p.ksplit ? 0 : kb * ykb) + k4 * 32);
-                    ptx::wgmma_m64n256k16_f16_ss(acc, da, db, ks != 0 ? 1u : 0u);
-                }
-                ptx::wgmma_commit();
-                ptx::wgmma_wait_all();
-                __syncwarp();
-                if (lane == 0) // this warp's share of the stage has been read
-                    ptx::mbar_arrive(&y_empty[ys]);
-                if (++ys == p.yStages) {
-                    ys = 0;
-                    yphase ^= 1;
-                }
-            }
-
-            // ---- filter: two rows x two 32-element chunks (128 columns each)
+            // filter of the tile's columns 128 c .. 128 c + 127 (acc[64 c .. 64 c + 63]) for both of the thread's rows
+            auto filterHalf = [&](int c) {
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-#pragma unroll
-                for (int c = 0; c < 2; c++) {
+                for (int h = 0; h < 2; h++) {
                     float r[32];
 #pragma unroll
                     for (int e = 0; e < 32; e++)
@@ -309,7 +280,70 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
                     else
                         epi_filter32<DUMP, SELF>(p, r, q0, colBase + 128 * c, inv, thr0, slack0, maxb, buf0, cnt0, minb);
                 }
+            };
+
+            // ---- scores of the tile: acc = Q[64 rows] . Y[256 rows]^T
+            if (!p.ksplit && p.kSteps == 2 * kKBlock / 16) {
+                // 112 < d <= 128, one stage per tile: two N = 128 halves committed separately, so that the filter of
+                // columns 0-127 runs while the tensor cores still work on columns 128-255 (otherwise a warpgroup's
+                // filter waits for all of its MMAs).  The K-step count must be a compile-time constant here: with a
+                // run-time count ptxas cannot tell which group is still in flight and serialises every MMA.
+                ptx::mbar_wait(&y_full[ys], yphase);
+                const uint32_t yaddr = sYaddr + (uint32_t)ys * (uint32_t)stageBytes;
+#pragma unroll
+                for (int c = 0; c < 2; c++) {
+                    ptx::wgmma_fence(); // each half is its own wgmma pipeline stage
+#pragma unroll
+                    for (int ks = 0; ks < 2 * kKBlock / 16; ks++) {
+                        const int kb = ks >> 2, k4 = ks & 3;
+                        const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + kb * qkb + k4 * 32);
+                        // database rows 128 c .. 128 c + 127 start 16 KB (whole swizzle atoms) into the K-block
+                        const uint64_t db = ptx::make_smem_desc_sw128(yaddr + kb * ykb + c * (ykb / 2) + k4 * 32);
+                        ptx::wgmma_m64n128k16_f16_ss(acc + 64 * c, da, db, ks != 0 ? 1u : 0u);
+                    }
+                    ptx::wgmma_commit();
+                }
+                ptx::wgmma_wait_all_but_one(); // columns 0-127 are final
+                filterHalf(0);
+                ptx::wgmma_wait_all();
+                __syncwarp();
+                if (lane == 0) // this warp's share of the stage has been read
+                    ptx::mbar_arrive(&y_empty[ys]);
+                if (++ys == p.yStages) {
+                    ys = 0;
+                    yphase ^= 1;
+                }
+            } else {
+                const int stagesPerTile = p.ksplit ? p.KB : 1;
+#pragma unroll 1
+                for (int kb0 = 0; kb0 < stagesPerTile; kb0++) {
+                    ptx::mbar_wait(&y_full[ys], yphase);
+                    const uint32_t yaddr = sYaddr + (uint32_t)ys * (uint32_t)stageBytes;
+                    // K-steps of this stage (d = 96: 6 of the 8 K-steps of the padded tile -- a quarter of the tensor
+                    // work is zeros otherwise)
+                    const int ks0 = p.ksplit ? 4 * kb0 : 0;
+                    const int ks1 = p.ksplit ? min(p.kSteps, ks0 + 4) : p.kSteps;
+                    ptx::wgmma_fence();
+#pragma unroll 1
+                    for (int ks = ks0; ks < ks1; ks++) {
+                        const int kb = ks >> 2, k4 = ks & 3;
+                        const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + kb * qkb + k4 * 32);
+                        const uint64_t db = ptx::make_smem_desc_sw128(yaddr + (p.ksplit ? 0 : kb * ykb) + k4 * 32);
+                        ptx::wgmma_m64n256k16_f16_ss(acc, da, db, ks != 0 ? 1u : 0u);
+                    }
+                    ptx::wgmma_commit();
+                    ptx::wgmma_wait_all();
+                    __syncwarp();
+                    if (lane == 0) // this warp's share of the stage has been read
+                        ptx::mbar_arrive(&y_empty[ys]);
+                    if (++ys == p.yStages) {
+                        ys = 0;
+                        yphase ^= 1;
+                    }
+                }
+                filterHalf(0);
             }
+            filterHalf(1);
         }
         __syncwarp();
         if (lane == 0) // the query tile may be overwritten

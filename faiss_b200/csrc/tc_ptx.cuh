@@ -124,6 +124,10 @@ __device__ __forceinline__ void wgmma_commit() {
 __device__ __forceinline__ void wgmma_wait_all() {
     asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
+// all but the most recent committed group have completed
+__device__ __forceinline__ void wgmma_wait_all_but_one() {
+    asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+}
 // D[64 x 256, registers] (+)= A[smem desc, 64 x 16] * B[smem desc, 256 x 16]^T, fp16 inputs, fp32 accumulate,
 // both operands K-major.  Fragment of D held by thread t of the warpgroup (warp w = t / 32, lane l):
 //   d[4 j + 2 h + b] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + b]   (j < 32, h, b < 2)
@@ -159,6 +163,28 @@ __device__ __forceinline__ void wgmma_m64n256k16_f16_ss(float (&d)[128], uint64_
               "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
               "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
               "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+            : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
+// D[64 x 128, registers] (+)= A[smem desc, 64 x 16] * B[smem desc, 128 x 16]^T: the same fragment layout as above with
+// j < 16.  d points into the caller's accumulator array at a compile-time offset (it stays in registers).
+__device__ __forceinline__ void wgmma_m64n128k16_f16_ss(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %66, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+            "%64, %65, p, 1, 1, 0, 0;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
             : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
