@@ -20,6 +20,22 @@ from ._lib import lib, check, FaissError  # noqa: F401  (loading fails loudly)
 METRIC_INNER_PRODUCT = 0
 METRIC_L2 = 1
 
+# faiss::ScalarQuantizer::QuantizerType (faiss/impl/ScalarQuantizer.h:27-40); GpuIndexIVFScalarQuantizer
+# accepts QT_8bit ... QT_6bit, as the reference GPU index does
+QT_8bit = 0
+QT_4bit = 1
+QT_8bit_uniform = 2
+QT_4bit_uniform = 3
+QT_fp16 = 4
+QT_8bit_direct = 5
+QT_6bit = 6
+QT_bf16 = 7
+# faiss::ScalarQuantizer::RangeStat (faiss/impl/ScalarQuantizer.h:66-71)
+RS_minmax = 0
+RS_meanstd = 1
+RS_quantiles = 2
+RS_optim = 3
+
 _c_f = ctypes.POINTER(ctypes.c_float)
 _c_i64 = ctypes.POINTER(ctypes.c_int64)
 _c_u8 = ctypes.POINTER(ctypes.c_uint8)
@@ -532,6 +548,70 @@ class GpuIndexIVFPQ(GpuIndexIVF):
 
     def setPrecomputedCodes(self, enable):
         check(lib.faiss_GpuIndexIVFPQ_setPrecomputedCodes(self._h, int(bool(enable))))
+
+
+class GpuIndexIVFScalarQuantizer(GpuIndexIVF):
+    """faiss::gpu::GpuIndexIVFScalarQuantizer (faiss/gpu/GpuIndexIVFScalarQuantizer.h:30-139).
+
+    qtype is a ScalarQuantizer::QuantizerType (QT_8bit ... QT_6bit); trained parameters use the CPU's
+    ScalarQuantizer::trained layout, lists the CPU's ArrayInvertedLists bytes."""
+
+    def __init__(self, res, d, nlist, qtype=None, metric=METRIC_L2, encodeResidual=True, device=0, quantizer=None):
+        """quantizer: a GpuIndexFlat to share as the coarse quantiser, or None"""
+        super().__init__()
+        self._keep.append(res)
+        qtype = QT_8bit if qtype is None else int(qtype)
+        if quantizer is not None:
+            self._keep.append(quantizer)
+            check(
+                lib.faiss_GpuIndexIVFScalarQuantizer_new_with_quantizer(
+                    ctypes.byref(self._h), res._h, quantizer._h, int(d), ctypes.c_int64(nlist), qtype, int(metric),
+                    int(bool(encodeResidual)), int(device),
+                )
+            )
+            return
+        check(
+            lib.faiss_GpuIndexIVFScalarQuantizer_new(
+                ctypes.byref(self._h), res._h, int(d), ctypes.c_int64(nlist), qtype, int(metric),
+                int(bool(encodeResidual)), int(device),
+            )
+        )
+
+    def _code_size(self):
+        out = ctypes.c_size_t()
+        check(lib.faiss_GpuIndexIVFScalarQuantizer_code_size(self._h, ctypes.byref(out)))
+        return out.value
+
+    @property
+    def code_size(self):
+        return self._code_size()
+
+    @property
+    def qtype(self):
+        out = ctypes.c_int()
+        check(lib.faiss_GpuIndexIVFScalarQuantizer_qtype(self._h, ctypes.byref(out)))
+        return out.value
+
+    @property
+    def by_residual(self):
+        out = ctypes.c_int()
+        check(lib.faiss_GpuIndexIVFScalarQuantizer_by_residual(self._h, ctypes.byref(out)))
+        return bool(out.value)
+
+    def getTrained(self):
+        n = ctypes.c_size_t()
+        check(lib.faiss_GpuIndexIVFScalarQuantizer_get_trained(self._h, ctypes.cast(None, _c_f), ctypes.byref(n)))
+        out = np.empty(n.value, dtype=np.float32)
+        check(lib.faiss_GpuIndexIVFScalarQuantizer_get_trained(self._h, _ptr(out, _c_f), ctypes.byref(n)))
+        return out
+
+    def setTrained(self, t):
+        t = np.ascontiguousarray(t, dtype=np.float32).reshape(-1)
+        check(lib.faiss_GpuIndexIVFScalarQuantizer_set_trained(self._h, _ptr(t, _c_f), ctypes.c_size_t(t.size)))
+
+    def setRangeStat(self, rangestat, rangestat_arg=0.0):
+        """ScalarQuantizer::rangestat / rangestat_arg for train(); only RS_minmax trains on the GPU"""
+        check(lib.faiss_GpuIndexIVFScalarQuantizer_set_rangestat(self._h, int(rangestat), ctypes.c_float(rangestat_arg)))
 
 
 class IndexShards(Index):

@@ -514,6 +514,102 @@ int faiss_GpuIndexIVFPQ_setPrecomputedCodes(FaissGpuIndex* p, int enable) {
     CATCH_AND_HANDLE
 }
 
+// ---------------------------------------------------------------- GpuIndexIVFScalarQuantizer
+int faiss_GpuIndexIVFScalarQuantizer_new(
+        FaissGpuIndex** p,
+        FaissStandardGpuResources* r,
+        int d,
+        idx_t nlist,
+        int qtype,
+        FaissMetricType metric,
+        int encodeResidual,
+        int device) {
+    try {
+        GpuIndexIVFScalarQuantizerConfig c;
+        c.device = device;
+        auto res = RES(r);
+        auto* h = new FaissIndex_H{nullptr, res};
+        try {
+            h->index = new GpuIndexIVFScalarQuantizer(res, d, nlist, qtype, MT(metric), encodeResidual != 0, c);
+        } catch (...) {
+            delete h;
+            throw;
+        }
+        *p = h;
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexIVFScalarQuantizer_new_with_quantizer(
+        FaissGpuIndex** p,
+        FaissStandardGpuResources* r,
+        FaissGpuIndex* coarse,
+        int d,
+        idx_t nlist,
+        int qtype,
+        FaissMetricType metric,
+        int encodeResidual,
+        int device) {
+    try {
+        GpuIndexIVFScalarQuantizerConfig c;
+        c.device = device;
+        auto res = RES(r);
+        auto* h = new FaissIndex_H{nullptr, res};
+        try {
+            h->index = new GpuIndexIVFScalarQuantizer(
+                    res, AS<GpuIndexFlat>(coarse, "GpuIndexFlat"), d, nlist, qtype, MT(metric), encodeResidual != 0, c);
+        } catch (...) {
+            delete h;
+            throw;
+        }
+        *p = h;
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexIVFScalarQuantizer_set_trained(FaissGpuIndex* p, const float* t, size_t n) {
+    try {
+        AS<GpuIndexIVFScalarQuantizer>(p, "GpuIndexIVFScalarQuantizer")->setTrained(t, n);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexIVFScalarQuantizer_get_trained(const FaissGpuIndex* p, float* out, size_t* n) {
+    try {
+        FB_THROW_IF_NOT_MSG(n != nullptr, "null length pointer");
+        const auto& t = AS<GpuIndexIVFScalarQuantizer>(p, "GpuIndexIVFScalarQuantizer")->getTrained();
+        if (out)
+            std::copy(t.begin(), t.end(), out);
+        *n = t.size();
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexIVFScalarQuantizer_code_size(const FaissGpuIndex* p, size_t* out) {
+    try {
+        auto* i = AS<GpuIndexIVFScalarQuantizer>(p, "GpuIndexIVFScalarQuantizer");
+        *out = (size_t)GpuIndexIVFScalarQuantizer::codeSizeFor(i->qtype(), i->d);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexIVFScalarQuantizer_qtype(const FaissGpuIndex* p, int* out) {
+    try {
+        *out = AS<GpuIndexIVFScalarQuantizer>(p, "GpuIndexIVFScalarQuantizer")->qtype();
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexIVFScalarQuantizer_by_residual(const FaissGpuIndex* p, int* out) {
+    try {
+        *out = AS<GpuIndexIVFScalarQuantizer>(p, "GpuIndexIVFScalarQuantizer")->by_residual ? 1 : 0;
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexIVFScalarQuantizer_set_rangestat(FaissGpuIndex* p, int rangestat, float arg) {
+    try {
+        auto* i = AS<GpuIndexIVFScalarQuantizer>(p, "GpuIndexIVFScalarQuantizer");
+        FB_THROW_IF_NOT_MSG(rangestat >= 0 && rangestat <= 3, "invalid rangestat");
+        i->rangestat = rangestat;
+        i->rangestat_arg = arg;
+    }
+    CATCH_AND_HANDLE
+}
+
 // ---------------------------------------------------------------- IndexShards
 int faiss_IndexShards_new(FaissIndexShards** p, idx_t d) {
     return faiss_IndexShards_new_with_options(p, d, 0, 1);

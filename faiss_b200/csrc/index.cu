@@ -1650,27 +1650,39 @@ void trainProductQuantizer(
     }
 }
 
+const float* subsampleRowsDevice(
+        GpuResources* res,
+        int device,
+        idx_t& n,
+        int d,
+        idx_t nmax,
+        int64_t seed,
+        const float* xDev,
+        GpuMemoryReservation& hold,
+        cudaStream_t stream) {
+    if (n <= nmax)
+        return xDev;
+    std::vector<int> perm(n);
+    rand_perm(perm.data(), n, seed);
+    auto pd = res->temp(device, sizeof(int) * nmax);
+    CUDA_VERIFY(cudaMemcpyAsync(pd.data, perm.data(), sizeof(int) * nmax, cudaMemcpyHostToDevice, stream));
+    hold = res->device_alloc(device, sizeof(float) * nmax * d, AllocType::Other);
+    gather_rows_int_kernel<<<(unsigned)nmax, std::min(256, d), 0, stream>>>(xDev, pd.as<int>(), nmax, d, hold.as<float>());
+    CUDA_CHECK_LAST();
+    CUDA_VERIFY(cudaStreamSynchronize(stream));
+    n = nmax;
+    return hold.as<float>();
+}
+
 void GpuIndexIVFPQ::trainResidualQuantizer_(idx_t n, const float* xDev) {
     auto stream = stream_();
     GpuResources* res = resources_.get();
     const int device = config_.device;
     const int ksub = 256;
     // fvecs_maybe_subsample (faiss/utils/utils.cpp:464-489) with pq.cp.seed
-    const idx_t nmax = (idx_t)pq_cp.max_points_per_centroid * ksub;
     GpuMemoryReservation sub;
-    const float* x = xDev;
-    if (n > nmax) {
-        std::vector<int> perm(n);
-        rand_perm(perm.data(), n, pq_cp.seed);
-        auto pd = res->temp(device, sizeof(int) * nmax);
-        CUDA_VERIFY(cudaMemcpyAsync(pd.data, perm.data(), sizeof(int) * nmax, cudaMemcpyHostToDevice, stream));
-        sub = res->device_alloc(device, sizeof(float) * nmax * d, AllocType::Other);
-        gather_rows_int_kernel<<<(unsigned)nmax, std::min(256, d), 0, stream>>>(x, pd.as<int>(), nmax, d, sub.as<float>());
-        CUDA_CHECK_LAST();
-        CUDA_VERIFY(cudaStreamSynchronize(stream));
-        x = sub.as<float>();
-        n = nmax;
-    }
+    const float* x = subsampleRowsDevice(
+            res, device, n, d, (idx_t)pq_cp.max_points_per_centroid * ksub, pq_cp.seed, xDev, sub, stream);
     if (verbose)
         printf("computing residuals\n");
     auto assign = res->device_alloc(device, sizeof(idx_t) * n, AllocType::Other);
@@ -1733,6 +1745,211 @@ void GpuIndexIVFPQ::scanImpl_(
             resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np, quantizer->vectorsDevice(),
             pqCentroids_.data(), M_, lists_->dStart(), lists_->dLen(), lists_->codes(), lists_->ids(), k, metric_type,
             dDev, iDev, stream_());
+}
+
+// ------------------------------------------------------------------------------------------
+// GpuIndexIVFScalarQuantizer
+// ------------------------------------------------------------------------------------------
+static bool sqTypeSupported(int qtype) { // faiss/gpu/impl/GpuScalarQuantizer.cuh:20-33
+    return qtype >= SQ_QT_8bit && qtype <= SQ_QT_6bit;
+}
+static bool sqUniform(int qtype) {
+    return qtype == SQ_QT_8bit_uniform || qtype == SQ_QT_4bit_uniform;
+}
+
+int GpuIndexIVFScalarQuantizer::codeSizeFor(int qtype, int d) {
+    FB_THROW_IF_NOT_MSG(sqTypeSupported(qtype), "Unsupported scalar QuantizerType on GPU");
+    switch (qtype) {
+        case SQ_QT_4bit:
+        case SQ_QT_4bit_uniform:
+            return (d + 1) / 2;
+        case SQ_QT_6bit:
+            return (d * 6 + 7) / 8;
+        case SQ_QT_fp16:
+            return 2 * d;
+        default:
+            return d;
+    }
+}
+
+GpuIndexIVFScalarQuantizer::GpuIndexIVFScalarQuantizer(
+        std::shared_ptr<GpuResources> resources,
+        int dims,
+        idx_t nlist,
+        int qtype,
+        MetricType metric,
+        bool encodeResidual,
+        GpuIndexIVFScalarQuantizerConfig config)
+        : GpuIndexIVF(std::move(resources), dims, metric, nlist, codeSizeFor(qtype, dims), config),
+          by_residual(encodeResidual),
+          qtype_(qtype),
+          params_(resources_.get(), config.device, AllocType::Quantizer) {
+    // faiss/gpu/GpuIndexIVFScalarQuantizer.cu:97-124: the per-dimension decode tables live in shared memory
+    const size_t maxTable = 200 * 1024;
+    FB_THROW_IF_NOT_FMT(
+            ivfSqScanTableBytes(dims) <= maxTable,
+            "GpuIndexIVFScalarQuantizer: Insufficient shared memory available on the GPU with %d dimensions; "
+            "maximum dimensions possible is %d",
+            dims,
+            (int)((maxTable / sizeof(float) - 4) / 2));
+    if (trainedSize() == 0)
+        setTrained(nullptr, 0);
+}
+
+GpuIndexIVFScalarQuantizer::GpuIndexIVFScalarQuantizer(
+        std::shared_ptr<GpuResources> resources,
+        GpuIndexFlat* coarseQuantizer,
+        int dims,
+        idx_t nlist,
+        int qtype,
+        MetricType metric,
+        bool encodeResidual,
+        GpuIndexIVFScalarQuantizerConfig config)
+        : GpuIndexIVFScalarQuantizer(std::move(resources), dims, nlist, qtype, metric, encodeResidual, config) {
+    setQuantizer(coarseQuantizer);
+}
+
+size_t GpuIndexIVFScalarQuantizer::trainedSize() const {
+    switch (qtype_) {
+        case SQ_QT_8bit_uniform:
+        case SQ_QT_4bit_uniform:
+            return 2;
+        case SQ_QT_8bit:
+        case SQ_QT_4bit:
+        case SQ_QT_6bit:
+            return 2 * (size_t)d;
+        default:
+            return 0;
+    }
+}
+
+void GpuIndexIVFScalarQuantizer::setTrained(const float* t, size_t n) {
+    DeviceScope scope(config_.device);
+    FB_THROW_IF_NOT_FMT(n == trainedSize(), "scalar quantizer expects %zu trained values, got %zu", trainedSize(), n);
+    trained_.assign(t, t + n);
+    // host tables [4][d]: vmin | vdiff for the encoder (the CPU's values), m | b for the scan's folded decode
+    std::vector<float> h((size_t)4 * d);
+    float* vmin = h.data();
+    float* vdiff = vmin + d;
+    float* m = vdiff + d;
+    float* b = m + d;
+    const float levels = (qtype_ == SQ_QT_4bit || qtype_ == SQ_QT_4bit_uniform) ? 15.f : qtype_ == SQ_QT_6bit ? 63.f : 255.f;
+    for (int i = 0; i < d; i++) {
+        if (n == 0) { // fp16, 8bit_direct: the code is the value
+            vmin[i] = 0.f;
+            vdiff[i] = 1.f;
+            m[i] = 0.f;
+            b[i] = 1.f;
+            continue;
+        }
+        vmin[i] = sqUniform(qtype_) ? trained_[0] : trained_[i];
+        vdiff[i] = sqUniform(qtype_) ? trained_[1] : trained_[d + i];
+        b[i] = vdiff[i] / levels;
+        m[i] = vmin[i] + 0.5f * b[i];
+    }
+    auto stream = stream_();
+    params_.resize(h.size(), stream);
+    CUDA_VERIFY(cudaMemcpyAsync(params_.data(), h.data(), sizeof(float) * h.size(), cudaMemcpyHostToDevice, stream));
+    CUDA_VERIFY(cudaStreamSynchronize(stream));
+}
+
+// IndexIVF::train (faiss/IndexIVF.cpp:1296-1329) with train_encoder_num_vectors() = 100000
+// (faiss/IndexScalarQuantizer.cpp:158-160) and ScalarQuantizer::train, RS_minmax
+void GpuIndexIVFScalarQuantizer::train(idx_t n, const float* x) {
+    DeviceScope scope(config_.device);
+    if (this->is_trained) {
+        FB_THROW_IF_NOT(quantizer->is_trained && quantizer->ntotal == nlist);
+        return;
+    }
+    const size_t nt = trainedSize();
+    FB_THROW_IF_NOT_MSG(nt == 0 || rangestat == 0, "GpuIndexIVFScalarQuantizer: only RS_minmax training runs on the GPU");
+    auto stream = stream_();
+    GpuResources* res = resources_.get();
+    const int device = config_.device;
+    DeviceView<float> xv(res, device, x, (size_t)n * d, stream);
+    trainQuantizer_(n, xv.ptr);
+    if (nt > 0) {
+        FB_THROW_IF_NOT(n > 0);
+        GpuMemoryReservation sub;
+        idx_t ns = n;
+        const float* xs = subsampleRowsDevice(res, device, ns, d, 100000, 1234, xv.ptr, sub, stream);
+        GpuMemoryReservation resid;
+        if (by_residual) {
+            auto assign = res->temp(device, sizeof(idx_t) * ns);
+            auto dis = res->temp(device, sizeof(float) * ns);
+            resid = res->device_alloc(device, sizeof(float) * ns * d, AllocType::Other);
+            quantizer->searchDevice(ns, xs, 1, dis.as<float>(), assign.as<idx_t>());
+            runCalcResidual(xs, quantizer->vectorsDevice(), assign.as<idx_t>(), ns, d, resid.as<float>(), stream);
+            xs = resid.as<float>();
+        }
+        auto mm = res->temp(device, sizeof(float) * 2 * d);
+        runSqMinMax(xs, ns, d, mm.as<float>(), mm.as<float>() + d, stream);
+        std::vector<float> h((size_t)2 * d);
+        CUDA_VERIFY(cudaMemcpyAsync(h.data(), mm.data, sizeof(float) * 2 * d, cudaMemcpyDeviceToHost, stream));
+        CUDA_VERIFY(cudaStreamSynchronize(stream));
+        std::vector<float> t(nt);
+        // training.cpp:221-234 (uniform: one range over all n*d values) and :345-365 (per dimension)
+        if (sqUniform(qtype_)) {
+            float vmin = HUGE_VALF, vmax = -HUGE_VALF;
+            for (int j = 0; j < d; j++) {
+                vmin = std::min(vmin, h[j]);
+                vmax = std::max(vmax, h[d + j]);
+            }
+            const float vexp = (vmax - vmin) * rangestat_arg;
+            vmin -= vexp;
+            vmax += vexp;
+            t[0] = vmin;
+            t[1] = vmax - vmin;
+        } else {
+            for (int j = 0; j < d; j++) {
+                float vmin = h[j], vmax = h[d + j];
+                const float vexp = (vmax - vmin) * rangestat_arg;
+                vmin -= vexp;
+                vmax += vexp;
+                t[j] = vmin;
+                t[d + j] = vmax - vmin;
+            }
+        }
+        setTrained(t.data(), nt);
+    }
+    this->is_trained = true;
+}
+
+void GpuIndexIVFScalarQuantizer::addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) {
+    auto stream = stream_();
+    FB_THROW_IF_NOT_MSG(params_.size() == (size_t)4 * d, "scalar quantizer not trained");
+    auto assign = resources_->temp(config_.device, sizeof(idx_t) * n);
+    auto dis = resources_->temp(config_.device, sizeof(float) * n);
+    auto codes = resources_->temp(config_.device, (size_t)n * lists_->codeSize());
+    quantizer->searchDevice(n, xDev, 1, dis.as<float>(), assign.as<idx_t>());
+    const float* src = xDev;
+    GpuMemoryReservation resid;
+    if (by_residual) { // IndexIVFScalarQuantizer::encode_vectors (faiss/IndexScalarQuantizer.cpp:162-200)
+        resid = resources_->temp(config_.device, sizeof(float) * n * d);
+        runCalcResidual(xDev, quantizer->vectorsDevice(), assign.as<idx_t>(), n, d, resid.as<float>(), stream);
+        src = resid.as<float>();
+    }
+    runSqEncode(src, n, d, qtype_, lists_->codeSize(), params_.data(), params_.data() + d, codes.as<uint8_t>(), stream);
+    lists_->append(n, codes.as<uint8_t>(), idsDev, assign.as<idx_t>(), stream);
+    this->ntotal += n;
+}
+
+void GpuIndexIVFScalarQuantizer::scanImpl_(
+        idx_t n,
+        const float* xDev,
+        const idx_t* probes,
+        const float* coarseDis,
+        int np,
+        int k,
+        float* dDev,
+        idx_t* iDev) const {
+    FB_THROW_IF_NOT_MSG(params_.size() == (size_t)4 * d, "scalar quantizer not trained");
+    const bool needCentroids = by_residual && metric_type == METRIC_L2;
+    runIvfSqScan(
+            resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np,
+            needCentroids ? quantizer->vectorsDevice() : nullptr, by_residual, qtype_, params_.data() + 2 * d,
+            lists_->dStart(), lists_->dLen(), lists_->codes(), lists_->ids(), lists_->arenaElems(), lists_->codeSize(), k,
+            metric_type, dDev, iDev, stream_());
 }
 
 // ------------------------------------------------------------------------------------------

@@ -630,6 +630,68 @@ class GpuIndexIVFPQ : public GpuIndexIVF {
     DeviceVector<float> pqCentroidsT_; // [256][M][dsub] (LUT build reads it coalesced)
 };
 
+struct GpuIndexIVFScalarQuantizerConfig : GpuIndexIVFConfig { // faiss/gpu/GpuIndexIVFScalarQuantizer.h:20-27
+    bool interleavedLayout = true; // accepted, not honoured: lists keep the CPU's [len][code_size] layout
+};
+
+// faiss::gpu::GpuIndexIVFScalarQuantizer (faiss/gpu/GpuIndexIVFScalarQuantizer.h:30-139); training and encoding
+// follow the CPU IndexIVFScalarQuantizer (faiss/IndexScalarQuantizer.cpp:122-215, faiss/IndexIVF.cpp:1296-1329)
+class GpuIndexIVFScalarQuantizer : public GpuIndexIVF {
+   public:
+    GpuIndexIVFScalarQuantizer(
+            std::shared_ptr<GpuResources> resources,
+            int dims,
+            idx_t nlist,
+            int qtype,
+            MetricType metric = METRIC_L2,
+            bool encodeResidual = true,
+            GpuIndexIVFScalarQuantizerConfig config = GpuIndexIVFScalarQuantizerConfig());
+    GpuIndexIVFScalarQuantizer(
+            std::shared_ptr<GpuResources> resources,
+            GpuIndexFlat* coarseQuantizer,
+            int dims,
+            idx_t nlist,
+            int qtype,
+            MetricType metric = METRIC_L2,
+            bool encodeResidual = true,
+            GpuIndexIVFScalarQuantizerConfig config = GpuIndexIVFScalarQuantizerConfig());
+
+    // ScalarQuantizer::code_size (faiss/impl/ScalarQuantizer.cpp:451-520)
+    static int codeSizeFor(int qtype, int d);
+    int qtype() const {
+        return qtype_;
+    }
+    bool by_residual;
+    // ScalarQuantizer::rangestat / rangestat_arg: train() implements RS_minmax (0) only
+    int rangestat = 0;
+    float rangestat_arg = 0.f;
+
+    void train(idx_t n, const float* x) override;
+    // ScalarQuantizer::trained: [vmin, vdiff] (uniform types), [vmin[d], vdiff[d]] (non-uniform), empty (fp16, direct)
+    void setTrained(const float* t, size_t n);
+    const std::vector<float>& getTrained() const {
+        return trained_;
+    }
+    size_t trainedSize() const; // the length setTrained expects
+
+   protected:
+    bool quantizerOnlyTraining_() const override {
+        return trainedSize() == 0;
+    }
+    void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) override;
+    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
+
+    int qtype_;
+    std::vector<float> trained_;
+    DeviceVector<float> params_; // [4][d]: vmin | vdiff (encode) | m | b (scan decode x = m + b * code)
+};
+
+// fvecs_maybe_subsample (faiss/utils/utils.cpp:464-489) on a device matrix: when n > nmax, the rows
+// rand_perm(n, seed)[0:nmax] are gathered into `hold` and n becomes nmax; returns the rows to use
+const float* subsampleRowsDevice(
+        GpuResources* res, int device, idx_t& n, int d, idx_t nmax, int64_t seed, const float* xDev,
+        GpuMemoryReservation& hold, cudaStream_t stream);
+
 // ------------------------------------------------------------------------------------------
 // IndexShards
 // ------------------------------------------------------------------------------------------

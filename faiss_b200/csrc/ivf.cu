@@ -15,6 +15,7 @@
 
 #include <cfloat>
 
+#include "ivf_scan.cuh"
 #include "kernels.h"
 #include "select.cuh"
 
@@ -279,51 +280,6 @@ void runIvfScatter(
 }
 
 // ------------------------------------------------------------------------------------------
-// block-level helper: merge the per-warp lists of a block into warp 0's list, write k results
-// ------------------------------------------------------------------------------------------
-constexpr int kScanWarps = 4;
-constexpr int kScanBuf = 64;
-
-template <typename IdT>
-__device__ void block_merge_and_write(
-        WarpTopK<IdT>& w,
-        int warp,
-        unsigned char* smemLists,
-        size_t perWarp,
-        int LIST,
-        int k,
-        const idx_t* __restrict__ ids, // list ids (arena + listStart), may be null
-        float addToKey,
-        float* __restrict__ outD,
-        idx_t* __restrict__ outI) {
-    w.finish();
-    __syncthreads();
-    if (warp == 0) {
-        for (int ow = 1; ow < kScanWarps; ow++) {
-            const float* ok = reinterpret_cast<const float*>(smemLists + perWarp * ow);
-            const IdT* oi = reinterpret_cast<const IdT*>(smemLists + perWarp * ow + sizeof(float) * (LIST + kScanBuf));
-            for (int e0 = 0; e0 < k; e0 += 32) {
-                int e = e0 + lane_id();
-                bool valid = e < k;
-                float key = valid ? ok[e] : 0.f;
-                IdT id = valid ? oi[e] : 0;
-                valid = valid && id != IdLimits<IdT>::max();
-                if (!__any_sync(kFullMask, valid && key <= w.thr))
-                    break; // sorted: nothing further can enter
-                w.add(valid, key, id);
-            }
-        }
-        w.finish();
-        for (int j = lane_id(); j < k; j += 32) {
-            IdT id = w.q.ids[j];
-            bool ok2 = id != IdLimits<IdT>::max();
-            outD[j] = ok2 ? w.q.keys[j] + addToKey : CUDART_INF_F;
-            outI[j] = ok2 ? (ids ? ids[id] : (idx_t)id) : -1;
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------
 // IVF-Flat scan: block per (query, chunk of its probes).  The per-warp top-k lists and thresholds live
 // across the probes of the chunk (list ids = arena positions), so threshold passes grow with
 // log(vectors per CTA) instead of with the number of (query, probe) pairs.
@@ -461,9 +417,6 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfflat_scan_kernel(
     }
     block_merge_and_write<IdT>(w, warp, lists, perWarp, LIST, k, arenaIds, 0.f, oD, oI);
 }
-
-void runMergeTopKKeyspace(
-        const float*, const idx_t*, int64_t, int, int, int, MetricType, int64_t, float*, idx_t*, cudaStream_t);
 
 // CTAs per query: 1 when the queries alone fill the machine several times over, else the probes are
 // split so that ~8 CTAs per SM exist

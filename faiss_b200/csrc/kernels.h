@@ -284,6 +284,67 @@ void runIvfPqScan(
         idx_t* outI,
         cudaStream_t stream);
 
+// ---------------------------------------------------------------- ivfsq_scan.cu
+// ScalarQuantizer::QuantizerType values (faiss/impl/ScalarQuantizer.h:27-34) the GPU index accepts
+enum SqQuantizerType {
+    SQ_QT_8bit = 0,
+    SQ_QT_4bit = 1,
+    SQ_QT_8bit_uniform = 2,
+    SQ_QT_4bit_uniform = 3,
+    SQ_QT_fp16 = 4,
+    SQ_QT_8bit_direct = 5,
+    SQ_QT_6bit = 6,
+};
+
+// per-dimension min / max over n rows (RS_minmax, faiss/impl/scalar_quantizer/training.cpp:209-383); outputs
+// are device arrays [d]
+void runSqMinMax(const float* x, int64_t n, int d, float* vminOut, float* vmaxOut, cudaStream_t stream);
+
+// ScalarQuantizer encode (quantizers.h:66-150, codecs.h): codes [n][codeSize], byte-exact with the CPU.
+// vmin / vdiff are per dimension (uniform types: the one range repeated); unused for fp16 / 8bit_direct.
+void runSqEncode(
+        const float* x,
+        int64_t n,
+        int d,
+        int qtype,
+        int codeSize,
+        const float* vmin,
+        const float* vdiff,
+        uint8_t* codes,
+        cudaStream_t stream);
+
+// shared-memory bytes of the per-(query, probe) decode tables of the IVF-SQ scan
+size_t ivfSqScanTableBytes(int d);
+
+// IVF-SQ list scan (role of the reference GPU IVFFlatScan with a scalar-quantiser codec): decode folded into
+// per-(query, probe) tables, lists in the CPU's [len][codeSize] layout.  decodeMB = m[d] | b[d] with the
+// decode x_i = m_i + b_i * code_i.  Distance forms follow faiss/impl/scalar_quantizer/scanners.h:44-135:
+// L2 on the residual q - c_list when byResidual; IP adds the coarse distance to every distance when byResidual.
+void runIvfSqScan(
+        GpuResources* res,
+        int device,
+        const float* Q,
+        int64_t nq,
+        int d,
+        const idx_t* probes,
+        const float* coarseDis,
+        int nprobe,
+        const float* coarseCentroids,
+        bool byResidual,
+        int qtype,
+        const float* decodeMB,
+        const int64_t* listStart,
+        const int* listLen,
+        const uint8_t* arenaCodes,
+        const idx_t* arenaIds,
+        int64_t arenaElems,
+        int codeSize,
+        int k,
+        MetricType metric,
+        float* outD,
+        idx_t* outI,
+        cudaStream_t stream);
+
 // ---- "rotated, interleaved-by-32" PQ code layout (native storage for M % 16 == 0, M <= 32) ----
 // List-relative vector v = 32*g + t is stored in group g; byte position j of the vector holds
 // code[(j + t) % M] and lives at  g*32*M + (j/16)*512 + t*16 + (j%16).  A warp therefore loads a

@@ -149,6 +149,22 @@ FB200_API int faiss_GpuIndexIVFPQ_set_pq_clustering(FaissGpuIndex* index, int ni
    rule (<= 2 GiB, faiss/IndexIVFPQ.cpp:345) for indexes with short lists.  Results agree to fp32 rounding. */
 FB200_API int faiss_GpuIndexIVFPQ_setPrecomputedCodes(FaissGpuIndex* index, int enable);
 
+/* ---- GpuIndexIVFScalarQuantizer (faiss/gpu/GpuIndexIVFScalarQuantizer.h:30-139) ----
+   qtype: ScalarQuantizer::QuantizerType 0-6 (QT_8bit, QT_4bit, QT_8bit_uniform, QT_4bit_uniform, QT_fp16,
+   QT_8bit_direct, QT_6bit); any other type fails with "Unsupported scalar QuantizerType on GPU".
+   trained: ScalarQuantizer::trained ([vmin, vdiff] uniform, [vmin[d], vdiff[d]] non-uniform, empty for fp16 and
+   8bit_direct).  get_trained writes *n values to out when out is non-NULL; pass NULL to query the length.
+   Lists, nprobe, reserve and search go through faiss_GpuIndexIVF_* and faiss_Index_*. */
+FB200_API int faiss_GpuIndexIVFScalarQuantizer_new(FaissGpuIndex** p_index, FaissStandardGpuResources* res, int d, idx_t nlist, int qtype, FaissMetricType metric, int encodeResidual, int device);
+FB200_API int faiss_GpuIndexIVFScalarQuantizer_new_with_quantizer(FaissGpuIndex** p_index, FaissStandardGpuResources* res, FaissGpuIndex* coarse, int d, idx_t nlist, int qtype, FaissMetricType metric, int encodeResidual, int device);
+FB200_API int faiss_GpuIndexIVFScalarQuantizer_set_trained(FaissGpuIndex* index, const float* trained, size_t n);
+FB200_API int faiss_GpuIndexIVFScalarQuantizer_get_trained(const FaissGpuIndex* index, float* out, size_t* n);
+FB200_API int faiss_GpuIndexIVFScalarQuantizer_code_size(const FaissGpuIndex* index, size_t* out);
+FB200_API int faiss_GpuIndexIVFScalarQuantizer_qtype(const FaissGpuIndex* index, int* out);
+FB200_API int faiss_GpuIndexIVFScalarQuantizer_by_residual(const FaissGpuIndex* index, int* out);
+/* ScalarQuantizer::rangestat / rangestat_arg used by train(); only RS_minmax (0) trains on the GPU */
+FB200_API int faiss_GpuIndexIVFScalarQuantizer_set_rangestat(FaissGpuIndex* index, int rangestat, float rangestat_arg);
+
 /* ---- IndexShards (c_api/IndexShards_c.h:28-40) ---- */
 FB200_API int faiss_IndexShards_new(FaissIndexShards** p_index, idx_t d);
 FB200_API int faiss_IndexShards_new_with_options(FaissIndexShards** p_index, idx_t d, int threaded, int successive_ids);
