@@ -808,28 +808,34 @@ struct SmemPlan {
     int yStages;
     size_t bytes;
     int ksplit; // ring stages hold single K-blocks (see flat_tc_kernel)
+    bool pipe;  // ring stages hold half tiles, for the pipelined consumer (flat_tc_kernel PIPE)
+    int boxRows; // database rows per TMA copy of mapY
 };
 
 constexpr int kMaxKB = 4; // d <= 256: the query tile (16 KB per K-block) + at least three 32 KB K-block stages in 227 KB
 
-// d <= 128: whole-tile stages (64 KB at d = 128: three of them); beyond, K-block stages (see flat_tc_kernel)
-SmemPlan planSmem(int KB) {
+// 112 < d <= 128: half-tile stages (32 KB: six of them); other d <= 128: whole-tile stages (64 KB at d = 128: three of
+// them); beyond, K-block stages (see flat_tc_kernel)
+SmemPlan planSmem(int KB, int kSteps) {
     FB_THROW_IF_NOT_MSG(KB <= kMaxKB, "dimension too large for the tensor-core Flat kernel");
     const int ksplit = KB > 2 ? 1 : 0;
+    const bool pipe = tc_pipelined(KB, kSteps);
+    const int boxRows = pipe ? kHalfN : kTileN;
     const size_t qtile = (size_t)KB * kTileM * kKBlock * 2;
     const size_t fixed = 1024 /*align slack*/ + 512 /*barriers*/ + qtile;
-    const size_t stage = (size_t)(ksplit ? 1 : KB) * kTileN * kKBlock * 2;
+    const size_t stage = (size_t)(ksplit ? 1 : KB) * boxRows * kKBlock * 2;
     const size_t budget = 226 * 1024; // 232448 B is the opt-in limit per CTA
     int ys = (int)std::min<size_t>(kMaxYStages, (budget - fixed) / stage);
     FB_THROW_IF_NOT(ys >= 3);
-    return {ys, fixed + ys * stage, ksplit};
+    return {ys, fixed + ys * stage, ksplit, pipe, boxRows};
 }
 
 template <bool DUMP>
-void launchTc(const CUtensorMap& mq, const CUtensorMap& my, const TcParams& p, int grid, size_t smem, cudaStream_t stream, bool self = false) {
-    auto kern = flat_tc_kernel<DUMP>;
+void launchTc(const CUtensorMap& mq, const CUtensorMap& my, const TcParams& p, int grid, const SmemPlan& sp, cudaStream_t stream, bool self = false) {
+    const size_t smem = sp.bytes;
+    auto kern = sp.pipe ? flat_tc_kernel<DUMP, false, true> : flat_tc_kernel<DUMP>;
     if (self && !DUMP) // k = 1 streaming mode (self-tightening thresholds)
-        kern = flat_tc_kernel<false, true>;
+        kern = sp.pipe ? flat_tc_kernel<false, true, true> : flat_tc_kernel<false, true>;
     CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTiming::begin("flat_tc", stream);
     kern<<<grid, kTcThreads, smem, stream>>>(mq, my, p);
@@ -916,8 +922,9 @@ void runFlatTcScoresDebug(
         cudaStream_t stream) {
     FB_THROW_IF_NOT(dpad % kKBlock == 0 && dpad <= kMaxKB * kKBlock);
     const int KB = dpad / kKBlock;
-    SmemPlan sp = planSmem(KB);
-    CUtensorMap my = makeTileMap(Y16, n, dpad, kTileN, sp.ksplit);
+    const int kSteps = dpad / 16; // debug seam: operands arrive padded
+    SmemPlan sp = planSmem(KB, kSteps);
+    CUtensorMap my = makeTileMap(Y16, n, dpad, sp.boxRows, sp.ksplit);
     const int64_t numTiles = ceil_div(n, kTileN);
     const int64_t qPairs = ceil_div(nq, kUnitM);
     // the kernel reads whole 128-row query tiles: zero-padded private copy
@@ -943,7 +950,7 @@ void runFlatTcScoresDebug(
     p.numTiles = (unsigned long long)numTiles;
     p.KB = KB;
     p.ksplit = sp.ksplit;
-    p.kSteps = dpad / 16; // debug seam: operands arrive padded
+    p.kSteps = kSteps;
     p.yStages = sp.yStages;
     p.invScalePtr = one;
     p.bias = nullptr;
@@ -958,7 +965,7 @@ void runFlatTcScoresDebug(
     int dev = 0, sms = 0;
     CUDA_VERIFY(cudaGetDevice(&dev));
     CUDA_VERIFY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    launchTc<true>(mq, my, p, (int)std::min<int64_t>(p.numUnits, sms), sp.bytes, stream);
+    launchTc<true>(mq, my, p, (int)std::min<int64_t>(p.numUnits, sms), sp, stream);
     CUDA_VERIFY(cudaFreeAsync(qpad, stream));
     CUDA_VERIFY(cudaFreeAsync(one, stream));
 }
@@ -989,7 +996,8 @@ void runFlatTcSearch(
         return;
     FB_THROW_IF_NOT(flatTcSupported(d, k, n));
     const int KB = dpad / kKBlock;
-    const SmemPlan sp = planSmem(KB);
+    const int kSteps = (d + 15) / 16;
+    const SmemPlan sp = planSmem(KB, kSteps);
     const int sms = res->numSMs(device);
     const int64_t T = ceil_div(n, kTileN);
     // Sharded search: every rank runs the SAME number of rounds (one all-reduce per round), so the schedule
@@ -1014,7 +1022,7 @@ void runFlatTcSearch(
     const float c1 = 1.01f * (ldexpf(1.f, -10) + (float)dpad * ldexpf(1.f, -22));
     const float c2 = (float)(dpad + 16) * ldexpf(1.f, -24);
 
-    CUtensorMap mapY = makeTileMap(Y16, n, dpad, kTileN, sp.ksplit);
+    CUtensorMap mapY = makeTileMap(Y16, n, dpad, sp.boxRows, sp.ksplit);
 
     // first round: ~40 k rows (16 tiles at k = 100).  Every score of round 0 becomes a candidate, so a
     // fixed 16 tiles would make small-k searches (k-means assignment: k = 1, millions of queries) pay 4096
@@ -1146,7 +1154,7 @@ void runFlatTcSearch(
             p.numTiles = (unsigned long long)T;
             p.KB = KB;
             p.ksplit = sp.ksplit;
-            p.kSteps = (d + 15) / 16;
+            p.kSteps = kSteps;
             p.yStages = sp.yStages;
             p.invScalePtr = sc + 2;
             p.bias = bias;
@@ -1161,7 +1169,7 @@ void runFlatTcSearch(
             p.dumpLd = 0;
             p.nq = (int)nq;
             if (p.tileBegin < p.tileEnd) {
-                launchTc<false>(mapQ, mapY, p, std::min(p.numUnits, sms), sp.bytes, stream, streaming);
+                launchTc<false>(mapQ, mapY, p, std::min(p.numUnits, sms), sp, stream, streaming);
             } else { // this shard has no tiles in this round of the common schedule: no candidates
                 CUDA_VERIFY(cudaMemsetAsync(counts.data, 0, (size_t)p.numUnits * kSegsPerUnit * sizeof(int), stream));
             }

@@ -5,12 +5,14 @@
 //               64 g .. 64 g + 63.  For every database tile it issues wgmma.m64n256k16 (fp16 operands straight
 //               from the 128B-swizzled shared-memory stages, fp32 accumulators in registers: 128 per thread),
 //               waits for them, hands the stage back and filters its own accumulator fragment (below).  At
-//               112 < d <= 128 the tile's MMAs run as two N = 128 halves, and the filter of the first half overlaps
-//               the MMAs of the second; otherwise a warpgroup's own MMAs and filter do not overlap.  The two warpgroups share the ring without
-//               synchronising with each other, so one's tensor work can overlap the other's filter.  Survivors (rare) are appended with plain stores to a thread-private candidate segment;
-//               scores never reach HBM.
-//   warp 8    : TMA producer -- the unit's query tile once, then database tiles (256 rows x dpad fp16,
-//               128B-swizzled K-major) through an mbarrier ring.
+//               112 < d <= 128 (PIPE) a tile runs as two N = 128 chains, A (columns 0-127) and B (128-255), each
+//               reading its own half-tile stage, and the warpgroup is software-pipelined: it filters A(t) while
+//               B(t) runs and B(t) while A(t + 1) runs, so it always has MMAs of its own in flight.  Otherwise a
+//               warpgroup's own MMAs and filter do not overlap.  The two warpgroups share the ring without
+//               synchronising with each other, so one's tensor work can also overlap the other's filter.  Survivors
+//               (rare) are appended with plain stores to a thread-private candidate segment; scores never reach HBM.
+//   warp 8    : TMA producer -- the unit's query tile once, then database tiles (256 rows x dpad fp16, or PIPE: two
+//               128-row halves of one, 128B-swizzled K-major) through an mbarrier ring.
 // Nine warps put three on one scheduler, which caps a thread at 168 registers: the 128 accumulators plus the filter
 // state fit without spills.
 //
@@ -30,6 +32,7 @@ constexpr int kTileM = 128;       // queries per work unit (the query tile)
 constexpr int kUnitM = kTileM;
 constexpr int kWgM = 64;          // query rows per consumer warpgroup (wgmma M)
 constexpr int kTileN = 256;       // database rows per tile (wgmma N)
+constexpr int kHalfN = kTileN / 2; // PIPE: database rows per ring stage and per MMA chain
 constexpr int kKBlock = 64;       // fp16 elements per 128-byte swizzle row
 constexpr int kParts = 4;         // column parts of a tile per query row (lanes of a quad)
 constexpr int kConsumerWarps = 8; // two warpgroups
@@ -62,6 +65,13 @@ struct TcParams {
     long long dumpLd;
     int nq;
 };
+
+// The pipelined consumer (PIPE) needs exactly 8 K-steps in one 2-K-block stage: 112 < d <= 128.  Its K-step count must
+// be a compile-time constant: with a run-time count ptxas cannot tell which wgmma group is in flight and serialises
+// every MMA.
+__host__ __device__ constexpr bool tc_pipelined(int KB, int kSteps) {
+    return KB == 2 && kSteps == 2 * kKBlock / 16;
+}
 
 __device__ __forceinline__ int perm_tile(const TcParams& p, int pos) {
     return (int)(((unsigned long long)pos * p.permA + p.permB) % p.numTiles);
@@ -142,7 +152,8 @@ __device__ __forceinline__ void epi_filter32(
 // SELF (k = 1 streaming mode, used for k-means assignment): one pass over all tiles, every consumer thread keeps
 // a running "best approximate score minus 2 eps" threshold for its two queries and emits only the candidates
 // that beat it -- about ln(columns per thread) plus the near-ties of the maximum.
-template <bool DUMP, bool SELF = false>
+// PIPE: tc_pipelined(p.KB, p.kSteps) holds, mapY's box is kHalfN rows and every ring stage holds one half of a tile.
+template <bool DUMP, bool SELF = false, bool PIPE = false>
 __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
         const __grid_constant__ CUtensorMap mapQ,
         const __grid_constant__ CUtensorMap mapY,
@@ -153,8 +164,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
             (reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
     const int qBytes = p.KB * kTileM * kKBlock * 2; // the query tile (128 rows)
     // one ring stage: a whole database tile (256 rows x dpad), or -- K-split mode, dpad > 128, where the query tile
-    // plus several whole-tile stages no longer fit 227 KB -- one 64-wide K-block of it
-    const int stageBytes = (p.ksplit ? 1 : p.KB) * kTileN * kKBlock * 2;
+    // plus several whole-tile stages no longer fit 227 KB -- one 64-wide K-block of it; PIPE: one 128-row half of a
+    // tile, laid out [kblock][128 rows][64] like a whole tile (the K-block stride is 16 KB)
+    const int stageBytes = PIPE ? p.KB * kHalfN * kKBlock * 2 : (p.ksplit ? 1 : p.KB) * kTileN * kKBlock * 2;
     unsigned char* sQ = smem;
     unsigned char* sY = smem + qBytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(sY + (size_t)p.yStages * stageBytes);
@@ -197,12 +209,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
                 const int pe = min(p.tileEnd, pb + p.tilesPerSlice);
                 for (int pp = pb; pp < pe; pp++) {
                     const int t = perm_tile(p, pp);
-                    // K-split: mapY's box is one K-block; both warpgroups consume every stage
-                    const int loads = p.ksplit ? p.KB : 1;
+                    // K-split: mapY's box is one K-block; PIPE: it is one half of the tile's rows (the second half of
+                    // the last tile may lie wholly past N: TMA zero-fills it and still counts the full box).  Both
+                    // warpgroups consume every stage.
+                    const int loads = PIPE ? 2 : p.ksplit ? p.KB : 1;
                     for (int l = 0; l < loads; l++) {
                         ptx::mbar_wait(&y_empty[ys], yphase ^ 1);
                         ptx::mbar_arrive_expect_tx(&y_full[ys], (uint32_t)stageBytes);
-                        ptx::tma_load_3d(sY + (size_t)ys * stageBytes, &mapY, &y_full[ys], 0, t * kTileN, l);
+                        if (PIPE)
+                            ptx::tma_load_3d(sY + (size_t)ys * stageBytes, &mapY, &y_full[ys], 0, t * kTileN + l * kHalfN, 0);
+                        else
+                            ptx::tma_load_3d(sY + (size_t)ys * stageBytes, &mapY, &y_full[ys], 0, t * kTileN, l);
                         if (++ys == p.yStages) {
                             ys = 0;
                             yphase ^= 1;
@@ -223,6 +240,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
     const uint32_t sYaddr = ptx::smem_u32(sY);
     const int qkb = kTileM * kKBlock * 2; // bytes per K-block of the query tile
     const int ykb = kTileN * kKBlock * 2; // bytes per K-block of a database tile
+    const int hkb = kHalfN * kKBlock * 2; // PIPE: bytes per K-block of a half-tile stage
     const int permStep = (int)(p.permA % p.numTiles);
     float acc[128];
 #pragma unroll
@@ -255,10 +273,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
         float maxbNext = (!DUMP && pb < pe) ? __ldg(p.tileMaxBias + t) : 0.f;
         float minbNext = (SELF && pb < pe) ? __ldg(p.tileMinBias + t) : 0.f;
         ptx::mbar_wait(q_full, it & 1);
-        for (int pp = pb; pp < pe; pp++) {
-            const long long colBase = (long long)t * kTileN + 2 * part;
-            const float maxb = maxbNext;
-            const float minb = minbNext;
+
+        // the tile being filtered: this thread's first column of it and its bias bounds
+        long long colBase = 0;
+        float maxb = 0.f, minb = 0.f;
+        auto nextTile = [&](int pp) {
+            colBase = (long long)t * kTileN + 2 * part;
+            maxb = maxbNext;
+            minb = minbNext;
             t += permStep;
             if (t >= (int)p.numTiles)
                 t -= (int)p.numTiles;
@@ -266,54 +288,85 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
                 maxbNext = __ldg(p.tileMaxBias + t);
             if (SELF && pp + 1 < pe)
                 minbNext = __ldg(p.tileMinBias + t);
-
-            // filter of the tile's columns 128 c .. 128 c + 127 (acc[64 c .. 64 c + 63]) for both of the thread's rows
-            auto filterHalf = [&](int c) {
+        };
+        // filter of the tile's columns 128 c .. 128 c + 127 (acc[64 c .. 64 c + 63]) for both of the thread's rows
+        auto filterHalf = [&](int c) {
 #pragma unroll
-                for (int h = 0; h < 2; h++) {
-                    float r[32];
+            for (int h = 0; h < 2; h++) {
+                float r[32];
 #pragma unroll
-                    for (int e = 0; e < 32; e++)
-                        r[e] = acc[4 * (16 * c + (e >> 1)) + 2 * h + (e & 1)];
-                    if (h)
-                        epi_filter32<DUMP, SELF>(p, r, q1, colBase + 128 * c, inv, thr1, slack1, maxb, buf1, cnt1, minb);
-                    else
-                        epi_filter32<DUMP, SELF>(p, r, q0, colBase + 128 * c, inv, thr0, slack0, maxb, buf0, cnt0, minb);
-                }
-            };
+                for (int e = 0; e < 32; e++)
+                    r[e] = acc[4 * (16 * c + (e >> 1)) + 2 * h + (e & 1)];
+                if (h)
+                    epi_filter32<DUMP, SELF>(p, r, q1, colBase + 128 * c, inv, thr1, slack1, maxb, buf1, cnt1, minb);
+                else
+                    epi_filter32<DUMP, SELF>(p, r, q0, colBase + 128 * c, inv, thr0, slack0, maxb, buf0, cnt0, minb);
+            }
+        };
 
-            // ---- scores of the tile: acc = Q[64 rows] . Y[256 rows]^T
-            if (!p.ksplit && p.kSteps == 2 * kKBlock / 16) {
-                // 112 < d <= 128, one stage per tile: two N = 128 halves committed separately, so that the filter of
-                // columns 0-127 runs while the tensor cores still work on columns 128-255 (otherwise a warpgroup's
-                // filter waits for all of its MMAs).  The K-step count must be a compile-time constant here: with a
-                // run-time count ptxas cannot tell which group is still in flight and serialises every MMA.
+        if constexpr (PIPE) {
+            // ring stages are taken and handed back one half-tile at a time
+            auto acquireStage = [&]() {
                 ptx::mbar_wait(&y_full[ys], yphase);
-                const uint32_t yaddr = sYaddr + (uint32_t)ys * (uint32_t)stageBytes;
-#pragma unroll
-                for (int c = 0; c < 2; c++) {
-                    ptx::wgmma_fence(); // each half is its own wgmma pipeline stage
-#pragma unroll
-                    for (int ks = 0; ks < 2 * kKBlock / 16; ks++) {
-                        const int kb = ks >> 2, k4 = ks & 3;
-                        const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + kb * qkb + k4 * 32);
-                        // database rows 128 c .. 128 c + 127 start 16 KB (whole swizzle atoms) into the K-block
-                        const uint64_t db = ptx::make_smem_desc_sw128(yaddr + kb * ykb + c * (ykb / 2) + k4 * 32);
-                        ptx::wgmma_m64n128k16_f16_ss(acc + 64 * c, da, db, ks != 0 ? 1u : 0u);
-                    }
-                    ptx::wgmma_commit();
-                }
-                ptx::wgmma_wait_all_but_one(); // columns 0-127 are final
-                filterHalf(0);
-                ptx::wgmma_wait_all();
-                __syncwarp();
-                if (lane == 0) // this warp's share of the stage has been read
-                    ptx::mbar_arrive(&y_empty[ys]);
+                const int s = ys;
                 if (++ys == p.yStages) {
                     ys = 0;
                     yphase ^= 1;
                 }
-            } else {
+                return s;
+            };
+            auto releaseStage = [&](int s) {
+                __syncwarp();
+                if (lane == 0) // this warp's share of the stage has been read
+                    ptx::mbar_arrive(&y_empty[s]);
+            };
+            // chain c: columns 128 c .. 128 c + 127 of the tile (the half in stage s) into acc[64 c .. 64 c + 63],
+            // committed as one wgmma group.  c must be a compile-time constant at every call.
+            auto issueHalf = [&](int c, int s) {
+                const uint32_t yaddr = sYaddr + (uint32_t)s * (uint32_t)stageBytes;
+                ptx::wgmma_fence_operands<64>(acc + 64 * c);
+                ptx::wgmma_fence(); // the accumulators were last read by the filter
+#pragma unroll
+                for (int ks = 0; ks < 2 * kKBlock / 16; ks++) {
+                    const int kb = ks >> 2, k4 = ks & 3;
+                    const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + kb * qkb + k4 * 32);
+                    const uint64_t db = ptx::make_smem_desc_sw128(yaddr + kb * hkb + k4 * 32);
+                    ptx::wgmma_m64n128k16_f16_ss(acc + 64 * c, da, db, ks != 0 ? 1u : 0u);
+                }
+                ptx::wgmma_commit();
+                ptx::wgmma_fence_operands<64>(acc + 64 * c);
+            };
+            // Iteration pp issues A(pp), filters B(pp - 1) while A(pp) runs, then issues B(pp) and filters A(pp) while
+            // B(pp) runs.  Nothing is in flight across the back-edge: ptxas cannot follow a group that is still in
+            // flight there and would serialise every MMA, so B(pp) is waited for at the end of the iteration and
+            // filtered at the start of the next (the unit's last one after the loop).  A half-stage goes back to the
+            // producer as soon as its chain retires.  The filter order per thread -- tile by tile, columns 0-127
+            // first -- is that of the unpipelined loop.
+            for (int pp = pb; pp < pe; pp++) {
+                const int sA = acquireStage();
+                issueHalf(0, sA);
+                // only A(pp) is in flight, so this returns at once; without it ptxas cannot tell that B(pp - 1) has
+                // retired and waits for A(pp) before the filter below
+                ptx::wgmma_wait_all_but_one();
+                if (pp > pb)
+                    filterHalf(1); // B(pp - 1)
+                nextTile(pp);
+                const int sB = acquireStage();
+                issueHalf(1, sB);
+                ptx::wgmma_wait_all_but_one(); // A(pp) retired
+                ptx::wgmma_fence_operands<64>(acc);
+                releaseStage(sA);
+                filterHalf(0);
+                ptx::wgmma_wait_all(); // B(pp) retired
+                ptx::wgmma_fence_operands<64>(acc + 64);
+                releaseStage(sB);
+            }
+            if (pb < pe)
+                filterHalf(1); // B of the unit's last tile
+        } else {
+            for (int pp = pb; pp < pe; pp++) {
+                nextTile(pp);
+                // ---- scores of the tile: acc = Q[64 rows] . Y[256 rows]^T
                 const int stagesPerTile = p.ksplit ? p.KB : 1;
 #pragma unroll 1
                 for (int kb0 = 0; kb0 < stagesPerTile; kb0++) {
@@ -342,8 +395,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
                     }
                 }
                 filterHalf(0);
+                filterHalf(1);
             }
-            filterHalf(1);
         }
         __syncwarp();
         if (lane == 0) // the query tile may be overwritten

@@ -128,6 +128,15 @@ __device__ __forceinline__ void wgmma_wait_all() {
 __device__ __forceinline__ void wgmma_wait_all_but_one() {
     asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
 }
+// Pins N accumulator registers at this point of the program: the compiler cannot move their reads or writes across
+// it.  The wait instructions above do not name the registers they make final, so without it a read of an accumulator
+// can be scheduled before the wait that retires its group, and ptxas then serialises the MMAs.
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operands(float* d) {
+#pragma unroll
+    for (int i = 0; i < N; i++)
+        asm volatile("" : "+f"(d[i])::"memory");
+}
 // D[64 x 256, registers] (+)= A[smem desc, 64 x 16] * B[smem desc, 256 x 16]^T, fp16 inputs, fp32 accumulate,
 // both operands K-major.  Fragment of D held by thread t of the warpgroup (warp w = t / 32, lane l):
 //   d[4 j + 2 h + b] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + b]   (j < 32, h, b < 2)
