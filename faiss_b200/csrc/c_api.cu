@@ -859,27 +859,7 @@ int faiss_b200_kmeans(
         int maxppc,
         float* centroids_out,
         float* obj_out) {
-    try {
-        auto res = RES(r);
-        ClusteringParameters cp;
-        if (niter > 0)
-            cp.niter = niter;
-        if (seed >= 0)
-            cp.seed = seed;
-        if (maxppc > 0)
-            cp.max_points_per_centroid = maxppc;
-        Clustering clus((int)d, (int)k, cp);
-        GpuIndexFlatConfig fc;
-        fc.device = device;
-        GpuIndexFlatL2 index(res, (int)d, fc);
-        clus.train((idx_t)n, x, index);
-        memcpy(centroids_out, clus.centroids.data(), sizeof(float) * d * k);
-        if (obj_out) {
-            for (size_t i = 0; i < clus.iteration_stats.size() && (int)i < cp.niter; i++)
-                obj_out[i] = clus.iteration_stats[i].obj;
-        }
-    }
-    CATCH_AND_HANDLE
+    return faiss_b200_kmeans_ex(r, device, d, n, k, x, niter, seed, maxppc, ::METRIC_L2, 0, centroids_out, obj_out);
 }
 
 int faiss_b200_kmeans_ex(

@@ -347,14 +347,19 @@ struct Clustering : ClusteringParameters {
     Clustering(int d, int k, const ClusteringParameters& cp) : ClusteringParameters(cp), d(d), k(k) {}
     // x: host or device pointer.  `index` is the assignment index (reset / add / search k=1).
     void train(idx_t n, const float* x, GpuIndexFlat& index);
-    // The same Lloyd iterations with the training set SHARDED over the ranks of `comm` (rank order = row order of
-    // the concatenated set) and the centroid table replicated: local Flat k=1 assignment, local partial sums
-    // (deterministic sort + segmented sum), ONE packed ncclAllReduce per iteration (k*d sums | k counts | objective),
-    // empty clusters refilled by the reference's deterministic split_clusters on every rank identically
-    // (SURVEY 8(e)).  Collective: every rank calls it with its own rows; sub-sampling is the caller's business.
-    // Every rank ends with identical centroids (also added to `index`).  splitSeconds: host time inside split_clusters.
+    // `train`'s Lloyd loop with the training set SHARDED over the ranks of `comm` (rank order = row order of the
+    // concatenated set) and the centroid table replicated; the only addition is one all-reduce per iteration, so the
+    // result equals `train` on the concatenated set (SURVEY 8(e)).  Collective: every rank calls it with its own
+    // rows; sub-sampling is the caller's business.  Every rank ends with identical centroids (also in `index`).
     void trainSharded(idx_t nLocal, const float* xLocal, GpuIndexFlat& index, const Communicator& comm);
-    double splitSeconds = 0;
+    double splitSeconds = 0; // host time inside split_clusters during the last train / trainSharded
+
+   private:
+    // One Lloyd run, initialisation to last iteration, over rows [off, off + nLocal) of an nTotal-row training set
+    // (xLocal on the device); comm == nullptr for a single process.  Fills `centroids`, appends to
+    // `iteration_stats` and returns the last objective.  t0 / tSearch: the run's start and its search-time total.
+    float lloyd_(idx_t nLocal, const float* xLocal, idx_t nTotal, idx_t off, GpuIndexFlat& index, int redo,
+                 const Communicator* comm, double t0, double& tSearch);
 };
 
 // ProductQuantizer::train, Train_default (faiss/impl/ProductQuantizer.cpp:130-195); x device [n,d], pqOut host [M][256][d/M]
