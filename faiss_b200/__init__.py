@@ -17,8 +17,20 @@ import numpy as np
 
 from ._lib import lib, check, FaissError  # noqa: F401  (loading fails loudly)
 
+# faiss::MetricType (faiss/MetricType.h:29-49).  Every index takes L2 and inner product; GpuIndexFlat and
+# bfKnn / knn_gpu also take the others (METRIC_Lp's exponent is Index.metric_arg / bfKnn's metric_arg).
+# METRIC_NaNEuclidean is not implemented.
 METRIC_INNER_PRODUCT = 0
 METRIC_L2 = 1
+METRIC_L1 = 2
+METRIC_Linf = 3
+METRIC_Lp = 4
+METRIC_Canberra = 20
+METRIC_BrayCurtis = 21
+METRIC_JensenShannon = 22
+METRIC_Jaccard = 23
+METRIC_NaNEuclidean = 24
+METRIC_GOWER = 25
 
 # faiss::ScalarQuantizer::QuantizerType (faiss/impl/ScalarQuantizer.h:27-40); GpuIndexIVFScalarQuantizer
 # accepts QT_8bit ... QT_6bit, as the reference GPU index does
@@ -194,6 +206,15 @@ class Index:
     @property
     def metric_type(self):
         return lib.faiss_Index_metric_type(self._h)
+
+    @property
+    def metric_arg(self):
+        """faiss::Index::metric_arg (the exponent of METRIC_Lp); read at search time"""
+        return lib.faiss_Index_metric_arg(self._h)
+
+    @metric_arg.setter
+    def metric_arg(self, v):
+        lib.faiss_Index_set_metric_arg(self._h, float(v))
 
     @property
     def verbose(self):
@@ -748,9 +769,10 @@ def kmeans_ex(res, x, k, niter=25, seed=1234, max_points_per_centroid=256, metri
     return cent, obj
 
 
-def bfKnn(res, xq, xb, k, metric=METRIC_L2, device=0):
+def bfKnn(res, xq, xb, k, metric=METRIC_L2, device=0, metric_arg=0.0):
     """faiss.knn_gpu / bfKnn (faiss/gpu/GpuDistance.h:33-181, faiss/python/gpu_wrappers.py:60-200): brute-force
-    k-NN of xq in xb, row-major fp32, numpy or torch CUDA inputs; outputs follow xq's residency."""
+    k-NN of xq in xb, row-major fp32, numpy or torch CUDA inputs; outputs follow xq's residency.  metric_arg is
+    GpuDistanceParams::metricArg (the exponent of METRIC_Lp)."""
     xq, xb = _as_f32(xq), _as_f32(xb)
     nq, d = xq.shape
     assert xb.shape[1] == d
@@ -761,18 +783,19 @@ def bfKnn(res, xq, xb, k, metric=METRIC_L2, device=0):
 
         res.setDefaultStream(device, torch.cuda.current_stream(device).cuda_stream)
     check(
-        lib.faiss_b200_bfKnn(
-            res._h, int(device), int(metric), ctypes.c_int64(k), int(d), _ptr(xb, _c_f), ctypes.c_int64(xb.shape[0]), _ptr(xq, _c_f),
+        lib.faiss_b200_bfKnn_ex(
+            res._h, int(device), int(metric), ctypes.c_float(metric_arg), ctypes.c_int64(k), int(d), _ptr(xb, _c_f),
+            ctypes.c_int64(xb.shape[0]), _ptr(xq, _c_f),
             ctypes.c_int64(nq), _ptr(D, _c_f), _ptr(I, _c_i64),
         )
     )
     return D, I
 
 
-def knn_gpu(res, xq, xb, k, D=None, I=None, metric=METRIC_L2, device=0):
+def knn_gpu(res, xq, xb, k, D=None, I=None, metric=METRIC_L2, device=0, metric_arg=0.0):
     """faiss.knn_gpu (faiss/python/gpu_wrappers.py:60-200) for row-major fp32 inputs: argument order of the reference,
     optional preallocated outputs."""
-    rD, rI = bfKnn(res, xq, xb, k, metric, device)
+    rD, rI = bfKnn(res, xq, xb, k, metric, device, metric_arg)
     if D is not None:
         D[...] = rD
         rD = D

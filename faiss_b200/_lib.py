@@ -33,6 +33,10 @@ lib.faiss_Index_ntotal.argtypes = [ctypes.c_void_p]
 lib.faiss_Index_d.argtypes = [ctypes.c_void_p]
 lib.faiss_Index_is_trained.argtypes = [ctypes.c_void_p]
 lib.faiss_Index_metric_type.argtypes = [ctypes.c_void_p]
+lib.faiss_Index_metric_arg.restype = ctypes.c_float
+lib.faiss_Index_metric_arg.argtypes = [ctypes.c_void_p]
+lib.faiss_Index_set_metric_arg.restype = None
+lib.faiss_Index_set_metric_arg.argtypes = [ctypes.c_void_p, ctypes.c_float]
 lib.faiss_Index_verbose.argtypes = [ctypes.c_void_p]
 lib.faiss_Index_set_verbose.argtypes = [ctypes.c_void_p, ctypes.c_int]
 lib.faiss_Index_set_verbose.restype = None

@@ -52,9 +52,19 @@ static std::shared_ptr<StandardGpuResources> RES(FaissStandardGpuResources* r) {
         FB_THROW_MSG("null resources handle");
     return r->res;
 }
+// every value of faiss/MetricType.h; the C++ constructors reject what they do not implement (METRIC_NaNEuclidean
+// anywhere, everything but L2 / IP in the IVF indexes)
 static MetricType MT(FaissMetricType m) {
-    if (m != ::METRIC_L2 && m != ::METRIC_INNER_PRODUCT)
+    const MetricType mt = (MetricType)(int)m;
+    if (!is_implemented_metric(mt) && mt != fb200::METRIC_NaNEuclidean)
         FB_THROW_MSG("unsupported metric type");
+    return mt;
+}
+// the entry points whose kernels are L2 / inner product only: the IVF constructors, k-means and the IVF seams
+// (faiss/gpu/GpuIndexIVF.cu:34-38)
+static MetricType MT_L2IP(FaissMetricType m) {
+    if (m != ::METRIC_L2 && m != ::METRIC_INNER_PRODUCT)
+        FB_THROW_FMT("unsupported metric type %d", (int)m);
     return m == ::METRIC_L2 ? fb200::METRIC_L2 : fb200::METRIC_INNER_PRODUCT;
 }
 
@@ -174,7 +184,14 @@ idx_t faiss_Index_ntotal(const FaissIndex* p) {
     return p && p->index ? p->index->ntotal : 0;
 }
 FaissMetricType faiss_Index_metric_type(const FaissIndex* p) {
-    return p && p->index && p->index->metric_type == fb200::METRIC_INNER_PRODUCT ? ::METRIC_INNER_PRODUCT : ::METRIC_L2;
+    return p && p->index ? (FaissMetricType)(int)p->index->metric_type : ::METRIC_L2;
+}
+float faiss_Index_metric_arg(const FaissIndex* p) {
+    return p && p->index ? p->index->metric_arg : 0.f;
+}
+void faiss_Index_set_metric_arg(FaissIndex* p, float v) {
+    if (p && p->index)
+        p->index->metric_arg = v;
 }
 int faiss_Index_verbose(const FaissIndex* p) {
     return p && p->index ? (int)p->index->verbose : 0;
@@ -456,7 +473,7 @@ int faiss_GpuIndexIVFFlat_new(
         auto res = RES(r);
         auto* h = new FaissIndex_H();
         h->res = res;
-        h->index = new GpuIndexIVFFlat(res, d, nlist, MT(metric), c);
+        h->index = new GpuIndexIVFFlat(res, d, nlist, MT_L2IP(metric), c);
         *p = h;
     }
     CATCH_AND_HANDLE
@@ -478,7 +495,7 @@ int faiss_GpuIndexIVFPQ_new(
         auto res = RES(r);
         auto* h = new FaissIndex_H();
         h->res = res;
-        h->index = new GpuIndexIVFPQ(res, d, nlist, M, nbits, MT(metric), c);
+        h->index = new GpuIndexIVFPQ(res, d, nlist, M, nbits, MT_L2IP(metric), c);
         *p = h;
     }
     CATCH_AND_HANDLE
@@ -530,7 +547,7 @@ int faiss_GpuIndexIVFScalarQuantizer_new(
         auto res = RES(r);
         auto* h = new FaissIndex_H{nullptr, res};
         try {
-            h->index = new GpuIndexIVFScalarQuantizer(res, d, nlist, qtype, MT(metric), encodeResidual != 0, c);
+            h->index = new GpuIndexIVFScalarQuantizer(res, d, nlist, qtype, MT_L2IP(metric), encodeResidual != 0, c);
         } catch (...) {
             delete h;
             throw;
@@ -556,7 +573,7 @@ int faiss_GpuIndexIVFScalarQuantizer_new_with_quantizer(
         auto* h = new FaissIndex_H{nullptr, res};
         try {
             h->index = new GpuIndexIVFScalarQuantizer(
-                    res, AS<GpuIndexFlat>(coarse, "GpuIndexFlat"), d, nlist, qtype, MT(metric), encodeResidual != 0, c);
+                    res, AS<GpuIndexFlat>(coarse, "GpuIndexFlat"), d, nlist, qtype, MT_L2IP(metric), encodeResidual != 0, c);
         } catch (...) {
             delete h;
             throw;
@@ -701,7 +718,7 @@ int faiss_GpuIndexIVFFlat_new_with_quantizer(
         cfg.device = device;
         auto* h = new FaissIndex_H{nullptr, res};
         try {
-            h->index = new GpuIndexIVFFlat(res, AS<GpuIndexFlat>(coarse, "GpuIndexFlat"), d, nlist, MT(metric), cfg);
+            h->index = new GpuIndexIVFFlat(res, AS<GpuIndexFlat>(coarse, "GpuIndexFlat"), d, nlist, MT_L2IP(metric), cfg);
         } catch (...) {
             delete h;
             throw;
@@ -726,7 +743,7 @@ int faiss_GpuIndexIVFPQ_new_with_quantizer(
         cfg.device = device;
         auto* h = new FaissIndex_H{nullptr, res};
         try {
-            h->index = new GpuIndexIVFPQ(res, AS<GpuIndexFlat>(coarse, "GpuIndexFlat"), d, nlist, M, nbits, MT(metric), cfg);
+            h->index = new GpuIndexIVFPQ(res, AS<GpuIndexFlat>(coarse, "GpuIndexFlat"), d, nlist, M, nbits, MT_L2IP(metric), cfg);
         } catch (...) {
             delete h;
             throw;
@@ -889,7 +906,7 @@ int faiss_b200_kmeans_ex(
         Clustering clus((int)d, (int)k, cp);
         GpuIndexFlatConfig fc;
         fc.device = device;
-        GpuIndexFlat index(res, (int)d, MT(metric), fc);
+        GpuIndexFlat index(res, (int)d, MT_L2IP(metric), fc);
         clus.train((idx_t)n, x, index);
         memcpy(centroids_out, clus.centroids.data(), sizeof(float) * d * k);
         if (obj_out) {
@@ -1032,12 +1049,29 @@ int b200_l2_norms(FaissStandardGpuResources* r, int device, const float* x, idx_
     CATCH_AND_HANDLE
 }
 // bfKnn (faiss/gpu/GpuDistance.h:33-181, GpuDistance.cu:229-571) for the case on the path: row-major fp32 vectors and
-// queries, L2 or inner product, host or device pointers.  Large problems take the tensor-core path through a transient
+// queries, any metric GpuIndexFlat takes, host or device pointers.  Large problems take the tensor-core path through a transient
 // GpuIndexFlat (vectors are copied once), small ones the exact SIMT kernel; results are identical either way.
 int faiss_b200_bfKnn(
         FaissStandardGpuResources* r,
         int device,
         FaissMetricType metric,
+        idx_t k,
+        int dims,
+        const float* vectors,
+        idx_t num_vectors,
+        const float* queries,
+        idx_t num_queries,
+        float* out_distances,
+        idx_t* out_indices) {
+    return faiss_b200_bfKnn_ex(
+            r, device, metric, 0.f, k, dims, vectors, num_vectors, queries, num_queries, out_distances, out_indices);
+}
+// GpuDistanceParams::metricArg (faiss/gpu/GpuDistance.h:41): the exponent of METRIC_Lp
+int faiss_b200_bfKnn_ex(
+        FaissStandardGpuResources* r,
+        int device,
+        FaissMetricType metric,
+        float metric_arg,
         idx_t k,
         int dims,
         const float* vectors,
@@ -1052,6 +1086,7 @@ int faiss_b200_bfKnn(
         GpuIndexFlatConfig cfg;
         cfg.device = device;
         GpuIndexFlat index(res, dims, MT(metric), cfg);
+        index.metric_arg = metric_arg;
         index.add(num_vectors, vectors);
         index.search(num_queries, queries, k, out_distances, out_indices);
     }
@@ -1132,7 +1167,7 @@ int b200_ivf_coarse(
         auto res = RES(r);
         DeviceScope s(device);
         FB_THROW_IF_NOT(nprobe >= 1 && nprobe <= kMaxNprobe);
-        runFlatExact(res.get(), device, Q, nq, centroids, nlist, d, nprobe, MT(metric), 0, coarse_dis, coarse_ids, res->getDefaultStream(device));
+        runFlatExact(res.get(), device, Q, nq, centroids, nlist, d, nprobe, MT_L2IP(metric), 0, coarse_dis, coarse_ids, res->getDefaultStream(device));
     }
     CATCH_AND_HANDLE
 }
@@ -1151,7 +1186,7 @@ int b200_kmeans_assign(
         // Clustering's index.search(n, x, 1) (faiss/Clustering.cpp:270-290) on raw device buffers, exact SIMT arithmetic
         auto res = RES(r);
         DeviceScope s(device);
-        runFlatArgmin(res.get(), device, x, n, centroids, k, d, MT(metric), dis, assign, res->getDefaultStream(device));
+        runFlatArgmin(res.get(), device, x, n, centroids, k, d, MT_L2IP(metric), dis, assign, res->getDefaultStream(device));
     }
     CATCH_AND_HANDLE
 }
@@ -1177,7 +1212,7 @@ int b200_ivfflat_scan(
         auto res = RES(r);
         DeviceScope s(device);
         FB_THROW_IF_NOT(k >= 1 && k <= kMaxK && nprobe >= 1 && nprobe <= kMaxNprobe);
-        runIvfFlatScan(res.get(), device, Q, nq, d, probes, nprobe, list_start, list_len, arena_vecs, arena_ids, arena_elems, k, MT(metric), D, I, res->getDefaultStream(device));
+        runIvfFlatScan(res.get(), device, Q, nq, d, probes, nprobe, list_start, list_len, arena_vecs, arena_ids, arena_elems, k, MT_L2IP(metric), D, I, res->getDefaultStream(device));
     }
     CATCH_AND_HANDLE
 }
@@ -1207,7 +1242,7 @@ int b200_ivfpq_scan(
         auto res = RES(r);
         DeviceScope s(device);
         FB_THROW_IF_NOT(k >= 1 && k <= kMaxK && nprobe >= 1 && nprobe <= kMaxNprobe);
-        runIvfPqScan(res.get(), device, Q, nq, d, probes, coarse_dis, nprobe, coarse_centroids, pq_centroids, M, list_start, list_len, arena_codes, arena_ids, k, MT(metric), D, I, res->getDefaultStream(device));
+        runIvfPqScan(res.get(), device, Q, nq, d, probes, coarse_dis, nprobe, coarse_centroids, pq_centroids, M, list_start, list_len, arena_codes, arena_ids, k, MT_L2IP(metric), D, I, res->getDefaultStream(device));
     }
     CATCH_AND_HANDLE
 }

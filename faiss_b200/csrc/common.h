@@ -17,8 +17,45 @@ namespace fb200 {
 
 using idx_t = int64_t; // faiss/MetricType.h:52
 
-// faiss/MetricType.h: METRIC_INNER_PRODUCT = 0, METRIC_L2 = 1
-enum MetricType : int { METRIC_INNER_PRODUCT = 0, METRIC_L2 = 1 };
+// faiss/MetricType.h:29-49 (same values).  Every index takes L2 and inner product; GpuIndexFlat and bfKnn also take
+// the others, which run on the exact SIMT kernel.  METRIC_NaNEuclidean is declared but not implemented.
+enum MetricType : int {
+    METRIC_INNER_PRODUCT = 0,
+    METRIC_L2 = 1,
+    METRIC_L1 = 2,
+    METRIC_Linf = 3,
+    METRIC_Lp = 4, // sum |a-b|^p, p = metric_arg, no root
+    METRIC_Canberra = 20,
+    METRIC_BrayCurtis = 21,
+    METRIC_JensenShannon = 22,
+    METRIC_Jaccard = 23,
+    METRIC_NaNEuclidean = 24,
+    METRIC_GOWER = 25,
+};
+
+// faiss/MetricType.h:56-58: larger is better for these two; every other metric is a distance
+inline bool is_similarity_metric(MetricType m) {
+    return m == METRIC_INNER_PRODUCT || m == METRIC_Jaccard;
+}
+
+// the metrics the exact kernel implements (all of the above but METRIC_NaNEuclidean)
+inline bool is_implemented_metric(MetricType m) {
+    switch (m) {
+        case METRIC_INNER_PRODUCT:
+        case METRIC_L2:
+        case METRIC_L1:
+        case METRIC_Linf:
+        case METRIC_Lp:
+        case METRIC_Canberra:
+        case METRIC_BrayCurtis:
+        case METRIC_JensenShannon:
+        case METRIC_Jaccard:
+        case METRIC_GOWER:
+            return true;
+        default:
+            return false;
+    }
+}
 
 // limits preserved from the reference (faiss/gpu/utils/DeviceDefs.cuh:61-68, impl/IndexUtils.cu:21-43)
 constexpr int kMaxK = 2048;

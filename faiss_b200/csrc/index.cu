@@ -207,9 +207,10 @@ GpuIndex::GpuIndex(
     metric_arg = metricArg;
     FB_THROW_IF_NOT_MSG(resources_ != nullptr, "null GpuResources");
     FB_THROW_IF_NOT_MSG(dims > 0, "Invalid number of dimensions");
-    FB_THROW_IF_NOT_MSG(
-            metric == METRIC_L2 || metric == METRIC_INNER_PRODUCT,
-            "faiss_b200 supports METRIC_L2 and METRIC_INNER_PRODUCT");
+    // every metric but METRIC_NaNEuclidean (faiss/gpu/impl/Distance.cuh:289); the IVF indexes and the clustering
+    // entry points narrow this to L2 / inner product themselves
+    if (!is_implemented_metric(metric))
+        FB_THROW_FMT("unimplemented metric type %d", (int)metric);
     resources_->initializeForDevice(config_.device);
 }
 
@@ -549,7 +550,8 @@ void GpuIndexFlat::prepareTensorCoreData_() const {
     y16_.resize((size_t)n * dpad_, stream);
     bias_.resize((size_t)padRows, stream);
     tileMaxBias_.resize((size_t)(padRows / 256) * 2, stream); // [T+1] max bias per tile, then [T+1] min bias per tile
-    const bool sorted = metric_type == METRIC_L2; // IP has no bias: row order is kept
+    const MetricType metric = searchMetric_();
+    const bool sorted = metric == METRIC_L2; // IP has no bias: row order is kept
     if (sorted)
         perm_.resize((size_t)n, stream);
     else
@@ -570,7 +572,7 @@ void GpuIndexFlat::prepareTensorCoreData_() const {
     fill_float_kernel<<<(unsigned)ceil_div(padRows, 256), 256, 0, stream>>>(bias_.data(), padRows, -INFINITY);
     CUDA_CHECK_LAST();
     runFlatTcPrepareRows(
-            resources_.get(), config_.device, rows_(), n, d, dpad_, scale, metric_type, y16_.data(), bias_.data(),
+            resources_.get(), config_.device, rows_(), n, d, dpad_, scale, metric, y16_.data(), bias_.data(),
             sorted ? perm_.data() : nullptr, tileMaxBias_.data(), norms.as<float>(), stream, yHalf_());
     runMaxOf(norms.as<float>(), n, scal.as<float>() + 1, stream);
     CUDA_VERIFY(cudaMemcpyAsync(h, scal.data, sizeof(float) * 2, cudaMemcpyDeviceToHost, stream));
@@ -580,40 +582,54 @@ void GpuIndexFlat::prepareTensorCoreData_() const {
     tcDirty_ = false;
 }
 
+// faiss/gpu/impl/Distance.cuh:223-239.  The reference GPU's p = -1 -> L2 branch is a test hook; the CPU sums
+// |a-b|^-1 there, and so does the Lp kernel.
+MetricType GpuIndexFlat::searchMetric_() const {
+    if (metric_type == METRIC_Lp && metric_arg == 1.f)
+        return METRIC_L1;
+    if (metric_type == METRIC_Lp && metric_arg == 2.f)
+        return METRIC_L2;
+    return metric_type;
+}
+
 void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
     auto stream = stream_();
     lastSearchUsedTensorCores = 0;
     lastSearchFallbackQueries = 0;
+    const MetricType metric = searchMetric_();
     if (this->ntotal == 0) {
         // faiss/gpu/impl/Distance.cu:152-164: fill with "no result"
-        std::vector<float> hd((size_t)n * k, metric_type == METRIC_L2 ? FLT_MAX : -FLT_MAX);
+        std::vector<float> hd((size_t)n * k, is_similarity_metric(metric_type) ? -FLT_MAX : FLT_MAX);
         std::vector<idx_t> hi((size_t)n * k, -1);
         CUDA_VERIFY(cudaMemcpyAsync(dDev, hd.data(), hd.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
         CUDA_VERIFY(cudaMemcpyAsync(iDev, hi.data(), hi.size() * sizeof(idx_t), cudaMemcpyHostToDevice, stream));
         CUDA_VERIFY(cudaStreamSynchronize(stream));
         return;
     }
-    // the tensor-core path pays a fixed cost per query tile of 128; tiny batches stay exact
-    const bool tc = flatConfig_.useTensorCores && flatTcSupported(d, k, this->ntotal) && n >= 16;
+    // the tensor-core path pays a fixed cost per query tile of 128; tiny batches stay exact.  Metrics without a
+    // product form (L1, Linf, Lp, Canberra, ...) always run the exact kernel.
+    const bool tc = flatConfig_.useTensorCores && tensorCoreMetric_() && flatTcSupported(d, k, this->ntotal) && n >= 16;
     GpuMemoryReservation qHold;
     xDev = roundedQueries_(n, xDev, qHold);
     if (tc) {
         prepareTensorCoreData_();
         runFlatTcSearch(
                 resources_.get(), config_.device, xDev, n, rows_(), y16_.data(), bias_.data(),
-                metric_type == METRIC_L2 ? perm_.data() : nullptr, tileMaxBias_.data(), yScale_,
-                yMaxNorm_, this->ntotal, d, dpad_, k, metric_type, dDev, iDev, stream, nullptr, yHalf_());
+                metric == METRIC_L2 ? perm_.data() : nullptr, tileMaxBias_.data(), yScale_,
+                yMaxNorm_, this->ntotal, d, dpad_, k, metric, dDev, iDev, stream, nullptr, yHalf_());
         lastSearchUsedTensorCores = 1;
         lastSearchFallbackQueries = lastFlatTcFallbacks();
     } else {
         runFlatExact(
-                resources_.get(), config_.device, xDev, n, rows_(), this->ntotal, d, k, metric_type, 0, dDev, iDev,
-                stream, yHalf_());
+                resources_.get(), config_.device, xDev, n, rows_(), this->ntotal, d, k, metric, 0, dDev, iDev,
+                stream, yHalf_(), metric_arg);
     }
 }
 
 bool GpuIndexFlat::shardPoolingEligible(int k, idx_t n) const {
-    return flatConfig_.useTensorCores && this->ntotal > 0 && flatTcSupported(d, k, this->ntotal) && n >= 16;
+    // pooled thresholds are a tensor-core certificate: other metrics take the plain all-gather + merge path
+    return flatConfig_.useTensorCores && tensorCoreMetric_() && this->ntotal > 0 && flatTcSupported(d, k, this->ntotal) &&
+            n >= 16;
 }
 
 void GpuIndexFlat::searchShardDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* flatShard) const {
@@ -626,10 +642,11 @@ void GpuIndexFlat::searchShardDevice(idx_t n, const float* xDev, int k, float* d
     prepareTensorCoreData_();
     GpuMemoryReservation qHold;
     xDev = roundedQueries_(n, xDev, qHold);
+    const MetricType metric = searchMetric_();
     runFlatTcSearch(
             resources_.get(), config_.device, xDev, n, rows_(), y16_.data(), bias_.data(),
-            metric_type == METRIC_L2 ? perm_.data() : nullptr, tileMaxBias_.data(), yScale_, yMaxNorm_, this->ntotal, d,
-            dpad_, k, metric_type, dDev, iDev, stream, flatShard, yHalf_());
+            metric == METRIC_L2 ? perm_.data() : nullptr, tileMaxBias_.data(), yScale_, yMaxNorm_, this->ntotal, d,
+            dpad_, k, metric, dDev, iDev, stream, flatShard, yHalf_());
     lastSearchUsedTensorCores = 1;
     lastSearchFallbackQueries = lastFlatTcFallbacks();
 }
@@ -888,7 +905,14 @@ float Clustering::lloyd_(
     return obj;
 }
 
+// the assignment step runs on the L2 / inner-product tensor-core path; the other metrics are not clustered
+static void checkClusteringMetric(const GpuIndexFlat& index) {
+    if (!(index.metric_type == METRIC_L2 || index.metric_type == METRIC_INNER_PRODUCT))
+        FB_THROW_FMT("unsupported metric type %d", (int)index.metric_type);
+}
+
 void Clustering::train(idx_t nx, const float* x_in, GpuIndexFlat& index) {
+    checkClusteringMetric(index);
     FB_THROW_IF_NOT_FMT(
             nx >= (idx_t)k,
             "Number of training points (%ld) should be at least as large as number of clusters (%zd)",
@@ -935,7 +959,7 @@ void Clustering::train(idx_t nx, const float* x_in, GpuIndexFlat& index) {
         printf("Clustering %ld points in %zdD to %zd clusters, redo %d times, %d iterations\n",
                (long)nx, d, k, nredo, niter);
 
-    const bool lower_is_better = index.metric_type == METRIC_L2;
+    const bool lower_is_better = !is_similarity_metric(index.metric_type);
     float best_obj = lower_is_better ? HUGE_VALF : -HUGE_VALF;
     std::vector<ClusteringIterationStats> best_stats;
     std::vector<float> best_centroids;
@@ -960,6 +984,7 @@ void Clustering::train(idx_t nx, const float* x_in, GpuIndexFlat& index) {
 }
 
 void Clustering::trainSharded(idx_t nLocal, const float* x_in, GpuIndexFlat& index, const Communicator& comm) {
+    checkClusteringMetric(index);
     FB_THROW_IF_NOT_FMT((size_t)index.d == d, "Index dimension %d not the same as data dimension %d", index.d, (int)d);
     FB_THROW_IF_NOT_MSG(!frozen_centroids, "Clustering: frozen_centroids (input centroids) is not supported by faiss_b200");
     FB_THROW_IF_NOT_MSG(nredo == 1, "sharded clustering supports nredo == 1");
@@ -1225,6 +1250,9 @@ GpuIndexIVF::GpuIndexIVF(
         GpuIndexIVFConfig config,
         bool pqInterleaved)
         : GpuIndex(std::move(resources), dims, metric, 0, config), nlist(nlist_), ivfConfig_(config) {
+    // faiss/gpu/GpuIndexIVF.cu:34-38: only L2 and inner product
+    if (!(metric == METRIC_L2 || metric == METRIC_INNER_PRODUCT))
+        FB_THROW_FMT("unsupported metric type %d", (int)metric);
     FB_THROW_IF_NOT_MSG(nlist > 0, "nlist must be > 0");
     // faiss/gpu/GpuIndexIVF.cu:72-80: spherical k-means for inner product, 10 iterations
     if (metric == METRIC_INNER_PRODUCT)
@@ -2022,7 +2050,7 @@ void merge_knn_results_host(
     // (faiss/utils/Heap.cpp:166-238)
     if (k == 0)
         return;
-    const bool l2 = metric == METRIC_L2;
+    const bool l2 = !is_similarity_metric(metric); // lower is better (faiss/IndexShards.cpp:246 tests METRIC_L2 only)
     const size_t stride = (size_t)n * k;
     for (idx_t i = 0; i < n; i++) {
         std::vector<idx_t> ptr(nshard, 0);

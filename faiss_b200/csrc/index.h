@@ -277,6 +277,13 @@ class GpuIndexFlat : public GpuIndex {
     void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) override;
     void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const override;
     void prepareTensorCoreData_() const;
+    // the metric the kernels run, read at search time: METRIC_Lp with metric_arg 1 is L1 and with 2 is L2
+    // (faiss/gpu/impl/Distance.cuh:223-239); only L2 and inner product can take the tensor-core path
+    MetricType searchMetric_() const;
+    bool tensorCoreMetric_() const {
+        const MetricType m = searchMetric_();
+        return m == METRIC_L2 || m == METRIC_INNER_PRODUCT;
+    }
 
     const void* rows_() const { // the stored rows, as the kernels take them (with yHalf_())
         return flatConfig_.useFloat16 ? (const void*)vecs16_.data() : (const void*)vecs_.data();
