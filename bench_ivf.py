@@ -3,9 +3,13 @@
 headline; bench.py is).  BASELINE.json configs[3]: GpuIndexIVFPQ N=100M d=128 nlist=4096 m=32
 nbits=8 nprobe=32 nq=10k k=100; configs[2]: GpuIndexIVFFlat N=10M nlist=4096 nprobe=64.
 
-  python bench_ivf.py --index ivfpq  [--n 100000000] [--steps 5]
+  python bench_ivf.py --index ivfpq  [--n 100000000] [--steps 5] [--nbits 4 --m 64]
   python bench_ivf.py --index ivfflat [--n 10000000]
   python bench_ivf.py --index ivfsq --qtype 8bit   (IVF-Flat config; --qtype one of QTYPES)
+
+--nbits 4/5/6 builds the IVF-PQ index with interleaved_layout (4-bit with M in {32, 64}: the nibble-pair scan,
+kernel "ivfpq_scan"; other shapes: the packed scan, kernel "ivfpq_scan_packed").  --dump-outputs DIR writes the
+last timed step's result (distances.npy, labels.npy), as bench.py does.
 
 Prints one JSON line: QPS (device-resident queries), e2e QPS (host buffers), and the HBM roofline of
 the scan kernel: algorithmic bytes = sum over (query, probe) of listLen * code_size, divided by the
@@ -40,12 +44,14 @@ def main():
     ap.add_argument("--d", type=int, default=128)
     ap.add_argument("--nlist", type=int, default=4096)
     ap.add_argument("--m", type=int, default=32)
+    ap.add_argument("--nbits", type=int, default=8, help="bits per PQ code (--index ivfpq)")
     ap.add_argument("--nprobe", type=int, default=None)
     ap.add_argument("--nq", type=int, default=10000)
     ap.add_argument("--k", type=int, default=100)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--ntrain", type=int, default=1 << 20)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's distances and labels as DIR/<name>.npy")
     ap.add_argument("--recall-queries", type=int, default=100, help="queries checked against exact fp32 ground truth (0 = skip)")
     args = ap.parse_args()
     N = args.n or (100_000_000 if args.index == "ivfpq" else 10_000_000)
@@ -68,9 +74,13 @@ def main():
         return torch.rand((n, d), dtype=torch.float32, device=dev, generator=g)
 
     if args.index == "ivfpq":
-        index = fb.GpuIndexIVFPQ(res, d, args.nlist, args.m, 8, fb.METRIC_L2)
-        code_size = args.m
-        kname = b"ivfpq_scan"
+        if args.nbits == 8:
+            index = fb.GpuIndexIVFPQ(res, d, args.nlist, args.m, 8, fb.METRIC_L2)
+        else:
+            index = fb.GpuIndexIVFPQ(res, d, args.nlist, args.m, args.nbits, fb.METRIC_L2, interleaved_layout=True)
+        code_size = (args.m * args.nbits + 7) // 8
+        nibble_pairs = args.nbits == 4 and args.m in (32, 64)
+        kname = b"ivfpq_scan" if args.nbits == 8 or nibble_pairs else b"ivfpq_scan_packed"
     elif args.index == "ivfflat":
         index = fb.GpuIndexIVFFlat(res, d, args.nlist, fb.METRIC_L2)
         code_size = 4 * d
@@ -131,6 +141,10 @@ def main():
     fb.lib.faiss_b200_kernel_timing_collect(kname, ctypes.byref(kms), ctypes.byref(kn))
     fb.lib.faiss_b200_kernel_timing(0)
     clocks = sampler.stop()
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "distances.npy"), D.cpu().numpy().astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "labels.npy"), I.cpu().numpy().astype(np.float64))  # ids < 2^53: exact
 
     for _ in range(2):
         index.search(xq_pin.numpy(), k, D=D_pin.numpy(), I=I_pin.numpy())
@@ -168,9 +182,9 @@ def main():
         roof.update({"achieved": alg_bytes / (kms_step * 1e-3) / 1e9, "kernel_ms_per_step": kms_step, "kernel_share_of_step": kms_step / ms})
         roof["frac"] = roof["achieved"] / roof["peak"]
     out = {"metric": "queries/sec (%s)" % args.index, "value": nq / (ms * 1e-3), "unit": "queries/s", "n_gpus": 1, "steps": args.steps,
-           "warmup": max(3, args.warmup), "ms_per_step": ms, "higher_is_better": True, "dtype": {"ivfpq": "u8 codes, f32 LUT", "ivfflat": "f32", "ivfsq": "SQ %s codes" % args.qtype}[args.index],
+           "warmup": max(3, args.warmup), "ms_per_step": ms, "higher_is_better": True, "dtype": {"ivfpq": "%d-bit codes, f32 LUT" % args.nbits if args.nbits != 8 else "u8 codes, f32 LUT", "ivfflat": "f32", "ivfsq": "SQ %s codes" % args.qtype}[args.index],
            "data": "synthetic", "config": {"workload": "%s N=%d d=%d nlist=%d %snprobe=%d nq=%d k=%d" % (
-               args.index, N, d, args.nlist, ("M=%d nbits=8 " % args.m) if args.index == "ivfpq" else ("qtype=%s " % args.qtype) if args.index == "ivfsq" else "", nprobe, nq, k),
+               args.index, N, d, args.nlist, ("M=%d nbits=%d " % (args.m, args.nbits)) if args.index == "ivfpq" else ("qtype=%s " % args.qtype) if args.index == "ivfsq" else "", nprobe, nq, k),
                "list_len_mean": float(lens.mean()), "list_len_max": int(lens.max()), "train_s": t_train, "add_s": t_add, "add_vec_per_s": N / t_add},
            "clocks": clocks, "e2e": {"value": nq / (e2e_ms * 1e-3), "unit": "queries/s", "ms_per_step": e2e_ms,
                                      "h2d_bytes_per_step": nq * d * 4, "d2h_bytes_per_step": nq * k * 12},

@@ -8,7 +8,7 @@ helpers work on that payload (numpy arrays), so any producer of the format -- th
 a file reader -- can feed them; nothing here depends on the reference's classes.
 
     payload = {"d", "nlist", "metric", "centroids" [nlist, d] f32,
-               "pq" [M, 256, dsub] f32 (IVFPQ only),
+               "pq" [M, 2^nbits, dsub] f32 (IVFPQ only; nbits != 8 builds the index with interleaved_layout),
                "sq" {"qtype", "by_residual", "trained" f32} (IVF scalar quantiser only: ScalarQuantizer::trained),
                "codes": [nlist] uint8 arrays, "ids": [nlist] int64 arrays}
 """
@@ -54,6 +54,15 @@ def shard_ivf_lists(codes, ids, code_size, nshard, shard_type=SHARD_BY_ID_MOD, n
     return out
 
 
+def _pq_nbits(pq):
+    """nbits of PQ centroids [M, 2^nbits, dsub]"""
+    ksub = int(pq.shape[1])
+    nbits = ksub.bit_length() - 1
+    if ksub != 1 << nbits:
+        raise ValueError("PQ centroids: %d centroids per sub-quantizer is not a power of two" % ksub)
+    return nbits
+
+
 def gpu_ivf_from_payload(res, payload, device=0):
     """GpuIndexIVFFlat / GpuIndexIVFPQ / GpuIndexIVFScalarQuantizer holding exactly the payload (the role of
     copyFrom, faiss/gpu/GpuIndexIVFPQ.cu:105-217, GpuIndexIVFFlat.cu:89-150, GpuIndexIVFScalarQuantizer.cu:126-210)."""
@@ -69,7 +78,11 @@ def gpu_ivf_from_payload(res, payload, device=0):
         index.setTrained(np.asarray(sq.get("trained", []), dtype=np.float32))
     elif "pq" in payload and payload["pq"] is not None:
         pq = np.ascontiguousarray(payload["pq"], dtype=np.float32)
-        index = fb.GpuIndexIVFPQ(res, d, nlist, int(pq.shape[0]), 8, metric, device=device)
+        M, nbits = int(pq.shape[0]), _pq_nbits(pq)
+        if nbits == 8:
+            index = fb.GpuIndexIVFPQ(res, d, nlist, M, 8, metric, device=device)
+        else:  # the reference GPU index takes 4-, 5- and 6-bit codes only with GpuIndexIVFPQConfig::interleavedLayout
+            index = fb.GpuIndexIVFPQ(res, d, nlist, M, nbits, metric, device=device, interleaved_layout=True)
         index.setCoarseCentroids(payload["centroids"])
         index.setPQCentroids(pq)
     else:
@@ -108,7 +121,11 @@ def gpu_ivf_shards_from_payload(resources, payload, shard_type=SHARD_BY_ID_MOD, 
                     sub_index.setList(l, ci[l], ii[l])
             shards.add_shard(sub_index)
         return shards
-    code_size = int(payload["pq"].shape[0]) if payload.get("pq") is not None else 4 * int(payload["d"])
+    if payload.get("pq") is not None:
+        pq = payload["pq"]
+        code_size = (int(pq.shape[0]) * _pq_nbits(pq) + 7) // 8  # ProductQuantizer::code_size
+    else:
+        code_size = 4 * int(payload["d"])
     parts = shard_ivf_lists(payload["codes"], payload["ids"], code_size, n, shard_type)
     shards = fb.IndexShards(int(payload["d"]), threaded=threaded, successive_ids=False)
     for r, dev, (ci, ii) in zip(resources, devices, parts):

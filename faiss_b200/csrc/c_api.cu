@@ -500,6 +500,35 @@ int faiss_GpuIndexIVFPQ_new(
     }
     CATCH_AND_HANDLE
 }
+// GpuIndexIVFPQConfig::interleavedLayout (faiss/gpu/GpuIndexIVFPQ.h:36-40): with it nbits may be 4, 5, 6 or 8
+int faiss_GpuIndexIVFPQ_new_with_config(
+        FaissGpuIndex** p,
+        FaissStandardGpuResources* r,
+        FaissGpuIndex* coarse,
+        int d,
+        idx_t nlist,
+        idx_t M,
+        idx_t nbits,
+        FaissMetricType metric,
+        int device,
+        int interleaved_layout) {
+    try {
+        auto res = RES(r);
+        GpuIndexIVFPQConfig cfg;
+        cfg.device = device;
+        cfg.interleavedLayout = interleaved_layout != 0;
+        auto* h = new FaissIndex_H{nullptr, res};
+        try {
+            h->index = coarse ? new GpuIndexIVFPQ(res, AS<GpuIndexFlat>(coarse, "GpuIndexFlat"), d, nlist, M, nbits, MT_L2IP(metric), cfg)
+                              : new GpuIndexIVFPQ(res, d, nlist, M, nbits, MT_L2IP(metric), cfg);
+        } catch (...) {
+            delete h;
+            throw;
+        }
+        *p = h;
+    }
+    CATCH_AND_HANDLE
+}
 int faiss_GpuIndexIVFPQ_setPQCentroids(FaissGpuIndex* p, const float* c) {
     try {
         AS<GpuIndexIVFPQ>(p, "GpuIndexIVFPQ")->setPQCentroids(c);
@@ -990,7 +1019,7 @@ int faiss_b200_pq_train(
             CUDA_VERIFY(cudaMemcpyAsync(hold.data, x, sizeof(float) * n * d, cudaMemcpyDefault, stream));
             xd = hold.as<float>();
         }
-        trainProductQuantizer(res, device, (idx_t)n, xd, (int)d, (int)M, cp, centroids_out);
+        trainProductQuantizer(res, device, (idx_t)n, xd, (int)d, (int)M, 256, cp, centroids_out);
     }
     CATCH_AND_HANDLE
 }
@@ -1242,7 +1271,7 @@ int b200_ivfpq_scan(
         auto res = RES(r);
         DeviceScope s(device);
         FB_THROW_IF_NOT(k >= 1 && k <= kMaxK && nprobe >= 1 && nprobe <= kMaxNprobe);
-        runIvfPqScan(res.get(), device, Q, nq, d, probes, coarse_dis, nprobe, coarse_centroids, pq_centroids, M, list_start, list_len, arena_codes, arena_ids, k, MT_L2IP(metric), D, I, res->getDefaultStream(device));
+        runIvfPqScan(res.get(), device, Q, nq, d, probes, coarse_dis, nprobe, coarse_centroids, pq_centroids, M, 8, list_start, list_len, arena_codes, arena_ids, k, MT_L2IP(metric), D, I, res->getDefaultStream(device));
     }
     CATCH_AND_HANDLE
 }

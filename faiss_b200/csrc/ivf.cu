@@ -137,6 +137,32 @@ void runPQEncode(
     CUDA_CHECK_LAST();
 }
 
+// PQEncoderGeneric (faiss/impl/ProductQuantizer-inl.h): the M codes of a vector, nbits each, LSB-first in a
+// bitstring of ceil(M * nbits / 8) bytes.  One thread per output byte, so no byte is written twice.
+__global__ void pq_pack_kernel(const uint8_t* __restrict__ codes, int64_t n, int M, int nbits, int codeSize, uint8_t* __restrict__ out) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n * codeSize)
+        return;
+    const int64_t i = e / codeSize;
+    const int b = (int)(e - i * codeSize);
+    const uint8_t* c = codes + i * M;
+    unsigned acc = 0;
+    for (int m = (b * 8) / nbits; m < M && m * nbits < (b + 1) * 8; m++) {
+        const int shift = m * nbits - b * 8; // bit position of code m relative to byte b (negative: starts earlier)
+        acc |= shift >= 0 ? (unsigned)c[m] << shift : (unsigned)c[m] >> -shift;
+    }
+    out[e] = (uint8_t)acc;
+}
+
+void runPQPack(const uint8_t* codes, int64_t n, int M, int nbits, uint8_t* packed, cudaStream_t stream) {
+    if (n == 0)
+        return;
+    FB_THROW_IF_NOT(nbits >= 1 && nbits <= 8);
+    const int codeSize = (M * nbits + 7) / 8;
+    pq_pack_kernel<<<(unsigned)ceil_div(n * codeSize, (int64_t)256), 256, 0, stream>>>(codes, n, M, nbits, codeSize, packed);
+    CUDA_CHECK_LAST();
+}
+
 // ------------------------------------------------------------------------------------------
 // append bookkeeping
 // ------------------------------------------------------------------------------------------
@@ -513,9 +539,10 @@ void runIvfFlatScan(
 }
 
 // ------------------------------------------------------------------------------------------
-// IVF-PQ scan: block per (query, probe)
+// IVF-PQ scan: block per (query, probe).  PACKED: codes of ksub = 2^nbits < 256 centroids, stored as the CPU's
+// LSB-first bitstring of ceil(M * nbits / 8) bytes per vector; each lane decodes its vector from a 64-bit window.
 // ------------------------------------------------------------------------------------------
-template <bool IS_L2>
+template <bool IS_L2, bool PACKED>
 __global__ void __launch_bounds__(kScanWarps * 32) ivfpq_scan_kernel(
         const float* __restrict__ Q,
         int d,
@@ -580,14 +607,37 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfpq_scan_kernel(
     __syncthreads();
 
     const int len = listLen[l];
-    const uint8_t* codes = arenaCodes + listStart[l] * (int64_t)M;
+    const int nbits = PACKED ? 31 - __clz(ksub) : 8;
+    const int codeSize = PACKED ? (M * nbits + 7) >> 3 : M;
+    const uint8_t* codes = arenaCodes + listStart[l] * (int64_t)codeSize;
     const bool vec16 = (M % 16) == 0; // list starts are multiples of 16 elements when M%16==0
     for (int v0 = threadIdx.x; v0 < round_up(len, 32); v0 += blockDim.x) {
         const bool valid = v0 < len;
         float acc = 0.f;
         if (valid) {
-            const uint8_t* cp = codes + (int64_t)v0 * M;
-            if (vec16) {
+            const uint8_t* cp = codes + (int64_t)v0 * codeSize;
+            if (PACKED) {
+                // bits [0, have) of win are the next codes; refilled 32 bits at a time (have < nbits <= 8, so
+                // the window never overflows), bytes past the row's end read as zero
+                const unsigned mask = (unsigned)ksub - 1;
+                uint64_t win = 0;
+                int have = 0, pos = 0;
+                for (int m = 0; m < M; m++) {
+                    if (have < nbits) {
+                        unsigned w = 0;
+#pragma unroll
+                        for (int b = 0; b < 4; b++)
+                            if (pos + b < codeSize)
+                                w |= (unsigned)__ldg(cp + pos + b) << (8 * b);
+                        win |= (uint64_t)w << have;
+                        have += 32;
+                        pos += 4;
+                    }
+                    acc += lut[m * ksub + ((unsigned)win & mask)];
+                    win >>= nbits;
+                    have -= nbits;
+                }
+            } else if (vec16) {
                 for (int m0 = 0; m0 < M; m0 += 16) {
                     const uint4 c4 = __ldg(reinterpret_cast<const uint4*>(cp + m0));
                     const unsigned wds[4] = {c4.x, c4.y, c4.z, c4.w};
@@ -624,6 +674,7 @@ void runIvfPqScan(
         const float* coarseCentroids,
         const float* pqCentroids,
         int M,
+        int nbits,
         const int64_t* listStart,
         const int* listLen,
         const uint8_t* arenaCodes,
@@ -635,7 +686,10 @@ void runIvfPqScan(
         cudaStream_t stream) {
     if (nq == 0)
         return;
-    const int ksub = 256;
+    FB_THROW_IF_NOT(nbits >= 1 && nbits <= 8);
+    const int ksub = 1 << nbits;
+    const bool packed = nbits != 8;
+    const char* name = packed ? "ivfpq_scan_packed" : "ivfpq_scan";
     const int LIST = std::max(64, next_pow2(k));
     size_t smem = sizeof(float) * M * ksub + round_up(sizeof(float) * d, 16) +
             SmemTopK<int>::bytes(LIST, kScanBuf) * kScanWarps;
@@ -646,21 +700,28 @@ void runIvfPqScan(
         auto partD = res->temp(device, sizeof(float) * nb * nprobe * k);
         auto partI = res->temp(device, sizeof(idx_t) * nb * nprobe * k);
         dim3 grid((unsigned)nprobe, (unsigned)nb);
-        KernelTiming::begin("ivfpq_scan", stream);
+        KernelTiming::begin(name, stream);
+#define SCAN(L2_, PK_)                                                                                              \
+    do {                                                                                                            \
+        CUDA_VERIFY(cudaFuncSetAttribute(                                                                           \
+                ivfpq_scan_kernel<L2_, PK_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
+        ivfpq_scan_kernel<L2_, PK_><<<grid, kScanWarps * 32, smem, stream>>>(                                       \
+                Q + q0 * d, d, probes + q0 * nprobe, coarseDis + q0 * nprobe, nprobe, coarseCentroids, pqCentroids, \
+                M, ksub, listStart, listLen, arenaCodes, arenaIds, k, LIST, partD.as<float>(), partI.as<idx_t>());  \
+    } while (0)
         if (metric == METRIC_L2) {
-            CUDA_VERIFY(cudaFuncSetAttribute(
-                    ivfpq_scan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            ivfpq_scan_kernel<true><<<grid, kScanWarps * 32, smem, stream>>>(
-                    Q + q0 * d, d, probes + q0 * nprobe, coarseDis + q0 * nprobe, nprobe, coarseCentroids, pqCentroids,
-                    M, ksub, listStart, listLen, arenaCodes, arenaIds, k, LIST, partD.as<float>(), partI.as<idx_t>());
+            if (packed)
+                SCAN(true, true);
+            else
+                SCAN(true, false);
         } else {
-            CUDA_VERIFY(cudaFuncSetAttribute(
-                    ivfpq_scan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            ivfpq_scan_kernel<false><<<grid, kScanWarps * 32, smem, stream>>>(
-                    Q + q0 * d, d, probes + q0 * nprobe, coarseDis + q0 * nprobe, nprobe, coarseCentroids, pqCentroids,
-                    M, ksub, listStart, listLen, arenaCodes, arenaIds, k, LIST, partD.as<float>(), partI.as<idx_t>());
+            if (packed)
+                SCAN(false, true);
+            else
+                SCAN(false, false);
         }
-        KernelTiming::end("ivfpq_scan", stream);
+#undef SCAN
+        KernelTiming::end(name, stream);
         CUDA_CHECK_LAST();
         runMergeTopKKeyspace(
                 partD.as<float>(), partI.as<idx_t>(), nb, nprobe, k, k, metric, 0, outD + q0 * k, outI + q0 * k, stream);

@@ -112,7 +112,10 @@ __device__ __forceinline__ float lds_f32(unsigned addr) {
 // SBASE: shared-window address of the dynamic shared memory (0x400 on sm_90: the first KB of the window is
 // reserved), folded into the LDS immediate so that the PRMT result IS the address; -1 = unknown (one extra
 // IADD per lookup).
-template <int M, bool IS_L2, bool PRECOMP, typename IdT, int SBASE>
+// NIB (table-build policy): 4-bit PQ with MQ = 2M sub-quantisers whose nibble pairs are the M code bytes.  The
+// 16 x MQ direct entries are built first (into `dir`), then each of the 256 x M table entries is the sum of two
+// of them, T'[j][b] = T[2j][b & 15] + T[2j+1][b >> 4]; everything after the build is the 8-bit kernel's.
+template <int M, bool IS_L2, bool PRECOMP, typename IdT, int SBASE, bool NIB>
 __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_interleaved_kernel(
         const float* __restrict__ Q,
         int d,
@@ -132,19 +135,22 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
         float* __restrict__ partD,
         idx_t* __restrict__ partI) {
     static_assert(!PRECOMP || IS_L2, "precomputed tables are an L2 decomposition");
+    static_assert(!PRECOMP || !NIB, "no precomputed tables for 4-bit codes");
     static_assert((kScanWarps & (kScanWarps - 1)) == 0, "kScanWarps must be a power of two");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr int kThreads = kScanWarps * 32;
     constexpr int kU = M == 32 ? 4 : 8;      // groups of 32 vectors per work unit: 4 KB of codes in flight per warp
     constexpr int H = M / 16;                // 16-byte words per lane and group
     constexpr int kEntriesPerThread = 256 * M / kThreads;
+    constexpr int MQ = NIB ? 2 * M : M; // sub-quantisers
     static_assert(256 * M % kThreads == 0, "LUT entries must divide evenly among the threads");
     const int q = blockIdx.y, chunk = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = lane_id();
-    const int dsub = d / M;
+    const int dsub = d / MQ;
     float* lut = reinterpret_cast<float*>(smem_raw);                 // [256][2][32]
     float* rs = lut + 256 * 64;                                      // [2][d] residuals of the probe pair / [d] query
-    int* ctl = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(rs) + round_up(sizeof(float) * 2 * d, 16));
+    float* dir = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(rs) + round_up(sizeof(float) * 2 * d, 16)); // NIB: [2][16][MQ]
+    int* ctl = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(dir) + (NIB ? sizeof(float) * 2 * 16 * MQ : 0));
     float* t1s = reinterpret_cast<float*>(ctl + 2);                  // [2] ||x - c||^2 of the pair (PRECOMP)
     unsigned char* listMem = reinterpret_cast<unsigned char*>(ctl) + 16;
     float* oD = partD + ((int64_t)q * gridDim.x + chunk) * k;
@@ -162,7 +168,7 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
     // direct LUT entry e = c*M + m from a vector r[d] in shared memory:
     //   L2: ||r|m - y||^2 (r = query - list centroid);  IP / PRECOMP term 3: <r|m, y> (r = query)
     auto entry = [&](const float* r, int e, bool l2form) {
-        const int c = e / M, m = e - c * M;
+        const int c = e / MQ, m = e - c * MQ;
         const float* cp = pqT + (size_t)e * dsub;
         const float* rp = r + m * dsub;
         float acc = 0.f;
@@ -201,6 +207,21 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
 #pragma unroll
         for (int s = 0; s < 32; s += M)
             lut[c * 64 + buf * 32 + s + m] = val;
+    };
+    // NIB: the 16 x MQ direct entries of table `buf` from r (IP: negated, as the 8-bit tables) ...
+    auto directBuild = [&](int buf, const float* r, bool l2form) {
+        for (int e = threadIdx.x; e < 16 * MQ; e += kThreads) {
+            const float v = entry(r, e, l2form);
+            dir[buf * 16 * MQ + e] = l2form ? v : -v;
+        }
+    };
+    // ... and, after a barrier, the 256 x M pair sums
+    auto pairBuild = [&](int buf) {
+        const float* t = dir + buf * 16 * MQ;
+        for (int e = threadIdx.x; e < 256 * M; e += kThreads) {
+            const int c = e / M, j = e - c * M;
+            store(buf, e, t[(c & 15) * MQ + 2 * j] + t[(c >> 4) * MQ + 2 * j + 1]);
+        }
     };
 
     // 32 vectors (one group, this lane's vector): sum of its M table entries in table `buf` (0 / 1: a runtime
@@ -280,14 +301,20 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
         for (int i = threadIdx.x; i < d; i += kThreads)
             rs[i] = Q[(int64_t)q * d + i];
         __syncthreads();
+        if (NIB) {
+            directBuild(0, rs, false);
+            __syncthreads();
+            pairBuild(0);
+        } else {
 #pragma unroll
-        for (int i = 0; i < kEntriesPerThread; i++) {
-            const int e = threadIdx.x + i * kThreads;
-            const float dot = entry(rs, e, false);
-            if (PRECOMP)
-                t3[i] = -2.f * dot;
-            else
-                store(0, e, -dot);
+            for (int i = 0; i < kEntriesPerThread; i++) {
+                const int e = threadIdx.x + i * kThreads;
+                const float dot = entry(rs, e, false);
+                if (PRECOMP)
+                    t3[i] = -2.f * dot;
+                else
+                    store(0, e, -dot);
+            }
         }
     }
     __syncthreads(); // list initialised (and the IP table built)
@@ -317,8 +344,19 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
                 }
             }
             __syncthreads(); // every warp is done with the previous pair's tables; residuals visible
+            if (NIB) {
 #pragma unroll
-            for (int s = 0; s < 2; s++) {
+                for (int s = 0; s < 2; s++)
+                    if (len[s] != 0)
+                        directBuild(s, rs + s * d, true);
+                __syncthreads();
+#pragma unroll
+                for (int s = 0; s < 2; s++)
+                    if (len[s] != 0)
+                        pairBuild(s);
+            }
+#pragma unroll
+            for (int s = 0; s < 2 && !NIB; s++) {
                 if (len[s] == 0)
                     continue;
                 if (PRECOMP) {
@@ -506,7 +544,7 @@ static int probedSmemBase(int device, cudaStream_t stream) {
     return (int)h;
 }
 
-template <int M, bool IS_L2, bool PRECOMP, typename IdT>
+template <int M, bool IS_L2, bool PRECOMP, typename IdT, bool NIB>
 static void launchScan(
         int smemBase,
         dim3 grid,
@@ -530,8 +568,8 @@ static void launchScan(
         float* partD,
         idx_t* partI) {
     // any other shared-window base than the expected one: generic addressing
-    auto kern = smemBase == kExpectedSmemBase ? ivfpq_scan_interleaved_kernel<M, IS_L2, PRECOMP, IdT, kExpectedSmemBase>
-                                              : ivfpq_scan_interleaved_kernel<M, IS_L2, PRECOMP, IdT, -1>;
+    auto kern = smemBase == kExpectedSmemBase ? ivfpq_scan_interleaved_kernel<M, IS_L2, PRECOMP, IdT, kExpectedSmemBase, NIB>
+                                              : ivfpq_scan_interleaved_kernel<M, IS_L2, PRECOMP, IdT, -1, NIB>;
     CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTiming::begin("ivfpq_scan", stream);
     kern<<<grid, kScanWarps * 32, smem, stream>>>(
@@ -554,6 +592,7 @@ void runIvfPqScanInterleaved(
         const float* pqCentroidsT,
         const float* term2,
         int M,
+        bool nibble,
         const int64_t* listStart,
         const int* listLen,
         const uint8_t* arenaCodes,
@@ -567,11 +606,13 @@ void runIvfPqScanInterleaved(
     if (nq == 0)
         return;
     FB_THROW_IF_NOT(ivfPqInterleavedSupported(M));
+    FB_THROW_IF_NOT(!nibble || term2 == nullptr);
     const int LIST = std::max(CtaTopK<int>::BUF, next_pow2(k)); // a sorted buffer (<= BUF entries) is merged into the list
     const bool wide = arenaElems >= (int64_t(1) << 31) - 1; // arena positions need 64-bit list ids
     const int smemBase = probedSmemBase(device, stream);
     const size_t listBytes = wide ? CtaTopK<long long>::bytes(LIST, kScanWarps) : CtaTopK<int>::bytes(LIST, kScanWarps);
-    size_t smem = sizeof(float) * 256 * kLutSlots + round_up(sizeof(float) * 2 * d, 16) + 16 + listBytes;
+    size_t smem = sizeof(float) * 256 * kLutSlots + round_up(sizeof(float) * 2 * d, 16) + 16 + listBytes +
+            (nibble ? sizeof(float) * 2 * 16 * 2 * M : 0);
     FB_THROW_IF_NOT_MSG(smem <= 220 * 1024, "LUT + top-k lists do not fit shared memory");
     const bool l2 = metric == METRIC_L2;
     int probesPerCta = 1;
@@ -582,33 +623,45 @@ void runIvfPqScanInterleaved(
         auto partD = res->temp(device, sizeof(float) * nb * chunks * k);
         auto partI = res->temp(device, sizeof(idx_t) * nb * chunks * k);
         dim3 grid((unsigned)chunks, (unsigned)nb);
-#define SCAN(M_, L2_, PRE_, ID_)                                                                                   \
-    launchScan<M_, L2_, PRE_, ID_>(                                                                                \
+#define SCAN(M_, L2_, PRE_, ID_, NIB_)                                                                             \
+    launchScan<M_, L2_, PRE_, ID_, NIB_>(                                                                              \
             smemBase, grid, smem, stream, Q + q0 * d, d, probes + q0 * nprobe, coarseDis + q0 * nprobe, nprobe, probesPerCta, \
             coarseCentroids, pqCentroidsT, term2, listStart, listLen, arenaCodes, arenaIds, k, LIST,               \
             partD.as<float>(), partI.as<idx_t>())
-#define SCAN_ID(M_, L2_, PRE_)          \
-    do {                                \
-        if (wide)                       \
-            SCAN(M_, L2_, PRE_, long long); \
-        else                            \
-            SCAN(M_, L2_, PRE_, int);   \
+#define SCAN_ID(M_, L2_, PRE_, NIB_)          \
+    do {                                      \
+        if (wide)                             \
+            SCAN(M_, L2_, PRE_, long long, NIB_); \
+        else                                  \
+            SCAN(M_, L2_, PRE_, int, NIB_);   \
     } while (0)
         const bool pre = l2 && term2 != nullptr;
-        if (M == 32) {
+        if (nibble) {
+            if (M == 32) {
+                if (l2)
+                    SCAN_ID(32, true, false, true);
+                else
+                    SCAN_ID(32, false, false, true);
+            } else {
+                if (l2)
+                    SCAN_ID(16, true, false, true);
+                else
+                    SCAN_ID(16, false, false, true);
+            }
+        } else if (M == 32) {
             if (pre)
-                SCAN_ID(32, true, true);
+                SCAN_ID(32, true, true, false);
             else if (l2)
-                SCAN_ID(32, true, false);
+                SCAN_ID(32, true, false, false);
             else
-                SCAN_ID(32, false, false);
+                SCAN_ID(32, false, false, false);
         } else {
             if (pre)
-                SCAN_ID(16, true, true);
+                SCAN_ID(16, true, true, false);
             else if (l2)
-                SCAN_ID(16, true, false);
+                SCAN_ID(16, true, false, false);
             else
-                SCAN_ID(16, false, false);
+                SCAN_ID(16, false, false, false);
         }
 #undef SCAN_ID
 #undef SCAN

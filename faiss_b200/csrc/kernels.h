@@ -212,6 +212,9 @@ void runPQEncode(
         const float* pqCentroids /*[M][ksub][dsub]*/,
         uint8_t* codes /*[n][M]*/,
         cudaStream_t stream);
+// codes [n][M] (one byte each, < 2^nbits) -> packed [n][ceil(M*nbits/8)], the CPU's LSB-first bitstring
+// (PQEncoderGeneric, faiss/impl/ProductQuantizer-inl.h)
+void runPQPack(const uint8_t* codes, int64_t n, int M, int nbits, uint8_t* packed, cudaStream_t stream);
 
 // histogram of list assignments + stable scatter positions (device-side append bookkeeping;
 // replaces the host unordered_map pass of IVFBase::addVectorsToLists_, IVFBase.cu:693-905)
@@ -266,6 +269,8 @@ void runIvfFlatScan(
 // running top-k stays on chip.  Distance form follows the reference CPU scanner
 // (faiss/impl/pq_code_distance/IVFPQ_QueryTables.cpp:126-192): L2 by_residual:
 //   dis = sum_m || (q - c_list)_m - pq[m][code_m] ||^2 ; IP: q.c_list + sum_m q_m . pq[m][code_m]
+// nbits < 8: lists hold the CPU's packed bitstring, ceil(M*nbits/8) bytes per vector (kernel timing name
+// "ivfpq_scan_packed").
 void runIvfPqScan(
         GpuResources* res,
         int device,
@@ -276,8 +281,9 @@ void runIvfPqScan(
         const float* coarseDis,
         int nprobe,
         const float* coarseCentroids /*[nlist,d]*/,
-        const float* pqCentroids /*[M][ksub][dsub]*/,
+        const float* pqCentroids /*[M][2^nbits][dsub]*/,
         int M,
+        int nbits,
         const int64_t* listStart,
         const int* listLen,
         const uint8_t* arenaCodes,
@@ -380,7 +386,10 @@ void runIvfPqListFromInterleaved(const uint8_t* listCodes, int64_t len, int M, u
 void runIvfPqPrecomputeTerm2(
         const float* coarse, const float* pqT, int64_t nlist, int d, int M, float* term2, cudaStream_t stream);
 
-// scan over the interleaved layout; pqCentroidsT is the [ksub][M][dsub] transpose of pqCentroids
+// scan over the interleaved layout; pqCentroidsT is the [ksub][M][dsub] transpose of pqCentroids.
+// nibble: 4-bit PQ with M sub-quantisers stored as M/2 code bytes (nibble pairs, byte j = code 2j | code 2j+1
+// << 4), scanned as M/2 "8-bit" codes over the pair table T'[j][b] = T[2j][b & 15] + T[2j+1][b >> 4];
+// pqCentroidsT is then [16][M][dsub] and M/2 must be 16 or 32.  No precomputed tables.
 void runIvfPqScanInterleaved(
         GpuResources* res,
         int device,
@@ -394,6 +403,7 @@ void runIvfPqScanInterleaved(
         const float* pqCentroidsT,
         const float* term2, // precomputed [nlist][256][M] table (L2) or null
         int M,
+        bool nibble,
         const int64_t* listStart,
         const int* listLen,
         const uint8_t* arenaCodes,

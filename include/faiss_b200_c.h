@@ -153,8 +153,12 @@ FB200_API int faiss_GpuIndexIVFFlat_new(FaissGpuIndex** p_index, FaissStandardGp
 
 /* ---- GpuIndexIVFPQ (faiss/gpu/GpuIndexIVFPQ.h:56-181) ---- */
 FB200_API int faiss_GpuIndexIVFPQ_new(FaissGpuIndex** p_index, FaissStandardGpuResources* res, int d, idx_t nlist, idx_t M, idx_t nbits, FaissMetricType metric, int device);
-FB200_API int faiss_GpuIndexIVFPQ_setPQCentroids(FaissGpuIndex* index, const float* centroids /* [M][256][dsub] */);
-FB200_API int faiss_GpuIndexIVFPQ_getPQCentroids(const FaissGpuIndex* index, float* centroids_out);
+/* GpuIndexIVFPQConfig::interleavedLayout (faiss/gpu/GpuIndexIVFPQ.h:36-40): with interleaved_layout != 0, nbits
+   may be 4, 5, 6 or 8 (else only 8); lists hold ceil(M * nbits / 8) code bytes per vector, the CPU's packed
+   bitstring.  coarse: a GpuIndexFlat to share as the coarse quantizer, or NULL. */
+FB200_API int faiss_GpuIndexIVFPQ_new_with_config(FaissGpuIndex** p_index, FaissStandardGpuResources* res, FaissGpuIndex* coarse /* nullable */, int d, idx_t nlist, idx_t M, idx_t nbits, FaissMetricType metric, int device, int interleaved_layout);
+FB200_API int faiss_GpuIndexIVFPQ_setPQCentroids(FaissGpuIndex* index, const float* centroids /* [M][2^nbits][dsub] */);
+FB200_API int faiss_GpuIndexIVFPQ_getPQCentroids(const FaissGpuIndex* index, float* centroids_out /* [M][2^nbits][dsub] */);
 FB200_API int faiss_GpuIndexIVFPQ_set_pq_clustering(FaissGpuIndex* index, int niter, int seed, int max_points_per_centroid);
 /* GpuIndexIVFPQ::setPrecomputedCodes (faiss/gpu/GpuIndexIVFPQ.h:114-118): force the precomputed term-2 table
    ([nlist][256][M] floats, L2 only) on or off; untouched, the index follows the CPU reference's "auto" size
