@@ -41,10 +41,6 @@
 #include "flat_tc_kernel.cuh"
 
 namespace fb200 {
-
-void runMergeTopKKeyspace(
-        const float*, const idx_t*, int64_t, int, int, int, MetricType, int64_t, float*, idx_t*, cudaStream_t);
-
 namespace {
 
 using namespace tc;

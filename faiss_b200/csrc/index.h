@@ -507,6 +507,8 @@ class GpuIndexIVF : public GpuIndex {
     void getCoarseCentroids(float* out) const;
     // bulk list load (copyFrom ArrayInvertedLists): codes [len*code_size], ids [len]
     void setList(idx_t listId, idx_t len, const uint8_t* codes, const idx_t* ids);
+    // the coarse quantiser (k-means, unless it already holds nlist centroids), then the encoder (trainEncoder_)
+    void train(idx_t n, const float* x) override;
 
     // faiss/gpu/GpuIndexIVF.cu:408-488
     void search_preassigned(
@@ -527,6 +529,16 @@ class GpuIndexIVF : public GpuIndex {
     virtual bool quantizerOnlyTraining_() const {
         return true;
     }
+    // train what encodes the list entries, after the coarse quantiser (IVF-Flat: nothing)
+    virtual void trainEncoder_(idx_t /*n*/, const float* /*xDev*/) {}
+    // coarse k = 1 assignment, encode_, append to the lists
+    void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) override;
+    // the list entries (codeSize bytes each) of n rows whose coarse assignment is assignDev; the result may live in
+    // `hold`.  Throws before anything is appended when the encoder is not trained.
+    virtual const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) = 0;
+    // x - (its coarse centroid).  In add, assignDev is the rows' assignment and the buffer comes from the temp stack;
+    // in training assignDev is null, the k = 1 assignment runs here, and the buffers are device allocations.
+    GpuMemoryReservation coarseResiduals_(idx_t n, const float* xDev, const idx_t* assignDev) const;
     void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const override;
     virtual void scanImpl_(
             idx_t n,
@@ -558,10 +570,9 @@ class GpuIndexIVFFlat : public GpuIndexIVF {
             idx_t nlist,
             MetricType metric = METRIC_L2,
             GpuIndexIVFConfig config = GpuIndexIVFConfig());
-    void train(idx_t n, const float* x) override;
 
    protected:
-    void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) override;
+    const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
     void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
 };
 
@@ -622,7 +633,6 @@ class GpuIndexIVFPQ : public GpuIndexIVF {
         return usePrecomputed_;
     }
     ClusteringParameters pq_cp; // ProductQuantizer::cp (faiss/impl/ProductQuantizer.h)
-    void train(idx_t n, const float* x) override;
     // PQ centroids, layout [M][ksub][dsub] (ksub = 2^nbits) as in faiss::ProductQuantizer::centroids
     void setPQCentroids(const float* c);
     void getPQCentroids(float* out) const;
@@ -631,8 +641,8 @@ class GpuIndexIVFPQ : public GpuIndexIVF {
     bool quantizerOnlyTraining_() const override {
         return false;
     }
-    void trainResidualQuantizer_(idx_t n, const float* xDev);
-    void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) override;
+    void trainEncoder_(idx_t n, const float* xDev) override; // the PQ, on residuals
+    const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
     void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
 
     int M_, nbits_;
@@ -691,7 +701,7 @@ class GpuIndexIVFScalarQuantizer : public GpuIndexIVF {
     int rangestat = 0;
     float rangestat_arg = 0.f;
 
-    void train(idx_t n, const float* x) override;
+    void train(idx_t n, const float* x) override; // rejects rangestat != RS_minmax before any training work
     // ScalarQuantizer::trained: [vmin, vdiff] (uniform types), [vmin[d], vdiff[d]] (non-uniform), empty (fp16, direct)
     void setTrained(const float* t, size_t n);
     const std::vector<float>& getTrained() const {
@@ -703,7 +713,8 @@ class GpuIndexIVFScalarQuantizer : public GpuIndexIVF {
     bool quantizerOnlyTraining_() const override {
         return trainedSize() == 0;
     }
-    void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) override;
+    void trainEncoder_(idx_t n, const float* xDev) override; // the RS_minmax ranges
+    const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
     void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
 
     int qtype_;

@@ -455,28 +455,40 @@ int ivfScanChunks(int device, int64_t nq, int nprobe, int* probesPerCta) {
     return ceil_div(nprobe, *probesPerCta);
 }
 
-template <bool IS_L2, typename IdT>
-static void launchIvfFlatScan(
-        dim3 grid,
-        size_t smem,
-        cudaStream_t stream,
-        const float* Q,
-        int d,
-        const idx_t* probes,
+void runIvfScanBatches(
+        GpuResources* res,
+        int device,
+        int64_t nq,
         int nprobe,
-        int probesPerCta,
-        const int64_t* listStart,
-        const int* listLen,
-        const float* arenaVecs,
-        const idx_t* arenaIds,
         int k,
-        int LIST,
-        float* partD,
-        idx_t* partI) {
-    auto kern = ivfflat_scan_kernel<IS_L2, IdT>;
-    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, kScanWarps * 32, smem, stream>>>(
-            Q, d, probes, nprobe, probesPerCta, listStart, listLen, arenaVecs, arenaIds, k, LIST, partD, partI);
+        MetricType metric,
+        bool oneProbePerCta,
+        const char* timingName,
+        float* outD,
+        idx_t* outI,
+        cudaStream_t stream,
+        const std::function<void(const IvfScanBatch&)>& launch) {
+    if (nq == 0)
+        return;
+    int probesPerCta = 1;
+    const int ctasPerQuery = oneProbePerCta ? nprobe : ivfScanChunks(device, nq, nprobe, &probesPerCta);
+    // query batches bound the partial-result scratch
+    const int64_t maxQ =
+            std::max<int64_t>(1, std::min<int64_t>(65535, (int64_t(1) << 30) / ((int64_t)ctasPerQuery * k * 12)));
+    for (int64_t q0 = 0; q0 < nq; q0 += maxQ) {
+        const int64_t nb = std::min(maxQ, nq - q0);
+        auto partD = res->temp(device, sizeof(float) * nb * ctasPerQuery * k);
+        auto partI = res->temp(device, sizeof(idx_t) * nb * ctasPerQuery * k);
+        const IvfScanBatch batch{
+                q0, nb, dim3((unsigned)ctasPerQuery, (unsigned)nb), probesPerCta, partD.as<float>(), partI.as<idx_t>()};
+        KernelTiming::begin(timingName, stream);
+        launch(batch);
+        KernelTiming::end(timingName, stream);
+        CUDA_CHECK_LAST();
+        runMergeTopKKeyspace(
+                partD.as<float>(), partI.as<idx_t>(), nb, ctasPerQuery, k, k, metric, 0, outD + q0 * k, outI + q0 * k,
+                stream);
+    }
 }
 
 void runIvfFlatScan(
@@ -504,38 +516,17 @@ void runIvfFlatScan(
     const size_t listBytes = wide ? SmemTopK<long long>::bytes(LIST, kScanBuf) : SmemTopK<int>::bytes(LIST, kScanBuf);
     size_t smem = round_up(sizeof(float) * d, 16) + listBytes * kScanWarps;
     FB_THROW_IF_NOT_MSG(smem <= 200 * 1024, "k / d too large for the IVF-Flat scan kernel");
-    int probesPerCta = 1;
-    const int chunks = ivfScanChunks(device, nq, nprobe, &probesPerCta);
-    // query batches bound the partial-result scratch
-    const int64_t maxQ = std::max<int64_t>(1, std::min<int64_t>(65535, (int64_t(1) << 30) / ((int64_t)chunks * k * 12)));
-    const bool l2 = metric == METRIC_L2;
-    for (int64_t q0 = 0; q0 < nq; q0 += maxQ) {
-        int64_t nb = std::min(maxQ, nq - q0);
-        auto partD = res->temp(device, sizeof(float) * nb * chunks * k);
-        auto partI = res->temp(device, sizeof(idx_t) * nb * chunks * k);
-        dim3 grid((unsigned)chunks, (unsigned)nb);
-        KernelTiming::begin("ivfflat_scan", stream);
-#define SCAN(L2_, ID_)                                                                                            \
-    launchIvfFlatScan<L2_, ID_>(                                                                                  \
-            grid, smem, stream, Q + q0 * d, d, probes + q0 * nprobe, nprobe, probesPerCta, listStart, listLen,   \
-            arenaVecs, arenaIds, k, LIST, partD.as<float>(), partI.as<idx_t>())
-        if (l2) {
-            if (wide)
-                SCAN(true, long long);
-            else
-                SCAN(true, int);
-        } else {
-            if (wide)
-                SCAN(false, long long);
-            else
-                SCAN(false, int);
-        }
-#undef SCAN
-        KernelTiming::end("ivfflat_scan", stream);
-        CUDA_CHECK_LAST();
-        runMergeTopKKeyspace(
-                partD.as<float>(), partI.as<idx_t>(), nb, chunks, k, k, metric, 0, outD + q0 * k, outI + q0 * k, stream);
-    }
+    runIvfScanBatches(res, device, nq, nprobe, k, metric, false, "ivfflat_scan", outD, outI, stream, [&](const IvfScanBatch& b) {
+        withBool(metric == METRIC_L2, [&](auto l2) {
+            withBool(wide, [&](auto wideIds) {
+                auto kern = ivfflat_scan_kernel<l2, ScanIdT<decltype(wideIds)>>;
+                CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
+                        Q + b.q0 * d, d, probes + b.q0 * nprobe, nprobe, b.probesPerCta, listStart, listLen, arenaVecs,
+                        arenaIds, k, LIST, b.partD, b.partI);
+            });
+        });
+    });
 }
 
 // ------------------------------------------------------------------------------------------
@@ -694,38 +685,17 @@ void runIvfPqScan(
     size_t smem = sizeof(float) * M * ksub + round_up(sizeof(float) * d, 16) +
             SmemTopK<int>::bytes(LIST, kScanBuf) * kScanWarps;
     FB_THROW_IF_NOT_MSG(smem <= 220 * 1024, "LUT + top-k lists do not fit shared memory (IVFPQ.cu:596-617)");
-    const int64_t maxQ = std::max<int64_t>(1, std::min<int64_t>(65535, (int64_t(1) << 30) / ((int64_t)nprobe * k * 12)));
-    for (int64_t q0 = 0; q0 < nq; q0 += maxQ) {
-        int64_t nb = std::min(maxQ, nq - q0);
-        auto partD = res->temp(device, sizeof(float) * nb * nprobe * k);
-        auto partI = res->temp(device, sizeof(idx_t) * nb * nprobe * k);
-        dim3 grid((unsigned)nprobe, (unsigned)nb);
-        KernelTiming::begin(name, stream);
-#define SCAN(L2_, PK_)                                                                                              \
-    do {                                                                                                            \
-        CUDA_VERIFY(cudaFuncSetAttribute(                                                                           \
-                ivfpq_scan_kernel<L2_, PK_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
-        ivfpq_scan_kernel<L2_, PK_><<<grid, kScanWarps * 32, smem, stream>>>(                                       \
-                Q + q0 * d, d, probes + q0 * nprobe, coarseDis + q0 * nprobe, nprobe, coarseCentroids, pqCentroids, \
-                M, ksub, listStart, listLen, arenaCodes, arenaIds, k, LIST, partD.as<float>(), partI.as<idx_t>());  \
-    } while (0)
-        if (metric == METRIC_L2) {
-            if (packed)
-                SCAN(true, true);
-            else
-                SCAN(true, false);
-        } else {
-            if (packed)
-                SCAN(false, true);
-            else
-                SCAN(false, false);
-        }
-#undef SCAN
-        KernelTiming::end(name, stream);
-        CUDA_CHECK_LAST();
-        runMergeTopKKeyspace(
-                partD.as<float>(), partI.as<idx_t>(), nb, nprobe, k, k, metric, 0, outD + q0 * k, outI + q0 * k, stream);
-    }
+    runIvfScanBatches(res, device, nq, nprobe, k, metric, true, name, outD, outI, stream, [&](const IvfScanBatch& b) {
+        withBool(metric == METRIC_L2, [&](auto l2) {
+            withBool(packed, [&](auto pk) {
+                auto kern = ivfpq_scan_kernel<l2, pk>;
+                CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
+                        Q + b.q0 * d, d, probes + b.q0 * nprobe, coarseDis + b.q0 * nprobe, nprobe, coarseCentroids,
+                        pqCentroids, M, ksub, listStart, listLen, arenaCodes, arenaIds, k, LIST, b.partD, b.partI);
+            });
+        });
+    });
 }
 
 } // namespace fb200

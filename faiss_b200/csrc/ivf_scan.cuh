@@ -1,18 +1,66 @@
-// faiss_b200 -- device helpers shared by the IVF list scans that keep per-warp top-k lists across a
-// chunk of probes (ivf.cu: IVF-Flat and the flat-layout IVF-PQ scan; ivfsq_scan.cu: IVF-SQ).
+// faiss_b200 -- helpers shared by the IVF list scans: the host-side batch-and-merge driver and template
+// dispatch of every scan launcher (ivf.cu, ivfpq_scan.cu, ivfsq_scan.cu), and the device-side block merge
+// of the scans that keep per-warp top-k lists across a chunk of probes (IVF-Flat, the flat-layout IVF-PQ
+// scan, IVF-SQ).
 #pragma once
 
 #include <cfloat>
+#include <functional>
+#include <type_traits>
 
 #include "kernels.h"
 #include "select.cuh"
 
 namespace fb200 {
 
-// the key-space merge of per-chunk partial results (flat_exact.cu) and the probe split of a scan launch (ivf.cu)
-void runMergeTopKKeyspace(
-        const float*, const idx_t*, int64_t, int, int, int, MetricType, int64_t, float*, idx_t*, cudaStream_t);
+// CTAs per query of a chunked scan: each CTA walks *probesPerCta consecutive probes of its query
 int ivfScanChunks(int device, int64_t nq, int nprobe, int* probesPerCta);
+
+// one query batch of a scan launch: queries [q0, q0 + nb), grid (CTAs per query, nb), partial results
+// [nb][CTAs per query][k] in key space
+struct IvfScanBatch {
+    int64_t q0, nb;
+    dim3 grid;
+    int probesPerCta;
+    float* partD;
+    idx_t* partI;
+};
+
+// Splits nq queries into batches that bound the partial-result scratch, calls `launch` once per batch (the
+// scan kernel launch, bracketed by KernelTiming `timingName`) and merges each batch's partial results into
+// outD / outI [nq][k].  oneProbePerCta: one CTA per (query, probe); else the probes are split by ivfScanChunks.
+void runIvfScanBatches(
+        GpuResources* res,
+        int device,
+        int64_t nq,
+        int nprobe,
+        int k,
+        MetricType metric,
+        bool oneProbePerCta,
+        const char* timingName,
+        float* outD,
+        idx_t* outI,
+        cudaStream_t stream,
+        const std::function<void(const IvfScanBatch&)>& launch);
+
+// runtime value -> compile-time constant for the scan launchers' kernel templates:
+// f(std::true_type{}) or f(std::false_type{}) ...
+template <typename F>
+void withBool(bool b, F&& f) {
+    if (b)
+        f(std::true_type{});
+    else
+        f(std::false_type{});
+}
+// ... and f(std::integral_constant<int, V>{}) for the V of Vs equal to v (v must be one of them)
+template <int... Vs, typename F>
+void withInt(int v, F&& f) {
+    const bool found = ((v == Vs ? (f(std::integral_constant<int, Vs>{}), true) : false) || ...);
+    FB_THROW_IF_NOT(found);
+}
+// list ids of the scans' top-k lists: arena positions, 64-bit once they do not fit an int
+template <typename Wide>
+using ScanIdT = std::conditional_t<Wide::value, long long, int>;
 
 // ------------------------------------------------------------------------------------------
 // block-level helper: merge the per-warp lists of a block into warp 0's list, write k results

@@ -14,19 +14,15 @@
 #include <cfloat>
 #include <type_traits>
 
+#include "ivf_scan.cuh"
 #include "kernels.h"
 #include "select.cuh"
 
 namespace fb200 {
-
-void runMergeTopKKeyspace(
-        const float*, const idx_t*, int64_t, int, int, int, MetricType, int64_t, float*, idx_t*, cudaStream_t);
-int ivfScanChunks(int device, int64_t nq, int nprobe, int* probesPerCta);
-
 namespace {
 
 constexpr int kLutSlots = 64; // 256 B per code value
-constexpr int kScanWarps = 16;  // warps per scan CTA
+constexpr int kIlvScanWarps = 16;  // warps per scan CTA (ivf_scan.cuh's kScanWarps is the 4-warp scans')
 constexpr int kScanMinCtas = 2; // CTAs per SM the scan kernel's register budget is set for (64 registers)
 
 __device__ __forceinline__ int64_t interleaved_pos(int64_t v, int j, int M) {
@@ -96,7 +92,7 @@ __device__ __forceinline__ float lds_f32(unsigned addr) {
     return v;
 }
 
-// One CTA = one query x one chunk of its probes, kScanWarps warps.
+// One CTA = one query x one chunk of its probes, kIlvScanWarps warps.
 //
 //   * ONE top-k list per CTA (CtaTopK, select.cuh): every warp filters against the CTA-wide k-th key,
 //     survivors go to a small per-warp buffer, only the final half-merge runs under a CTA lock.  The list
@@ -116,7 +112,7 @@ __device__ __forceinline__ float lds_f32(unsigned addr) {
 // 16 x MQ direct entries are built first (into `dir`), then each of the 256 x M table entries is the sum of two
 // of them, T'[j][b] = T[2j][b & 15] + T[2j+1][b >> 4]; everything after the build is the 8-bit kernel's.
 template <int M, bool IS_L2, bool PRECOMP, typename IdT, int SBASE, bool NIB>
-__global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_interleaved_kernel(
+__global__ void __launch_bounds__(kIlvScanWarps * 32, kScanMinCtas) ivfpq_scan_interleaved_kernel(
         const float* __restrict__ Q,
         int d,
         const idx_t* __restrict__ probes,
@@ -136,9 +132,9 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
         idx_t* __restrict__ partI) {
     static_assert(!PRECOMP || IS_L2, "precomputed tables are an L2 decomposition");
     static_assert(!PRECOMP || !NIB, "no precomputed tables for 4-bit codes");
-    static_assert((kScanWarps & (kScanWarps - 1)) == 0, "kScanWarps must be a power of two");
+    static_assert((kIlvScanWarps & (kIlvScanWarps - 1)) == 0, "kIlvScanWarps must be a power of two");
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    constexpr int kThreads = kScanWarps * 32;
+    constexpr int kThreads = kIlvScanWarps * 32;
     constexpr int kU = M == 32 ? 4 : 8;      // groups of 32 vectors per work unit: 4 KB of codes in flight per warp
     constexpr int H = M / 16;                // 16-byte words per lane and group
     constexpr int kEntriesPerThread = 256 * M / kThreads;
@@ -157,7 +153,7 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
     idx_t* oI = partI + ((int64_t)q * gridDim.x + chunk) * k;
 
     CtaTopK<IdT> top;
-    top.init(listMem, ctl, LIST, k, kScanWarps);
+    top.init(listMem, ctl, LIST, k, kIlvScanWarps);
     const unsigned sbase = (unsigned)__cvta_generic_to_shared(lut);
     if (SBASE >= 0 && sbase != (unsigned)SBASE)
         __trap(); // compiled for another shared-window base: refuse to read the wrong addresses
@@ -321,7 +317,7 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
 
     const int pBegin = chunk * probesPerCta;
     const int pEnd = min(nprobe, pBegin + probesPerCta);
-    int base = 0; // work units dealt so far (identical in every warp): unit i belongs to warp i % kScanWarps
+    int base = 0; // work units dealt so far (identical in every warp): unit i belongs to warp i % kIlvScanWarps
     if (IS_L2) {
         for (int p0 = pBegin; p0 < pEnd; p0 += 2) {
             idx_t l[2];
@@ -412,7 +408,7 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
                 const int ngroups = (len[s] + 31) >> 5;
                 const int units = (ngroups + kU - 1) / kU;
                 const float add = PRECOMP ? t1s[s] : 0.f;
-                for (int u = (warp - base) & (kScanWarps - 1); u < units; u += kScanWarps)
+                for (int u = (warp - base) & (kIlvScanWarps - 1); u < units; u += kIlvScanWarps)
                     scanUnit(s, codes, ngroups, u * kU, len[s], ls[s], add);
                 base += units;
             }
@@ -430,7 +426,7 @@ __global__ void __launch_bounds__(kScanWarps * 32, kScanMinCtas) ivfpq_scan_inte
             const int ngroups = (len + 31) >> 5;
             const int units = (ngroups + kU - 1) / kU;
             const float add = -coarseDis[(int64_t)q * nprobe + p];
-            for (int u = (warp - base) & (kScanWarps - 1); u < units; u += kScanWarps)
+            for (int u = (warp - base) & (kIlvScanWarps - 1); u < units; u += kIlvScanWarps)
                 scanUnit(0, codes, ngroups, u * kU, len, ls, add);
             base += units;
         }
@@ -544,41 +540,6 @@ static int probedSmemBase(int device, cudaStream_t stream) {
     return (int)h;
 }
 
-template <int M, bool IS_L2, bool PRECOMP, typename IdT, bool NIB>
-static void launchScan(
-        int smemBase,
-        dim3 grid,
-        size_t smem,
-        cudaStream_t stream,
-        const float* Q,
-        int d,
-        const idx_t* probes,
-        const float* coarseDis,
-        int nprobe,
-        int probesPerCta,
-        const float* coarse,
-        const float* pqT,
-        const float* term2,
-        const int64_t* listStart,
-        const int* listLen,
-        const uint8_t* codes,
-        const idx_t* ids,
-        int k,
-        int LIST,
-        float* partD,
-        idx_t* partI) {
-    // any other shared-window base than the expected one: generic addressing
-    auto kern = smemBase == kExpectedSmemBase ? ivfpq_scan_interleaved_kernel<M, IS_L2, PRECOMP, IdT, kExpectedSmemBase, NIB>
-                                              : ivfpq_scan_interleaved_kernel<M, IS_L2, PRECOMP, IdT, -1, NIB>;
-    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    KernelTiming::begin("ivfpq_scan", stream);
-    kern<<<grid, kScanWarps * 32, smem, stream>>>(
-            Q, d, probes, coarseDis, nprobe, probesPerCta, coarse, pqT, term2, listStart, listLen, codes, ids, k, LIST,
-            partD, partI);
-    KernelTiming::end("ivfpq_scan", stream);
-    CUDA_CHECK_LAST();
-}
-
 void runIvfPqScanInterleaved(
         GpuResources* res,
         int device,
@@ -610,64 +571,37 @@ void runIvfPqScanInterleaved(
     const int LIST = std::max(CtaTopK<int>::BUF, next_pow2(k)); // a sorted buffer (<= BUF entries) is merged into the list
     const bool wide = arenaElems >= (int64_t(1) << 31) - 1; // arena positions need 64-bit list ids
     const int smemBase = probedSmemBase(device, stream);
-    const size_t listBytes = wide ? CtaTopK<long long>::bytes(LIST, kScanWarps) : CtaTopK<int>::bytes(LIST, kScanWarps);
+    const size_t listBytes = wide ? CtaTopK<long long>::bytes(LIST, kIlvScanWarps) : CtaTopK<int>::bytes(LIST, kIlvScanWarps);
     size_t smem = sizeof(float) * 256 * kLutSlots + round_up(sizeof(float) * 2 * d, 16) + 16 + listBytes +
             (nibble ? sizeof(float) * 2 * 16 * 2 * M : 0);
     FB_THROW_IF_NOT_MSG(smem <= 220 * 1024, "LUT + top-k lists do not fit shared memory");
     const bool l2 = metric == METRIC_L2;
-    int probesPerCta = 1;
-    const int chunks = ivfScanChunks(device, nq, nprobe, &probesPerCta);
-    const int64_t maxQ = std::max<int64_t>(1, std::min<int64_t>(65535, (int64_t(1) << 30) / ((int64_t)chunks * k * 12)));
-    for (int64_t q0 = 0; q0 < nq; q0 += maxQ) {
-        int64_t nb = std::min(maxQ, nq - q0);
-        auto partD = res->temp(device, sizeof(float) * nb * chunks * k);
-        auto partI = res->temp(device, sizeof(idx_t) * nb * chunks * k);
-        dim3 grid((unsigned)chunks, (unsigned)nb);
-#define SCAN(M_, L2_, PRE_, ID_, NIB_)                                                                             \
-    launchScan<M_, L2_, PRE_, ID_, NIB_>(                                                                              \
-            smemBase, grid, smem, stream, Q + q0 * d, d, probes + q0 * nprobe, coarseDis + q0 * nprobe, nprobe, probesPerCta, \
-            coarseCentroids, pqCentroidsT, term2, listStart, listLen, arenaCodes, arenaIds, k, LIST,               \
-            partD.as<float>(), partI.as<idx_t>())
-#define SCAN_ID(M_, L2_, PRE_, NIB_)          \
-    do {                                      \
-        if (wide)                             \
-            SCAN(M_, L2_, PRE_, long long, NIB_); \
-        else                                  \
-            SCAN(M_, L2_, PRE_, int, NIB_);   \
-    } while (0)
-        const bool pre = l2 && term2 != nullptr;
-        if (nibble) {
-            if (M == 32) {
-                if (l2)
-                    SCAN_ID(32, true, false, true);
-                else
-                    SCAN_ID(32, false, false, true);
-            } else {
-                if (l2)
-                    SCAN_ID(16, true, false, true);
-                else
-                    SCAN_ID(16, false, false, true);
-            }
-        } else if (M == 32) {
-            if (pre)
-                SCAN_ID(32, true, true, false);
-            else if (l2)
-                SCAN_ID(32, true, false, false);
-            else
-                SCAN_ID(32, false, false, false);
-        } else {
-            if (pre)
-                SCAN_ID(16, true, true, false);
-            else if (l2)
-                SCAN_ID(16, true, false, false);
-            else
-                SCAN_ID(16, false, false, false);
-        }
-#undef SCAN_ID
-#undef SCAN
-        runMergeTopKKeyspace(
-                partD.as<float>(), partI.as<idx_t>(), nb, chunks, k, k, metric, 0, outD + q0 * k, outI + q0 * k, stream);
-    }
+    const bool pre = l2 && term2 != nullptr;
+    runIvfScanBatches(res, device, nq, nprobe, k, metric, false, "ivfpq_scan", outD, outI, stream, [&](const IvfScanBatch& b) {
+        withInt<16, 32>(M, [&](auto m) {
+            withBool(nibble, [&](auto nib) {
+                withBool(l2, [&](auto isL2) {
+                    withBool(pre, [&](auto precomp) {
+                        withBool(wide, [&](auto wideIds) {
+                            // precomputed tables are an L2 decomposition of 8-bit codes (pre implies l2 and !nibble)
+                            if constexpr (!precomp || (isL2 && !nib)) {
+                                using IdT = ScanIdT<decltype(wideIds)>;
+                                // any other shared-window base than the expected one: generic addressing
+                                auto kern = smemBase == kExpectedSmemBase
+                                        ? ivfpq_scan_interleaved_kernel<m, isL2, precomp, IdT, kExpectedSmemBase, nib>
+                                        : ivfpq_scan_interleaved_kernel<m, isL2, precomp, IdT, -1, nib>;
+                                CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                                kern<<<b.grid, kIlvScanWarps * 32, smem, stream>>>(
+                                        Q + b.q0 * d, d, probes + b.q0 * nprobe, coarseDis + b.q0 * nprobe, nprobe,
+                                        b.probesPerCta, coarseCentroids, pqCentroidsT, term2, listStart, listLen,
+                                        arenaCodes, arenaIds, k, LIST, b.partD, b.partI);
+                            }
+                        });
+                    });
+                });
+            });
+        });
+    });
 }
 
 } // namespace fb200

@@ -410,41 +410,6 @@ size_t ivfSqScanTableBytes(int d) {
     return round_up(sizeof(float) * (2 * d + kScanWarps), 16);
 }
 
-template <int CODEC, bool IS_L2, typename IdT>
-static void launchIvfSqScan(dim3 grid, size_t smem, cudaStream_t stream, const float* Q, int d, const idx_t* probes,
-                            const float* coarseDis, int nprobe, int probesPerCta, const float* coarse, const float* mb,
-                            const int64_t* listStart, const int* listLen, const uint8_t* codes, const idx_t* ids,
-                            int codeSize, int fast, int k, int LIST, float* partD, idx_t* partI) {
-    auto kern = ivfsq_scan_kernel<CODEC, IS_L2, IdT>;
-    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, kScanWarps * 32, smem, stream>>>(
-            Q, d, probes, coarseDis, nprobe, probesPerCta, coarse, mb, listStart, listLen, codes, ids, codeSize, fast, k,
-            LIST, partD, partI);
-}
-
-template <int CODEC>
-static void dispatchIvfSqScan(bool l2, bool wide, dim3 grid, size_t smem, cudaStream_t stream, const float* Q, int d,
-                              const idx_t* probes, const float* coarseDis, int nprobe, int probesPerCta,
-                              const float* coarse, const float* mb, const int64_t* listStart, const int* listLen,
-                              const uint8_t* codes, const idx_t* ids, int codeSize, int fast, int k, int LIST,
-                              float* partD, idx_t* partI) {
-#define SQSCAN(L2_, ID_)                                                                                          \
-    launchIvfSqScan<CODEC, L2_, ID_>(grid, smem, stream, Q, d, probes, coarseDis, nprobe, probesPerCta, coarse, mb, \
-                                     listStart, listLen, codes, ids, codeSize, fast, k, LIST, partD, partI)
-    if (l2) {
-        if (wide)
-            SQSCAN(true, long long);
-        else
-            SQSCAN(true, int);
-    } else {
-        if (wide)
-            SQSCAN(false, long long);
-        else
-            SQSCAN(false, int);
-    }
-#undef SQSCAN
-}
-
 void runIvfSqScan(
         GpuResources* res,
         int device,
@@ -484,39 +449,20 @@ void runIvfSqScan(
     const bool l2 = metric == METRIC_L2;
     const float* coarse = (l2 && byResidual) ? coarseCentroids : nullptr;
     const float* cdis = (!l2 && byResidual) ? coarseDis : nullptr;
-    int probesPerCta = 1;
-    const int chunks = ivfScanChunks(device, nq, nprobe, &probesPerCta);
-    const int64_t maxQ = std::max<int64_t>(1, std::min<int64_t>(65535, (int64_t(1) << 30) / ((int64_t)chunks * k * 12)));
-    for (int64_t q0 = 0; q0 < nq; q0 += maxQ) {
-        const int64_t nb = std::min(maxQ, nq - q0);
-        auto partD = res->temp(device, sizeof(float) * nb * chunks * k);
-        auto partI = res->temp(device, sizeof(idx_t) * nb * chunks * k);
-        dim3 grid((unsigned)chunks, (unsigned)nb);
-        KernelTiming::begin("ivfsq_scan", stream);
-#define SQDISPATCH(C_)                                                                                             \
-    dispatchIvfSqScan<C_>(l2, wide, grid, smem, stream, Q + q0 * d, d, probes + q0 * nprobe, cdis ? cdis + q0 * nprobe : nullptr, \
-                          nprobe, probesPerCta, coarse, decodeMB, listStart, listLen, arenaCodes, arenaIds, codeSize,   \
-                          fast, k, LIST, partD.as<float>(), partI.as<idx_t>())
-        switch (codec) {
-            case SQC_BYTE:
-                SQDISPATCH(SQC_BYTE);
-                break;
-            case SQC_NIBBLE:
-                SQDISPATCH(SQC_NIBBLE);
-                break;
-            case SQC_SIX:
-                SQDISPATCH(SQC_SIX);
-                break;
-            default:
-                SQDISPATCH(SQC_HALF);
-                break;
-        }
-#undef SQDISPATCH
-        KernelTiming::end("ivfsq_scan", stream);
-        CUDA_CHECK_LAST();
-        runMergeTopKKeyspace(
-                partD.as<float>(), partI.as<idx_t>(), nb, chunks, k, k, metric, 0, outD + q0 * k, outI + q0 * k, stream);
-    }
+    runIvfScanBatches(res, device, nq, nprobe, k, metric, false, "ivfsq_scan", outD, outI, stream, [&](const IvfScanBatch& b) {
+        withInt<SQC_BYTE, SQC_NIBBLE, SQC_SIX, SQC_HALF>(codec, [&](auto c) {
+            withBool(l2, [&](auto isL2) {
+                withBool(wide, [&](auto wideIds) {
+                    auto kern = ivfsq_scan_kernel<c, isL2, ScanIdT<decltype(wideIds)>>;
+                    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                    kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
+                            Q + b.q0 * d, d, probes + b.q0 * nprobe, cdis ? cdis + b.q0 * nprobe : nullptr, nprobe,
+                            b.probesPerCta, coarse, decodeMB, listStart, listLen, arenaCodes, arenaIds, codeSize, fast,
+                            k, LIST, b.partD, b.partI);
+                });
+            });
+        });
+    });
 }
 
 } // namespace fb200

@@ -86,6 +86,21 @@ void runMergeTopKListMajor(
         idx_t* outI,
         cudaStream_t stream);
 
+// runMergeTopK over inputs already in key space (smaller is better: IP distances negated), without id offsets;
+// idBase is added to every id.  Merges the per-CTA partial results of the Flat and IVF scans.
+void runMergeTopKKeyspace(
+        const float* inD,
+        const idx_t* inI,
+        int64_t rows,
+        int nlists,
+        int kin,
+        int k,
+        MetricType metric,
+        int64_t idBase,
+        float* outD,
+        idx_t* outI,
+        cudaStream_t stream);
+
 // residual x - c[assign] (NaN if assign = -1) ; role of runCalcResidual (VectorResidual.cu:26-176)
 void runCalcResidual(
         const float* x,
