@@ -2,6 +2,7 @@
 #include "faiss_b200_adapter.h"
 
 #include <faiss/impl/FaissAssert.h>
+#include <faiss/impl/IDSelector.h>
 #include <faiss/invlists/InvertedLists.h>
 
 #include <cstring>
@@ -21,6 +22,49 @@ void ck(int rc) {
     FAISS_THROW_IF_NOT_MSG(m == faiss::METRIC_L2 || m == faiss::METRIC_INNER_PRODUCT, "faiss_b200 supports METRIC_L2 and METRIC_INNER_PRODUCT");
     return m == faiss::METRIC_L2 ? ::METRIC_L2 : ::METRIC_INNER_PRODUCT;
 }
+int selectorIsMember(void* ctx, ::idx_t id) {
+    return static_cast<const faiss::IDSelector*>(ctx)->is_member(id) ? 1 : 0;
+}
+
+// a faiss::IDSelector as the library's selector tree: the reference's Range / Array / Batch / Bitmap / Not / And /
+// Or / XOr by their contents (their is_member is final, so a subclass cannot change it), any other subclass
+// (IDSelectorAll, IDSelectorTranslated, a user class) as a callback
+struct SelectorHandles {
+    std::vector<FaissIDSelector*> owned;
+    ~SelectorHandles() {
+        for (auto* h : owned)
+            faiss_IDSelector_free(h);
+    }
+    FaissIDSelector* convert(const faiss::IDSelector* s) {
+        FaissIDSelector* h = nullptr;
+        if (auto* r = dynamic_cast<const faiss::IDSelectorRange*>(s)) {
+            ck(faiss_IDSelectorRange_new(&h, r->imin, r->imax));
+        } else if (auto* a = dynamic_cast<const faiss::IDSelectorArray*>(s)) {
+            ck(faiss_IDSelectorArray_new(&h, a->n, a->ids));
+        } else if (auto* b = dynamic_cast<const faiss::IDSelectorBatch*>(s)) {
+            std::vector<::idx_t> ids(b->set.begin(), b->set.end());
+            ck(faiss_IDSelectorBatch_new(&h, ids.size(), ids.data()));
+        } else if (auto* bm = dynamic_cast<const faiss::IDSelectorBitmap*>(s)) {
+            ck(faiss_IDSelectorBitmap_new(&h, bm->n, bm->bitmap));
+        } else if (auto* n = dynamic_cast<const faiss::IDSelectorNot*>(s)) {
+            FaissIDSelector* c = convert(n->sel);
+            ck(faiss_IDSelectorNot_new(&h, c));
+        } else if (auto* x = dynamic_cast<const faiss::IDSelectorAnd*>(s)) {
+            FaissIDSelector* l = convert(x->lhs);
+            ck(faiss_IDSelectorAnd_new(&h, l, convert(x->rhs)));
+        } else if (auto* x = dynamic_cast<const faiss::IDSelectorOr*>(s)) {
+            FaissIDSelector* l = convert(x->lhs);
+            ck(faiss_IDSelectorOr_new(&h, l, convert(x->rhs)));
+        } else if (auto* x = dynamic_cast<const faiss::IDSelectorXOr*>(s)) {
+            FaissIDSelector* l = convert(x->lhs);
+            ck(faiss_IDSelectorXOr_new(&h, l, convert(x->rhs)));
+        } else {
+            ck(faiss_b200_IDSelectorCallback_new(&h, selectorIsMember, const_cast<faiss::IDSelector*>(s)));
+        }
+        owned.push_back(h);
+        return h;
+    }
+};
 } // namespace
 
 B200Resources::B200Resources() {
@@ -57,8 +101,16 @@ void B200Index::add_with_ids(faiss::idx_t n, const float* x, const faiss::idx_t*
 }
 void B200Index::search(
         faiss::idx_t n, const float* x, faiss::idx_t k, float* distances, faiss::idx_t* labels, const faiss::SearchParameters* params) const {
-    FAISS_THROW_IF_NOT_MSG(!params || !params->sel, "faiss_b200: IDSelector is not supported");
-    ck(faiss_Index_search(h_, n, x, k, distances, labels));
+    if (!params || !params->sel) {
+        ck(faiss_Index_search(h_, n, x, k, distances, labels));
+        return;
+    }
+    SelectorHandles sel;
+    FaissSearchParameters* sp = nullptr;
+    ck(faiss_SearchParameters_new(&sp, sel.convert(params->sel)));
+    int rc = faiss_Index_search_with_params(h_, n, x, k, sp, distances, labels);
+    faiss_SearchParameters_free(sp);
+    ck(rc);
 }
 void B200Index::reset() {
     ck(faiss_Index_reset(h_));
@@ -103,15 +155,18 @@ void B200IndexIVF::search(
         faiss::idx_t n, const float* x, faiss::idx_t k, float* distances, faiss::idx_t* labels, const faiss::SearchParameters* params) const {
     size_t use_nprobe = nprobe;
     size_t max_codes = 0;
+    SelectorHandles sel;
+    FaissIDSelector* selHandle = nullptr;
     if (params) {
-        FAISS_THROW_IF_NOT_MSG(!params->sel, "faiss_b200: IDSelector is not supported");
+        if (params->sel)
+            selHandle = sel.convert(params->sel);
         auto* ivf = dynamic_cast<const faiss::SearchParametersIVF*>(params);
         FAISS_THROW_IF_NOT_MSG(ivf, "IVF search: search parameters must be SearchParametersIVF");
         use_nprobe = ivf->nprobe;
         max_codes = ivf->max_codes;
     }
     FaissSearchParametersIVF* sp = nullptr;
-    ck(faiss_SearchParametersIVF_new_with(&sp, use_nprobe, max_codes));
+    ck(faiss_SearchParametersIVF_new_with_sel(&sp, selHandle, use_nprobe, max_codes));
     int rc = faiss_Index_search_with_params(h_, n, x, k, sp, distances, labels);
     faiss_SearchParameters_free(sp);
     ck(rc);

@@ -708,11 +708,84 @@ struct FaissSearchParameters_H {
     SearchParameters* p;
 };
 int faiss_SearchParametersIVF_new_with(FaissSearchParametersIVF** out, size_t nprobe, size_t max_codes) {
+    return faiss_SearchParametersIVF_new_with_sel(out, nullptr, nprobe, max_codes);
+}
+
+// ---------------------------------------------------------------- IDSelector
+} // extern "C"
+struct FaissIDSelector_H {
+    IDSelector* sel;
+};
+static const IDSelector* SEL(const FaissIDSelector* p) {
+    if (!p || !p->sel)
+        FB_THROW_MSG("null IDSelector handle");
+    return p->sel;
+}
+template <typename F>
+static int newSelector(FaissIDSelector** out, F make) {
     try {
-        auto* sp = new SearchParametersIVF();
+        FB_THROW_IF_NOT_MSG(out != nullptr, "null output pointer");
+        std::unique_ptr<IDSelector> s(make());
+        *out = new FaissIDSelector_H{s.release()};
+    }
+    CATCH_AND_HANDLE
+}
+extern "C" {
+void faiss_IDSelector_free(FaissIDSelector* p) {
+    if (p) {
+        delete p->sel;
+        delete p;
+    }
+}
+int faiss_IDSelector_is_member(const FaissIDSelector* p, idx_t id) {
+    if (!p || !p->sel)
+        return -1;
+    return p->sel->is_member(id) ? 1 : 0;
+}
+int faiss_IDSelectorRange_new(FaissIDSelectorRange** out, idx_t imin, idx_t imax) {
+    return newSelector(out, [&] { return IDSelector::range(imin, imax); });
+}
+int faiss_IDSelectorArray_new(FaissIDSelectorArray** out, size_t n, const idx_t* ids) {
+    return newSelector(out, [&] { return IDSelector::array(n, ids); });
+}
+int faiss_IDSelectorBatch_new(FaissIDSelectorBatch** out, size_t n, const idx_t* indices) {
+    return newSelector(out, [&] { return IDSelector::batch(n, indices); });
+}
+int faiss_IDSelectorBitmap_new(FaissIDSelectorBitmap** out, size_t n, const uint8_t* bitmap) {
+    return newSelector(out, [&] { return IDSelector::bitmapOf(n, bitmap); });
+}
+int faiss_IDSelectorNot_new(FaissIDSelectorNot** out, const FaissIDSelector* sel) {
+    return newSelector(out, [&] { return IDSelector::negation(SEL(sel)); });
+}
+int faiss_IDSelectorAnd_new(FaissIDSelectorAnd** out, const FaissIDSelector* lhs, const FaissIDSelector* rhs) {
+    return newSelector(out, [&] { return IDSelector::binary(IDSelector::AND, SEL(lhs), SEL(rhs)); });
+}
+int faiss_IDSelectorOr_new(FaissIDSelectorOr** out, const FaissIDSelector* lhs, const FaissIDSelector* rhs) {
+    return newSelector(out, [&] { return IDSelector::binary(IDSelector::OR, SEL(lhs), SEL(rhs)); });
+}
+int faiss_IDSelectorXOr_new(FaissIDSelectorXOr** out, const FaissIDSelector* lhs, const FaissIDSelector* rhs) {
+    return newSelector(out, [&] { return IDSelector::binary(IDSelector::XOR, SEL(lhs), SEL(rhs)); });
+}
+int faiss_b200_IDSelectorCallback_new(FaissIDSelector** out, int (*is_member)(void* ctx, idx_t id), void* ctx) {
+    return newSelector(out, [&] { return IDSelector::callback(is_member, ctx); });
+}
+int faiss_SearchParameters_new(FaissSearchParameters** out, FaissIDSelector* sel) {
+    try {
+        FB_THROW_IF_NOT_MSG(out != nullptr, "null output pointer");
+        auto sp = std::make_unique<SearchParameters>();
+        sp->sel = sel ? SEL(sel) : nullptr;
+        *out = new FaissSearchParameters_H{sp.release()};
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_SearchParametersIVF_new_with_sel(FaissSearchParametersIVF** out, FaissIDSelector* sel, size_t nprobe, size_t max_codes) {
+    try {
+        FB_THROW_IF_NOT_MSG(out != nullptr, "null output pointer");
+        auto sp = std::make_unique<SearchParametersIVF>();
+        sp->sel = sel ? SEL(sel) : nullptr;
         sp->nprobe = nprobe;
         sp->max_codes = max_codes;
-        *out = new FaissSearchParameters_H{sp};
+        *out = new FaissSearchParameters_H{sp.release()};
     }
     CATCH_AND_HANDLE
 }

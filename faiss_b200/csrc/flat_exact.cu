@@ -193,7 +193,8 @@ struct OpGower {
     __device__ static float finish(const Acc& a, float) { return a.a / a.b; }
 };
 
-template <int TQ, int TN, class Op, bool K1>
+// MASK: only rows whose bit is set in rowMask (bit r & 31 of word r >> 5) enter the results (SearchParameters::sel)
+template <int TQ, int TN, class Op, bool K1, bool MASK>
 __global__ void __launch_bounds__(256) flat_exact_kernel(
         const float* __restrict__ Q,
         int nq,
@@ -206,7 +207,8 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
         int64_t rowsPerSplit,
         float arg,                  // metric_arg (the exponent of METRIC_Lp)
         float* __restrict__ partD,  // [nq, nsplit, k]   keys ("smaller is better")
-        idx_t* __restrict__ partI)  // [nq, nsplit, k]   row index (or -1)
+        idx_t* __restrict__ partI,  // [nq, nsplit, k]   row index (or -1)
+        const uint32_t* __restrict__ rowMask)
 {
     using C = ExactCfg<TQ, TN>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -360,7 +362,7 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
 #pragma unroll
                 for (int c = 0; c < 4; c++) {
                     int64_t row = nb + tx * 4 + c;
-                    if (row < r1) {
+                    if (row < r1 && (!MASK || ((rowMask[row >> 5] >> (row & 31)) & 1u))) {
                         const float dist = Op::finish(acc[r][c], arg);
                         float key = Op::kSimilarity ? -dist : dist;
                         if (key == key && (!Op::kSentinel || key < FLT_MAX)) { // NaN never wins
@@ -380,7 +382,8 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
                     int64_t row = nb + tx * 4 + c;
                     const float dist = Op::finish(acc[r][c], arg);
                     float key = Op::kSimilarity ? -dist : dist;
-                    if (row < r1 && key <= thr && (!Op::kSentinel || key < FLT_MAX)) {
+                    if (row < r1 && key <= thr && (!Op::kSentinel || key < FLT_MAX) &&
+                        (!MASK || ((rowMask[row >> 5] >> (row & 31)) & 1u))) {
                         int pos = atomicAdd(&cntS[q], 1);
                         s.keys[LIST + pos] = key;
                         s.ids[LIST + pos] = (int)(row - r0);
@@ -482,7 +485,7 @@ __global__ void merge_topk_kernel(
             const int64_t at = l * listStride + (e - l * kin);
             id = I[at];
             key = D[at];
-            if (id < 0) {
+            if (id == -1) { // the "no result" marker; any other id is a stored one (IVF ids may be negative)
                 valid = false;
             } else {
                 if (idOffsets)
@@ -603,6 +606,7 @@ static void launchExact(
         int64_t rowsPerSplit,
         float* partD,
         idx_t* partI,
+        const uint32_t* rowMask,
         cudaStream_t stream) {
     using C = ExactCfg<TQ, TN>;
     size_t smem = sizeof(float) * kDK * (C::QS + C::YS) + TQ * (sizeof(int) + sizeof(float) + sizeof(unsigned long long));
@@ -611,39 +615,46 @@ static void launchExact(
     dim3 grid((unsigned)ceil_div(nq, TQ), (unsigned)nsplit);
     auto launch = [&](auto kern) {
         CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, C::kThreads, smem, stream>>>(Q, (int)nq, Y, yHalf, n, d, k, LIST, rowsPerSplit, metricArg, partD, partI);
+        kern<<<grid, C::kThreads, smem, stream>>>(Q, (int)nq, Y, yHalf, n, d, k, LIST, rowsPerSplit, metricArg, partD, partI, rowMask);
+    };
+    auto launchOp = [&](auto op) {
+        using Op = decltype(op);
+        if (rowMask)
+            launch(flat_exact_kernel<TQ, TN, Op, K1, true>);
+        else
+            launch(flat_exact_kernel<TQ, TN, Op, K1, false>);
     };
     // METRIC_Lp arrives here with p != 1, 2: GpuIndexFlat::searchMetric_ sends those to L1 / L2
     switch (metric) {
         case METRIC_L2:
-            launch(flat_exact_kernel<TQ, TN, OpL2, K1>);
+            launchOp(OpL2{});
             break;
         case METRIC_INNER_PRODUCT:
-            launch(flat_exact_kernel<TQ, TN, OpIP, K1>);
+            launchOp(OpIP{});
             break;
         case METRIC_L1:
-            launch(flat_exact_kernel<TQ, TN, OpL1, K1>);
+            launchOp(OpL1{});
             break;
         case METRIC_Linf:
-            launch(flat_exact_kernel<TQ, TN, OpLinf, K1>);
+            launchOp(OpLinf{});
             break;
         case METRIC_Lp:
-            launch(flat_exact_kernel<TQ, TN, OpLp, K1>);
+            launchOp(OpLp{});
             break;
         case METRIC_Canberra:
-            launch(flat_exact_kernel<TQ, TN, OpCanberra, K1>);
+            launchOp(OpCanberra{});
             break;
         case METRIC_BrayCurtis:
-            launch(flat_exact_kernel<TQ, TN, OpBrayCurtis, K1>);
+            launchOp(OpBrayCurtis{});
             break;
         case METRIC_JensenShannon:
-            launch(flat_exact_kernel<TQ, TN, OpJensenShannon, K1>);
+            launchOp(OpJensenShannon{});
             break;
         case METRIC_Jaccard:
-            launch(flat_exact_kernel<TQ, TN, OpJaccard, K1>);
+            launchOp(OpJaccard{});
             break;
         case METRIC_GOWER:
-            launch(flat_exact_kernel<TQ, TN, OpGower, K1>);
+            launchOp(OpGower{});
             break;
         default:
             FB_THROW_FMT("unimplemented metric type %d", (int)metric); // faiss/gpu/impl/Distance.cuh:289
@@ -666,6 +677,7 @@ static void flatExactImpl(
         int64_t idBase,
         float* outD,
         idx_t* outI,
+        const uint32_t* rowMask,
         cudaStream_t stream) {
     if (!is_implemented_metric(metric))
         FB_THROW_FMT("unimplemented metric type %d", (int)metric);
@@ -711,7 +723,7 @@ static void flatExactImpl(
 
 #define LAUNCH(TQ_, TN_, K1_)                                                                        \
     launchExact<TQ_, TN_, K1_>(                                                                      \
-            Q, nq, Y, yHalf, n, d, k, LIST, metric, metricArg, (int)nsplit, rowsPerSplit, partD.as<float>(), partI.as<idx_t>(), stream)
+            Q, nq, Y, yHalf, n, d, k, LIST, metric, metricArg, (int)nsplit, rowsPerSplit, partD.as<float>(), partI.as<idx_t>(), rowMask, stream)
     if (K1) {
         LAUNCH(32, 64, true);
     } else if (TQ == 32) {
@@ -741,8 +753,9 @@ void runFlatExact(
         idx_t* outI,
         cudaStream_t stream,
         int yHalf,
-        float metricArg) {
-    flatExactImpl(res, device, Q, nq, Y, yHalf, n, d, k, metric, metricArg, idBase, outD, outI, stream);
+        float metricArg,
+        const uint32_t* rowMask) {
+    flatExactImpl(res, device, Q, nq, Y, yHalf, n, d, k, metric, metricArg, idBase, outD, outI, rowMask, stream);
 }
 
 void runFlatArgmin(
@@ -764,7 +777,7 @@ void runFlatArgmin(
         tmp = res->temp(device, sizeof(float) * nq);
         outD = tmp.as<float>();
     }
-    flatExactImpl(res, device, Q, nq, Y, 0, n, d, 1, metric, 0.f, 0, outD, outI, stream);
+    flatExactImpl(res, device, Q, nq, Y, 0, n, d, 1, metric, 0.f, 0, outD, outI, nullptr, stream);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -896,6 +896,11 @@ void runFlatTcPrepareRows(
     }
     tc_prepare_rows_kernel<<<rowBlocks, warps * 32, 0, stream>>>(Y, yHalf, n, d, dpad, scale, isL2, perm, Y16, bias, nullptr);
     CUDA_CHECK_LAST();
+    runFlatTcTileBias(bias, n, tileMaxBias, stream);
+}
+
+void runFlatTcTileBias(const float* bias, int64_t n, float* tileMaxBias, cudaStream_t stream) {
+    const int warps = 8;
     const int64_t numTiles = ceil_div(n, kTileN);
     tc_tile_max_bias_kernel<<<(unsigned)ceil_div(numTiles, warps), warps * 32, 0, stream>>>(bias, numTiles, tileMaxBias);
     CUDA_CHECK_LAST();
@@ -987,7 +992,8 @@ void runFlatTcSearch(
         idx_t* outI,
         cudaStream_t stream,
         const FlatTcShard* shard,
-        int yHalf) {
+        int yHalf,
+        const uint32_t* rowMask) {
     if (nqAll == 0)
         return;
     FB_THROW_IF_NOT(flatTcSupported(d, k, n));
@@ -1264,7 +1270,9 @@ void runFlatTcSearch(
                 auto fI = res->temp(device, sizeof(idx_t) * (size_t)nflag * k);
                 tc_gather_queries_kernel<<<nflag, 128, 0, stream>>>(Qb, list.as<int>(), d, fq.as<float>());
                 CUDA_CHECK_LAST();
-                runFlatExact(res, device, fq.as<float>(), nflag, Y, n, d, k, metric, 0, fD.as<float>(), fI.as<idx_t>(), stream, yHalf);
+                runFlatExact(
+                        res, device, fq.as<float>(), nflag, Y, n, d, k, metric, 0, fD.as<float>(), fI.as<idx_t>(), stream,
+                        yHalf, 0.f, rowMask);
                 tc_scatter_results_kernel<<<nflag, 128, 0, stream>>>(
                         fD.as<float>(), fI.as<idx_t>(), list.as<int>(), k, outD + qb * k, outI + qb * k);
                 CUDA_CHECK_LAST();

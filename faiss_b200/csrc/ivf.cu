@@ -310,7 +310,7 @@ void runIvfScatter(
 // across the probes of the chunk (list ids = arena positions), so threshold passes grow with
 // log(vectors per CTA) instead of with the number of (query, probe) pairs.
 // ------------------------------------------------------------------------------------------
-template <bool IS_L2, typename IdT>
+template <bool IS_L2, typename IdT, bool MASKED>
 __global__ void __launch_bounds__(kScanWarps * 32) ivfflat_scan_kernel(
         const float* __restrict__ Q,
         int d,
@@ -324,7 +324,8 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfflat_scan_kernel(
         int k,
         int LIST,
         float* __restrict__ partD, // [nq, chunks, k] keys
-        idx_t* __restrict__ partI) {
+        idx_t* __restrict__ partI,
+        const uint32_t* __restrict__ slotMask) { // MASKED: the selector's arena mask
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int q = blockIdx.y, chunk = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = lane_id();
@@ -403,7 +404,8 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfflat_scan_kernel(
                         vals[j] = keep + __shfl_xor_sync(kFullMask, send, s);
                     }
                 }
-                w.add(v0 + lane < len, IS_L2 ? vals[0] : -vals[0], (IdT)(ls + v0 + lane));
+                w.add(v0 + lane < len && slotSelected<MASKED>(slotMask, ls + v0), IS_L2 ? vals[0] : -vals[0],
+                      (IdT)(ls + v0 + lane));
             }
         }
         block_merge_and_write<IdT>(w, warp, lists, perWarp, LIST, k, arenaIds, 0.f, oD, oI);
@@ -438,7 +440,7 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfflat_scan_kernel(
                 if (lane == v)
                     mineKey = IS_L2 ? acc : -acc;
             }
-            w.add(lane < cntv, mineKey, (IdT)(ls + v0 + lane));
+            w.add(lane < cntv && slotSelected<MASKED>(slotMask, ls + v0), mineKey, (IdT)(ls + v0 + lane));
         }
     }
     block_merge_and_write<IdT>(w, warp, lists, perWarp, LIST, k, arenaIds, 0.f, oD, oI);
@@ -508,7 +510,8 @@ void runIvfFlatScan(
         MetricType metric,
         float* outD,
         idx_t* outI,
-        cudaStream_t stream) {
+        cudaStream_t stream,
+        const uint32_t* slotMask) {
     if (nq == 0)
         return;
     const int LIST = std::max(64, next_pow2(k));
@@ -519,11 +522,13 @@ void runIvfFlatScan(
     runIvfScanBatches(res, device, nq, nprobe, k, metric, false, "ivfflat_scan", outD, outI, stream, [&](const IvfScanBatch& b) {
         withBool(metric == METRIC_L2, [&](auto l2) {
             withBool(wide, [&](auto wideIds) {
-                auto kern = ivfflat_scan_kernel<l2, ScanIdT<decltype(wideIds)>>;
-                CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
-                        Q + b.q0 * d, d, probes + b.q0 * nprobe, nprobe, b.probesPerCta, listStart, listLen, arenaVecs,
-                        arenaIds, k, LIST, b.partD, b.partI);
+                withBool(slotMask != nullptr, [&](auto masked) {
+                    auto kern = ivfflat_scan_kernel<l2, ScanIdT<decltype(wideIds)>, masked>;
+                    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                    kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
+                            Q + b.q0 * d, d, probes + b.q0 * nprobe, nprobe, b.probesPerCta, listStart, listLen,
+                            arenaVecs, arenaIds, k, LIST, b.partD, b.partI, slotMask);
+                });
             });
         });
     });
@@ -533,7 +538,7 @@ void runIvfFlatScan(
 // IVF-PQ scan: block per (query, probe).  PACKED: codes of ksub = 2^nbits < 256 centroids, stored as the CPU's
 // LSB-first bitstring of ceil(M * nbits / 8) bytes per vector; each lane decodes its vector from a 64-bit window.
 // ------------------------------------------------------------------------------------------
-template <bool IS_L2, bool PACKED>
+template <bool IS_L2, bool PACKED, bool MASKED>
 __global__ void __launch_bounds__(kScanWarps * 32) ivfpq_scan_kernel(
         const float* __restrict__ Q,
         int d,
@@ -551,7 +556,8 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfpq_scan_kernel(
         int k,
         int LIST,
         float* __restrict__ partD,
-        idx_t* __restrict__ partI) {
+        idx_t* __restrict__ partI,
+        const uint32_t* __restrict__ slotMask) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int q = blockIdx.y, p = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = lane_id();
@@ -646,7 +652,7 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfpq_scan_kernel(
                     acc += lut[m * ksub + cp[m]];
             }
         }
-        w.add(valid, acc, v0);
+        w.add(valid && slotSelected<MASKED>(slotMask, listStart[l] + (v0 & ~31)), acc, v0);
     }
     // IP: total = q.c_list + sum_m q_m.pq  -> key = -(coarse + sum) ; L2: residual form, no add
     const float add = IS_L2 ? 0.f : -coarseDis[(int64_t)q * nprobe + p];
@@ -674,7 +680,8 @@ void runIvfPqScan(
         MetricType metric,
         float* outD,
         idx_t* outI,
-        cudaStream_t stream) {
+        cudaStream_t stream,
+        const uint32_t* slotMask) {
     if (nq == 0)
         return;
     FB_THROW_IF_NOT(nbits >= 1 && nbits <= 8);
@@ -688,11 +695,14 @@ void runIvfPqScan(
     runIvfScanBatches(res, device, nq, nprobe, k, metric, true, name, outD, outI, stream, [&](const IvfScanBatch& b) {
         withBool(metric == METRIC_L2, [&](auto l2) {
             withBool(packed, [&](auto pk) {
-                auto kern = ivfpq_scan_kernel<l2, pk>;
-                CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
-                        Q + b.q0 * d, d, probes + b.q0 * nprobe, coarseDis + b.q0 * nprobe, nprobe, coarseCentroids,
-                        pqCentroids, M, ksub, listStart, listLen, arenaCodes, arenaIds, k, LIST, b.partD, b.partI);
+                withBool(slotMask != nullptr, [&](auto masked) {
+                    auto kern = ivfpq_scan_kernel<l2, pk, masked>;
+                    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                    kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
+                            Q + b.q0 * d, d, probes + b.q0 * nprobe, coarseDis + b.q0 * nprobe, nprobe, coarseCentroids,
+                            pqCentroids, M, ksub, listStart, listLen, arenaCodes, arenaIds, k, LIST, b.partD, b.partI,
+                            slotMask);
+                });
             });
         });
     });

@@ -58,6 +58,16 @@ void withInt(int v, F&& f) {
     const bool found = ((v == Vs ? (f(std::integral_constant<int, Vs>{}), true) : false) || ...);
     FB_THROW_IF_NOT(found);
 }
+// SearchParameters::sel over the arena (idselector.h): is this lane's slot of the group of 32 slots that starts
+// at arena position slot0 selected?  Lists start 32-aligned, so a group is one mask word: one broadcast load per
+// warp.  MASKED = false (no selector) compiles to nothing.
+template <bool MASKED>
+__device__ __forceinline__ bool slotSelected(const uint32_t* __restrict__ mask, int64_t slot0) {
+    if (!MASKED)
+        return true;
+    return (__ldg(mask + (slot0 >> 5)) >> lane_id()) & 1u;
+}
+
 // list ids of the scans' top-k lists: arena positions, 64-bit once they do not fit an int
 template <typename Wide>
 using ScanIdT = std::conditional_t<Wide::value, long long, int>;

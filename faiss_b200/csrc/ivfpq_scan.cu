@@ -111,7 +111,7 @@ __device__ __forceinline__ float lds_f32(unsigned addr) {
 // NIB (table-build policy): 4-bit PQ with MQ = 2M sub-quantisers whose nibble pairs are the M code bytes.  The
 // 16 x MQ direct entries are built first (into `dir`), then each of the 256 x M table entries is the sum of two
 // of them, T'[j][b] = T[2j][b & 15] + T[2j+1][b >> 4]; everything after the build is the 8-bit kernel's.
-template <int M, bool IS_L2, bool PRECOMP, typename IdT, int SBASE, bool NIB>
+template <int M, bool IS_L2, bool PRECOMP, typename IdT, int SBASE, bool NIB, bool MASKED>
 __global__ void __launch_bounds__(kIlvScanWarps * 32, kScanMinCtas) ivfpq_scan_interleaved_kernel(
         const float* __restrict__ Q,
         int d,
@@ -129,7 +129,8 @@ __global__ void __launch_bounds__(kIlvScanWarps * 32, kScanMinCtas) ivfpq_scan_i
         int k,
         int LIST,
         float* __restrict__ partD,
-        idx_t* __restrict__ partI) {
+        idx_t* __restrict__ partI,
+        const uint32_t* __restrict__ slotMask) { // MASKED: the selector's arena mask
     static_assert(!PRECOMP || IS_L2, "precomputed tables are an L2 decomposition");
     static_assert(!PRECOMP || !NIB, "no precomputed tables for 4-bit codes");
     static_assert((kIlvScanWarps & (kIlvScanWarps - 1)) == 0, "kIlvScanWarps must be a power of two");
@@ -286,7 +287,8 @@ __global__ void __launch_bounds__(kIlvScanWarps * 32, kScanMinCtas) ivfpq_scan_i
             const float sum = groupSum(cur[u], Pbase);
             const int v = (g0 + u) * 32 + lane;
             const float key = (IS_L2 && !PRECOMP) ? sum : sum + add;
-            top.add(g0 + u < ngroups && v < len, key, (IdT)(ls + v));
+            top.add(g0 + u < ngroups && v < len && slotSelected<MASKED>(slotMask, ls + (int64_t)(g0 + u) * 32), key,
+                    (IdT)(ls + v));
         }
     };
 
@@ -563,7 +565,8 @@ void runIvfPqScanInterleaved(
         MetricType metric,
         float* outD,
         idx_t* outI,
-        cudaStream_t stream) {
+        cudaStream_t stream,
+        const uint32_t* slotMask) {
     if (nq == 0)
         return;
     FB_THROW_IF_NOT(ivfPqInterleavedSupported(M));
@@ -583,19 +586,21 @@ void runIvfPqScanInterleaved(
                 withBool(l2, [&](auto isL2) {
                     withBool(pre, [&](auto precomp) {
                         withBool(wide, [&](auto wideIds) {
-                            // precomputed tables are an L2 decomposition of 8-bit codes (pre implies l2 and !nibble)
-                            if constexpr (!precomp || (isL2 && !nib)) {
-                                using IdT = ScanIdT<decltype(wideIds)>;
-                                // any other shared-window base than the expected one: generic addressing
-                                auto kern = smemBase == kExpectedSmemBase
-                                        ? ivfpq_scan_interleaved_kernel<m, isL2, precomp, IdT, kExpectedSmemBase, nib>
-                                        : ivfpq_scan_interleaved_kernel<m, isL2, precomp, IdT, -1, nib>;
-                                CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                                kern<<<b.grid, kIlvScanWarps * 32, smem, stream>>>(
-                                        Q + b.q0 * d, d, probes + b.q0 * nprobe, coarseDis + b.q0 * nprobe, nprobe,
-                                        b.probesPerCta, coarseCentroids, pqCentroidsT, term2, listStart, listLen,
-                                        arenaCodes, arenaIds, k, LIST, b.partD, b.partI);
-                            }
+                            withBool(slotMask != nullptr, [&](auto masked) {
+                                // precomputed tables are an L2 decomposition of 8-bit codes (pre implies l2 and !nibble)
+                                if constexpr (!precomp || (isL2 && !nib)) {
+                                    using IdT = ScanIdT<decltype(wideIds)>;
+                                    // any other shared-window base than the expected one: generic addressing
+                                    auto kern = smemBase == kExpectedSmemBase
+                                            ? ivfpq_scan_interleaved_kernel<m, isL2, precomp, IdT, kExpectedSmemBase, nib, masked>
+                                            : ivfpq_scan_interleaved_kernel<m, isL2, precomp, IdT, -1, nib, masked>;
+                                    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                                    kern<<<b.grid, kIlvScanWarps * 32, smem, stream>>>(
+                                            Q + b.q0 * d, d, probes + b.q0 * nprobe, coarseDis + b.q0 * nprobe, nprobe,
+                                            b.probesPerCta, coarseCentroids, pqCentroidsT, term2, listStart, listLen,
+                                            arenaCodes, arenaIds, k, LIST, b.partD, b.partI, slotMask);
+                                }
+                            });
                         });
                     });
                 });

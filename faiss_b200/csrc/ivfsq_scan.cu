@@ -227,7 +227,7 @@ __device__ __forceinline__ float sq_row_comp(const uint8_t* __restrict__ cp, int
     }
 }
 
-template <int CODEC, bool IS_L2, typename IdT>
+template <int CODEC, bool IS_L2, typename IdT, bool MASKED>
 __global__ void __launch_bounds__(kScanWarps * 32) ivfsq_scan_kernel(
         const float* __restrict__ Q,
         int d,
@@ -246,7 +246,8 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfsq_scan_kernel(
         int k,
         int LIST,
         float* __restrict__ partD, // [nq, chunks, k] keys
-        idx_t* __restrict__ partI) {
+        idx_t* __restrict__ partI,
+        const uint32_t* __restrict__ slotMask) { // MASKED: the selector's arena mask
     using F = SqFast<CODEC>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int q = blockIdx.y, chunk = blockIdx.x;
@@ -367,7 +368,8 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfsq_scan_kernel(
                         vals[j] = keep + __shfl_xor_sync(kFullMask, send, s);
                     }
                 }
-                w.add(v0 + lane < len, IS_L2 ? vals[0] : -(vals[0] + Kp), (IdT)(ls + v0 + lane));
+                w.add(v0 + lane < len && slotSelected<MASKED>(slotMask, ls + v0), IS_L2 ? vals[0] : -(vals[0] + Kp),
+                      (IdT)(ls + v0 + lane));
             }
         } else {
             // generic path: lane = vector, components in order; the table reads are shared-memory broadcasts
@@ -385,7 +387,7 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfsq_scan_kernel(
                         acc = fmaf(ta[i], cv, acc);
                     }
                 }
-                w.add(valid, IS_L2 ? acc : -(acc + Kp), (IdT)(ls + v));
+                w.add(valid && slotSelected<MASKED>(slotMask, ls + v0), IS_L2 ? acc : -(acc + Kp), (IdT)(ls + v));
             }
         }
     }
@@ -433,7 +435,8 @@ void runIvfSqScan(
         MetricType metric,
         float* outD,
         idx_t* outI,
-        cudaStream_t stream) {
+        cudaStream_t stream,
+        const uint32_t* slotMask) {
     if (nq == 0)
         return;
     const int codec = sqCodec(qtype);
@@ -453,12 +456,14 @@ void runIvfSqScan(
         withInt<SQC_BYTE, SQC_NIBBLE, SQC_SIX, SQC_HALF>(codec, [&](auto c) {
             withBool(l2, [&](auto isL2) {
                 withBool(wide, [&](auto wideIds) {
-                    auto kern = ivfsq_scan_kernel<c, isL2, ScanIdT<decltype(wideIds)>>;
-                    CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                    kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
-                            Q + b.q0 * d, d, probes + b.q0 * nprobe, cdis ? cdis + b.q0 * nprobe : nullptr, nprobe,
-                            b.probesPerCta, coarse, decodeMB, listStart, listLen, arenaCodes, arenaIds, codeSize, fast,
-                            k, LIST, b.partD, b.partI);
+                    withBool(slotMask != nullptr, [&](auto masked) {
+                        auto kern = ivfsq_scan_kernel<c, isL2, ScanIdT<decltype(wideIds)>, masked>;
+                        CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                        kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
+                                Q + b.q0 * d, d, probes + b.q0 * nprobe, cdis ? cdis + b.q0 * nprobe : nullptr, nprobe,
+                                b.probesPerCta, coarse, decodeMB, listStart, listLen, arenaCodes, arenaIds, codeSize,
+                                fast, k, LIST, b.partD, b.partI, slotMask);
+                    });
                 });
             });
         });

@@ -22,6 +22,7 @@ void runL2Norms(const float* x, int64_t n, int d, float* norms, cudaStream_t str
 //   Q [nq,d], Y [n,d] row-major; outD [nq,k], outI [nq,k] (int64, row index + idBase; -1 missing)
 //   yHalf: Y holds __half rows (GpuIndexFlatConfig::useFloat16 storage), widened to fp32 on load
 //   metricArg: the exponent p of METRIC_Lp (ignored by the other metrics)
+//   rowMask: null, or [ceil(n/32)] words: only rows whose bit is set can be returned (SearchParameters::sel)
 void runFlatExact(
         GpuResources* res,
         int device,
@@ -37,7 +38,8 @@ void runFlatExact(
         idx_t* outI,
         cudaStream_t stream,
         int yHalf = 0,
-        float metricArg = 0.f);
+        float metricArg = 0.f,
+        const uint32_t* rowMask = nullptr);
 
 // k = 1 convenience (assignment): outI int64 [nq], outD optional
 void runFlatArgmin(
@@ -55,7 +57,7 @@ void runFlatArgmin(
 
 // Row-wise top-k over candidate lists (role of runBlockSelectPair / merge_knn_results,
 // faiss/gpu/utils/BlockSelectFloat.cu:98, faiss/utils/Heap.cpp:166-238).
-//   inD/inI: [rows, nlists, kin]; ids < 0 are skipped; idOffsets (optional, [nlists]) is added to
+//   inD/inI: [rows, nlists, kin]; ids == -1 are skipped; idOffsets (optional, [nlists]) is added to
 //   ids of list l (IndexShards successive_ids translation, faiss/IndexShards.cpp:214-220).
 //   Keys are user-facing distances (larger is better for is_similarity_metric: IP, Jaccard).
 void runMergeTopK(
@@ -176,7 +178,12 @@ void runFlatTcSearch(
         idx_t* outI,
         cudaStream_t stream,
         const FlatTcShard* shard = nullptr,
-        int yHalf = 0);
+        int yHalf = 0,
+        const uint32_t* rowMask = nullptr); // passed to the exact recompute of certificate failures
+
+// per-tile max / min of a stored-order bias array [round_up(n, 256) + 256] into tileMaxBias (the layout
+// runFlatTcPrepareRows writes): recomputed after a selector's mask set excluded rows' biases to -inf
+void runFlatTcTileBias(const float* bias, int64_t n, float* tileMaxBias, cudaStream_t stream);
 
 // number of queries the last runFlatTcSearch on this thread recomputed with the exact kernel
 int& lastFlatTcFallbacks();
@@ -276,7 +283,8 @@ void runIvfFlatScan(
         MetricType metric,
         float* outD,
         idx_t* outI,
-        cudaStream_t stream);
+        cudaStream_t stream,
+        const uint32_t* slotMask = nullptr); // SearchParameters::sel over the arena, or null
 
 // IVF-PQ list scan (role of runPQScanMultiPassNoPrecomputed + pqCodeDistances,
 // faiss/gpu/impl/PQScanMultiPassNoPrecomputed-inl.cuh:527, PQCodeDistances-inl.cuh:591): the
@@ -307,7 +315,8 @@ void runIvfPqScan(
         MetricType metric,
         float* outD,
         idx_t* outI,
-        cudaStream_t stream);
+        cudaStream_t stream,
+        const uint32_t* slotMask = nullptr); // SearchParameters::sel over the arena, or null
 
 // ---------------------------------------------------------------- ivfsq_scan.cu
 // ScalarQuantizer::QuantizerType values (faiss/impl/ScalarQuantizer.h:27-34) the GPU index accepts
@@ -368,7 +377,8 @@ void runIvfSqScan(
         MetricType metric,
         float* outD,
         idx_t* outI,
-        cudaStream_t stream);
+        cudaStream_t stream,
+        const uint32_t* slotMask = nullptr); // SearchParameters::sel over the arena, or null
 
 // ---- "rotated, interleaved-by-32" PQ code layout (native storage for M % 16 == 0, M <= 32) ----
 // List-relative vector v = 32*g + t is stored in group g; byte position j of the vector holds
@@ -428,6 +438,7 @@ void runIvfPqScanInterleaved(
         MetricType metric,
         float* outD,
         idx_t* outI,
-        cudaStream_t stream);
+        cudaStream_t stream,
+        const uint32_t* slotMask = nullptr); // SearchParameters::sel over the arena, or null
 
 } // namespace fb200

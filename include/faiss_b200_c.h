@@ -199,7 +199,42 @@ typedef struct FaissSearchParameters_H FaissSearchParameters;
 typedef struct FaissSearchParameters_H FaissSearchParametersIVF;
 FB200_API int faiss_SearchParametersIVF_new_with(FaissSearchParametersIVF** p_sp, size_t nprobe, size_t max_codes);
 FB200_API void faiss_SearchParameters_free(FaissSearchParameters* sp);
-/* c_api/Index_c.h faiss_Index_search_with_params: per-call nprobe for IVF indexes (max_codes must be 0, no IDSelector) */
+
+/* ---- IDSelector (c_api/impl/AuxIndexStructures_c.h names and argument order; faiss/impl/IDSelector.h semantics).
+   A selector restricts a search to the stored ids it accepts: the row number for GpuIndexFlat, the id stored
+   in the list (add_with_ids) for the IVF indexes, whose coarse search is not filtered.  Leaves copy their
+   inputs; Not / And / Or / XOr keep pointers to their operands, which must outlive them.  Array and Batch
+   select by membership (duplicates and ids past ntotal are harmless); an empty Range selects nothing. ---- */
+typedef struct FaissIDSelector_H FaissIDSelector;
+typedef struct FaissIDSelector_H FaissIDSelectorRange;
+typedef struct FaissIDSelector_H FaissIDSelectorArray;
+typedef struct FaissIDSelector_H FaissIDSelectorBatch;
+typedef struct FaissIDSelector_H FaissIDSelectorBitmap;
+typedef struct FaissIDSelector_H FaissIDSelectorNot;
+typedef struct FaissIDSelector_H FaissIDSelectorAnd;
+typedef struct FaissIDSelector_H FaissIDSelectorOr;
+typedef struct FaissIDSelector_H FaissIDSelectorXOr;
+FB200_API void faiss_IDSelector_free(FaissIDSelector* sel);
+/* 1 if id is selected, 0 if not, -1 on a null handle */
+FB200_API int faiss_IDSelector_is_member(const FaissIDSelector* sel, idx_t id);
+FB200_API int faiss_IDSelectorRange_new(FaissIDSelectorRange** p_sel, idx_t imin, idx_t imax);
+FB200_API int faiss_IDSelectorArray_new(FaissIDSelectorArray** p_sel, size_t n, const idx_t* ids);
+FB200_API int faiss_IDSelectorBatch_new(FaissIDSelectorBatch** p_sel, size_t n, const idx_t* indices);
+/* bit (id & 7) of byte id >> 3, for id >> 3 < n */
+FB200_API int faiss_IDSelectorBitmap_new(FaissIDSelectorBitmap** p_sel, size_t n, const uint8_t* bitmap);
+FB200_API int faiss_IDSelectorNot_new(FaissIDSelectorNot** p_sel, const FaissIDSelector* sel);
+FB200_API int faiss_IDSelectorAnd_new(FaissIDSelectorAnd** p_sel, const FaissIDSelector* lhs_sel, const FaissIDSelector* rhs_sel);
+FB200_API int faiss_IDSelectorOr_new(FaissIDSelectorOr** p_sel, const FaissIDSelector* lhs_sel, const FaissIDSelector* rhs_sel);
+FB200_API int faiss_IDSelectorXOr_new(FaissIDSelectorXOr** p_sel, const FaissIDSelector* lhs_sel, const FaissIDSelector* rhs_sel);
+/* a selector this library cannot see into: is_member(id) = (is_member(ctx, id) != 0), called on the host once per
+   stored entry and search call */
+FB200_API int faiss_b200_IDSelectorCallback_new(FaissIDSelector** p_sel, int (*is_member)(void* ctx, idx_t id), void* ctx);
+/* c_api/Index_c.h:44 and c_api/IndexIVF_c.h faiss_SearchParametersIVF_new_with: sel may be NULL and is not owned */
+FB200_API int faiss_SearchParameters_new(FaissSearchParameters** p_sp, FaissIDSelector* sel);
+FB200_API int faiss_SearchParametersIVF_new_with_sel(FaissSearchParametersIVF** p_sp, FaissIDSelector* sel, size_t nprobe, size_t max_codes);
+
+/* c_api/Index_c.h faiss_Index_search_with_params: per-call nprobe for IVF indexes (max_codes must be 0) and an
+   IDSelector for GPU indexes */
 FB200_API int faiss_Index_search_with_params(const FaissIndex* index, idx_t n, const float* x, idx_t k, const FaissSearchParameters* params, float* distances, idx_t* labels);
 /* polled between query pages, add pages and clustering iterations; non-zero return -> the running call fails with
    "computation interrupted" (-2).  NULL clears it. */
