@@ -33,14 +33,19 @@ __global__ void pq_encode_kernel(
         int ksub,
         int dsubRt,
         const float* __restrict__ pq,
-        uint8_t* __restrict__ codes) {
-    extern __shared__ float cent[]; // [ksub][dsub]
+        uint8_t* __restrict__ codes,
+        bool stageInSmem) {
+    extern __shared__ float centSmem[]; // [ksub][dsub] when staged
     const int dsub = DSUB > 0 ? DSUB : dsubRt;
     const int m = blockIdx.y;
     const float* src = pq + (size_t)m * ksub * dsub;
-    for (int i = threadIdx.x; i < ksub * dsub; i += blockDim.x)
-        cent[i] = src[i];
-    __syncthreads();
+    const float* cent = src; // a codebook larger than shared memory (ksub * dsub * 4 > 227 KiB) is read from L1/L2
+    if (stageInSmem) { // block-uniform
+        for (int i = threadIdx.x; i < ksub * dsub; i += blockDim.x)
+            centSmem[i] = src[i];
+        __syncthreads();
+        cent = centSmem;
+    }
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n)
         return;
@@ -93,13 +98,19 @@ void runPQEncode(
         return;
     FB_THROW_IF_NOT(ksub <= 256 && d % M == 0);
     const int dsub = d / M;
-    size_t smem = sizeof(float) * ksub * dsub;
+    // the sub-quantiser's codebook is staged in shared memory when it fits the per-block opt-in limit; with
+    // ksub = 256 that holds up to dsub = 227, and larger sub-vectors (e.g. d = 1024, M = 4) read it from global
+    int device = 0, smemOptin = 0;
+    CUDA_VERIFY(cudaGetDevice(&device));
+    CUDA_VERIFY(cudaDeviceGetAttribute(&smemOptin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+    const bool stage = sizeof(float) * ksub * dsub <= (size_t)smemOptin;
+    const size_t smem = stage ? sizeof(float) * ksub * dsub : 0;
     dim3 grid((unsigned)ceil_div(n, 128), (unsigned)M);
 #define PQENC(DS)                                                                                      \
     do {                                                                                               \
         CUDA_VERIFY(cudaFuncSetAttribute(                                                              \
                 pq_encode_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));        \
-        pq_encode_kernel<DS><<<grid, 128, smem, stream>>>(resid, n, d, M, ksub, dsub, pq, codes);      \
+        pq_encode_kernel<DS><<<grid, 128, smem, stream>>>(resid, n, d, M, ksub, dsub, pq, codes, stage); \
     } while (0)
     switch (dsub) {
         case 1:
