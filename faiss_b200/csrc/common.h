@@ -12,6 +12,7 @@
 #include <exception>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 namespace fb200 {
 
@@ -153,6 +154,15 @@ inline int next_pow2(int v) {
     while (p < v)
         p <<= 1;
     return p;
+}
+
+// runtime value -> compile-time constant for a launcher's kernel template: f(std::true_type{}) or f(std::false_type{})
+template <typename F>
+void withBool(bool b, F&& f) {
+    if (b)
+        f(std::true_type{});
+    else
+        f(std::false_type{});
 }
 
 } // namespace fb200

@@ -35,6 +35,7 @@
 #include <vector>
 
 #include "comm.h"
+#include "flat_tc.h"
 #include "kernels.h"
 #include "select.cuh"
 #include "tc_ptx.cuh"
@@ -117,6 +118,12 @@ __global__ void tc_prepare_rows_kernel(
     }
 }
 
+__global__ void fill_float_kernel(float* out, int64_t n, float v) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n)
+        out[i] = v;
+}
+
 __global__ void tc_iota_kernel(int* v, int64_t n) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n)
@@ -145,6 +152,23 @@ __global__ void tc_tile_max_bias_kernel(const float* __restrict__ bias, int64_t 
         tileMax[t] = m;
         tileMax[numTiles + 1 + t] = mn;
     }
+}
+
+// bias copy with -inf at rows whose mask bit is clear: out[p] = mask[perm[p]] ? bias[p] : -inf for p < n (perm null:
+// identity), -inf for n <= p < padRows
+__global__ void mask_bias_kernel(
+        const float* __restrict__ bias, const int* __restrict__ perm, const uint32_t* __restrict__ mask, int64_t n,
+        int64_t padRows, float* __restrict__ out) {
+    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= padRows)
+        return;
+    float b = -CUDART_INF_F;
+    if (p < n) {
+        const int64_t r = perm ? perm[p] : p;
+        if ((mask[r >> 5] >> (r & 31)) & 1u)
+            b = bias[p];
+    }
+    out[p] = b;
 }
 
 // per-batch query preparation: power-of-two scale from absmax, fp16 conversion, eps, 1/(sq*sy)
@@ -325,7 +349,6 @@ __global__ void tc_select_kernel(
 // by a 32-step bitwise bisection (one compare per register and step + one warp reduction), and the entries above the
 // new threshold are written back compacted (unsorted; the exact re-rank orders them).  ~2-3 k instructions per query
 // and round instead of the ~15 k of the bitonic list maintenance, and no bank conflicts.
-constexpr int kSelCap = 1536;
 constexpr int kSelPerLane = kSelCap / 32;
 constexpr int kSelWarps = 4;
 
@@ -791,15 +814,6 @@ CUtensorMap makeTileMap(const __half* base, int64_t rows, int dpad, int boxRows,
     return m;
 }
 
-unsigned long long gcd64(unsigned long long a, unsigned long long b) {
-    while (b) {
-        unsigned long long t = a % b;
-        a = b;
-        b = t;
-    }
-    return a;
-}
-
 struct SmemPlan {
     int yStages;
     size_t bytes;
@@ -826,6 +840,29 @@ SmemPlan planSmem(int KB, int kSteps) {
     return {ys, fixed + ys * stage, ksplit, pipe, boxRows};
 }
 
+// the kernel's parameters for one round over nq queries (the search's pointers are filled in by the caller)
+TcParams roundParams(const SmemPlan& sp, int KB, int kSteps, int64_t nq, int64_t qPairs, const FlatTcRound& r, int64_t T,
+                     unsigned long long permA, unsigned long long permB, const float* invScale) {
+    TcParams p{};
+    p.slices = r.slices;
+    p.qPairs = (int)qPairs;
+    p.numUnits = (int)(qPairs * r.slices);
+    p.tileBegin = (int)std::min<int64_t>(r.begin, T); // schedule laid out over the largest shard: clamp to ours
+    p.tileEnd = (int)std::min<int64_t>(r.end, T);
+    p.tilesPerSlice = r.tilesPerSlice;
+    p.permA = permA;
+    p.permB = permB;
+    p.numTiles = (unsigned long long)T;
+    p.KB = KB;
+    p.ksplit = sp.ksplit;
+    p.kSteps = kSteps;
+    p.yStages = sp.yStages;
+    p.invScalePtr = invScale;
+    p.cap = r.cap;
+    p.nq = (int)nq;
+    return p;
+}
+
 template <bool DUMP>
 void launchTc(const CUtensorMap& mq, const CUtensorMap& my, const TcParams& p, int grid, const SmemPlan& sp, cudaStream_t stream, bool self = false) {
     const size_t smem = sp.bytes;
@@ -839,12 +876,9 @@ void launchTc(const CUtensorMap& mq, const CUtensorMap& my, const TcParams& p, i
     CUDA_CHECK_LAST();
 }
 
-} // namespace
-
-// ------------------------------------------------------------------------------------------
-// public launchers
-// ------------------------------------------------------------------------------------------
-void runAbsMax(const void* x, int64_t count, float* out, cudaStream_t stream, int yHalf) {
+// max |x| over a matrix into a zeroed device scalar (float) -- picks the power-of-two fp16 scale; on non-negative
+// values (squared norms), their max
+void runAbsMax(const void* x, int64_t count, float* out, cudaStream_t stream, int yHalf = 0) {
     if (count == 0)
         return;
     int blocks = (int)std::min<int64_t>(1184, ceil_div(count, 256));
@@ -852,59 +886,15 @@ void runAbsMax(const void* x, int64_t count, float* out, cudaStream_t stream, in
     CUDA_CHECK_LAST();
 }
 
-void runMaxOf(const float* x, int64_t count, float* out, cudaStream_t stream) {
-    runAbsMax(x, count, out, stream, 0);
-}
-
-void runFlatTcPrepareRows(
-        GpuResources* res,
-        int device,
-        const void* Y,
-        int64_t n,
-        int d,
-        int dpad,
-        float scale,
-        MetricType metric,
-        __half* Y16,
-        float* bias,
-        int* perm,
-        float* tileMaxBias,
-        float* norms,
-        cudaStream_t stream,
-        int yHalf) {
-    if (n == 0)
-        return;
-    const int warps = 8;
-    const unsigned rowBlocks = (unsigned)ceil_div(n, warps);
-    const int isL2 = metric == METRIC_L2 ? 1 : 0;
-    // squared norms in row order (also feeds the caller's max-norm reduction)
-    tc_prepare_rows_kernel<<<rowBlocks, warps * 32, 0, stream>>>(Y, yHalf, n, d, dpad, scale, isL2, nullptr, nullptr, nullptr, norms);
-    CUDA_CHECK_LAST();
-    if (perm) {
-        // stored order = rows sorted by squared norm: the biases of a 256-row tile are then nearly
-        // equal, which is what makes the kernel's per-tile score bound tight (flat_tc_kernel.cuh)
-        auto keysOut = res->temp(device, sizeof(float) * n);
-        auto valsIn = res->temp(device, sizeof(int) * n);
-        tc_iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, stream>>>(valsIn.as<int>(), n);
-        CUDA_CHECK_LAST();
-        size_t tmpBytes = 0;
-        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
-                nullptr, tmpBytes, norms, keysOut.as<float>(), valsIn.as<int>(), perm, (int)n, 0, 32, stream));
-        auto tmp = res->temp(device, tmpBytes);
-        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
-                tmp.data, tmpBytes, norms, keysOut.as<float>(), valsIn.as<int>(), perm, (int)n, 0, 32, stream));
-    }
-    tc_prepare_rows_kernel<<<rowBlocks, warps * 32, 0, stream>>>(Y, yHalf, n, d, dpad, scale, isL2, perm, Y16, bias, nullptr);
-    CUDA_CHECK_LAST();
-    runFlatTcTileBias(bias, n, tileMaxBias, stream);
-}
-
-void runFlatTcTileBias(const float* bias, int64_t n, float* tileMaxBias, cudaStream_t stream) {
+// per-tile max / min of a stored-order bias array [round_up(n, 256) + 256] (see FlatTcDatabase)
+void runTileBias(const float* bias, int64_t n, float* tileBias, cudaStream_t stream) {
     const int warps = 8;
     const int64_t numTiles = ceil_div(n, kTileN);
-    tc_tile_max_bias_kernel<<<(unsigned)ceil_div(numTiles, warps), warps * 32, 0, stream>>>(bias, numTiles, tileMaxBias);
+    tc_tile_max_bias_kernel<<<(unsigned)ceil_div(numTiles, warps), warps * 32, 0, stream>>>(bias, numTiles, tileBias);
     CUDA_CHECK_LAST();
 }
+
+} // namespace
 
 bool flatTcSupported(int d, int k, int64_t n) {
     int dpad = (int)round_up(d, kKBlock);
@@ -913,14 +903,301 @@ bool flatTcSupported(int d, int k, int64_t n) {
     return dpad <= kMaxKB * kKBlock && k >= 1 && k <= 2048 && n >= (k == 1 ? 2048 : 32768) && n < (int64_t(1) << 31) - 512;
 }
 
-void runFlatTcScoresDebug(
-        const __half* Q16,
-        int64_t nq,
-        const __half* Y16,
-        int64_t n,
-        int dpad,
-        float* S,
-        cudaStream_t stream) {
+FlatTcDatabase::FlatTcDatabase(GpuResources* res, int device, int d)
+        : res_(res),
+          device_(device),
+          d_(d),
+          dpad_((int)round_up(d, kKBlock)),
+          y16_(res, device, AllocType::FlatData),
+          bias_(res, device, AllocType::FlatData),
+          perm_(res, device, AllocType::FlatData),
+          tileBias_(res, device, AllocType::FlatData) {}
+
+void FlatTcDatabase::clear() {
+    y16_.clear();
+    bias_.clear();
+    perm_.clear();
+    tileBias_.clear();
+    dirty_ = true;
+}
+
+void FlatTcDatabase::prepare(const void* rows, int64_t n, MetricType metric, int yHalf, cudaStream_t stream) {
+    if (!dirty_)
+        return;
+    const int d = d_, dpad = dpad_;
+    const int64_t padRows = round_up(n, 256) + 256; // whole 256-row tiles, -inf beyond n
+    y16_.resize((size_t)n * dpad, stream);
+    bias_.resize((size_t)padRows, stream);
+    tileBias_.resize((size_t)(padRows / 256) * 2, stream); // [T+1] max bias per tile, then [T+1] min bias per tile
+    const bool sorted = metric == METRIC_L2; // IP has no bias: row order is kept
+    if (sorted)
+        perm_.resize((size_t)n, stream);
+    else
+        perm_.clear();
+    auto scal = res_->temp(device_, sizeof(float) * 2);
+    auto norms = res_->temp(device_, sizeof(float) * n);
+    CUDA_VERIFY(cudaMemsetAsync(scal.data, 0, sizeof(float) * 2, stream));
+    runAbsMax(rows, n * (int64_t)d, scal.as<float>(), stream, yHalf);
+    float h[2] = {0.f, 0.f};
+    CUDA_VERIFY(cudaMemcpyAsync(h, scal.data, sizeof(float), cudaMemcpyDeviceToHost, stream));
+    CUDA_VERIFY(cudaStreamSynchronize(stream));
+    float scale = 1.f;
+    if (h[0] > 0.f) {
+        int e;
+        std::frexp(h[0], &e);
+        scale = std::ldexp(1.f, 14 - e); // max |y| * scale in [2^13, 2^14)
+    }
+    fill_float_kernel<<<(unsigned)ceil_div(padRows, 256), 256, 0, stream>>>(bias_.data(), padRows, -INFINITY);
+    CUDA_CHECK_LAST();
+    const int warps = 8;
+    const unsigned rowBlocks = (unsigned)ceil_div(n, warps);
+    int* perm = sorted ? perm_.data() : nullptr;
+    // squared norms in row order (also feed the max-norm reduction)
+    tc_prepare_rows_kernel<<<rowBlocks, warps * 32, 0, stream>>>(
+            rows, yHalf, n, d, dpad, scale, sorted, nullptr, nullptr, nullptr, norms.as<float>());
+    CUDA_CHECK_LAST();
+    if (perm) {
+        // stored order = rows sorted by squared norm: the biases of a 256-row tile are then nearly
+        // equal, which is what makes the kernel's per-tile score bound tight (flat_tc_kernel.cuh)
+        auto keysOut = res_->temp(device_, sizeof(float) * n);
+        auto valsIn = res_->temp(device_, sizeof(int) * n);
+        tc_iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, stream>>>(valsIn.as<int>(), n);
+        CUDA_CHECK_LAST();
+        size_t tmpBytes = 0;
+        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
+                nullptr, tmpBytes, norms.as<float>(), keysOut.as<float>(), valsIn.as<int>(), perm, (int)n, 0, 32, stream));
+        auto tmp = res_->temp(device_, tmpBytes);
+        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
+                tmp.data, tmpBytes, norms.as<float>(), keysOut.as<float>(), valsIn.as<int>(), perm, (int)n, 0, 32, stream));
+    }
+    tc_prepare_rows_kernel<<<rowBlocks, warps * 32, 0, stream>>>(
+            rows, yHalf, n, d, dpad, scale, sorted, perm, y16_.data(), bias_.data(), nullptr);
+    CUDA_CHECK_LAST();
+    runTileBias(bias_.data(), n, tileBias_.data(), stream);
+    runAbsMax(norms.as<float>(), n, scal.as<float>() + 1, stream);
+    CUDA_VERIFY(cudaMemcpyAsync(h, scal.data, sizeof(float) * 2, cudaMemcpyDeviceToHost, stream));
+    CUDA_VERIFY(cudaStreamSynchronize(stream));
+    scale_ = scale;
+    maxNorm_ = std::sqrt(h[1]) * 1.0001f;
+    rows_ = rows;
+    n_ = n;
+    metric_ = metric;
+    yHalf_ = yHalf;
+    dirty_ = false;
+}
+
+// one search call: the schedule, the launch configuration and the bias arrays (the masked copies under a row mask)
+struct FlatTcDatabase::Call {
+    cudaStream_t stream;
+    const FlatTcSchedule& s;
+    int KB, kSteps;
+    SmemPlan sp;
+    const float* bias;
+    const float* tileBias;
+    CUtensorMap mapY;
+    const FlatTcShard* shard;
+};
+
+// device state of one query batch
+struct FlatTcDatabase::Batch {
+    const float* Q; // [nq][d]
+    int64_t nq, qPairs;
+    GpuMemoryReservation q16, scal, eps, thr, flags, baseKey, baseId;
+    CUtensorMap mapQ;
+};
+
+// the batch's queries -> scaled fp16 tiles, eps and thresholds; empty base lists
+void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
+    const int64_t nq = b.nq, qPairs = b.qPairs;
+    cudaStream_t stream = c.stream;
+    b.q16 = res_->temp(device_, sizeof(__half) * qPairs * kUnitM * dpad_);
+    b.scal = res_->temp(device_, sizeof(float) * 4); // [absmax, qScale, inv, -]
+    b.eps = res_->temp(device_, sizeof(float) * nq);
+    b.thr = res_->temp(device_, sizeof(float) * nq);
+    b.flags = res_->temp(device_, sizeof(int) * (nq + 1));
+    b.baseKey = res_->temp(device_, c.s.streaming ? sizeof(float) : sizeof(float) * nq * c.s.LIST);
+    b.baseId = res_->temp(device_, c.s.streaming ? sizeof(int) : sizeof(int) * nq * c.s.LIST);
+
+    // error model constants (DESIGN.md): fp16 rounding of both operands + fp32 accumulation slack
+    const float c1 = 1.01f * (ldexpf(1.f, -10) + (float)dpad_ * ldexpf(1.f, -22));
+    const float c2 = (float)(dpad_ + 16) * ldexpf(1.f, -24);
+
+    CUDA_VERIFY(cudaMemsetAsync(b.scal.data, 0, sizeof(float) * 4, stream));
+    CUDA_VERIFY(cudaMemsetAsync(b.flags.data, 0, sizeof(int) * (nq + 1), stream));
+    CUDA_VERIFY(cudaMemsetAsync(b.q16.data, 0, sizeof(__half) * qPairs * kUnitM * dpad_, stream));
+    float* sc = b.scal.as<float>();
+    runAbsMax(b.Q, nq * d_, sc + 0, stream);
+    tc_query_scale_kernel<<<1, 1, 0, stream>>>(sc + 0, scale_, sc + 1, sc + 2);
+    CUDA_CHECK_LAST();
+    tc_prepare_queries_kernel<<<(unsigned)ceil_div(nq, 8), 256, 0, stream>>>(
+            b.Q, nq, d_, dpad_, sc + 1, c1, c2, maxNorm_, b.q16.as<__half>(), b.eps.as<float>(), b.thr.as<float>());
+    CUDA_CHECK_LAST();
+    if (!c.s.streaming) {
+        int64_t cnt = nq * c.s.LIST;
+        tc_init_base_kernel<<<(unsigned)ceil_div(cnt, 256), 256, 0, stream>>>(b.baseKey.as<float>(), b.baseId.as<int>(), cnt);
+        CUDA_CHECK_LAST();
+    }
+    b.mapQ = makeTileMap(b.q16.as<__half>(), qPairs * kUnitM, dpad_, kTileM);
+}
+
+// One round: score its tiles and emit candidates, then fold them into the base lists and thresholds (and, sharded,
+// pool the thresholds across the ranks) -- or, streaming, select and re-rank in one pass into outD / outI.
+void FlatTcDatabase::runRound(const Call& c, const Batch& b, const FlatTcRound& r, uint2* arena, int* counts, float* contrib,
+                              float* outD, idx_t* outI) const {
+    const FlatTcSchedule& s = c.s;
+    cudaStream_t stream = c.stream;
+    const int nq = (int)b.nq;
+    TcParams p = roundParams(c.sp, c.KB, c.kSteps, b.nq, b.qPairs, r, s.T, s.permA, s.permB, b.scal.as<float>() + 2);
+    p.bias = c.bias;
+    p.tileMaxBias = c.tileBias;
+    p.tileMinBias = c.tileBias + s.T + 1; // second half of the array (see tc_tile_max_bias_kernel)
+    p.thr = b.thr.as<float>();
+    p.eps = b.eps.as<float>();
+    p.cand = arena;
+    p.candCount = counts;
+    if (p.tileBegin < p.tileEnd) {
+        launchTc<false>(b.mapQ, c.mapY, p, std::min(p.numUnits, s.sms), c.sp, stream, s.streaming);
+    } else { // this shard has no tiles in this round of the common schedule: no candidates
+        CUDA_VERIFY(cudaMemsetAsync(counts, 0, (size_t)p.numUnits * kSegsPerUnit * sizeof(int), stream));
+    }
+    if (s.streaming) { // select + exact re-rank fused: one warp per query
+        const int fw = 8;
+        KernelTiming::begin("tc_argmin_finish", stream);
+        withBool(metric_ == METRIC_L2, [&](auto l2) {
+            withBool(yHalf_ != 0, [&](auto yh) {
+                tc_argmin_finish_kernel<l2, yh><<<(unsigned)ceil_div(nq, fw), fw * 32, 0, stream>>>(
+                        nq, d_, r.slices, kParts, arena, r.cap, counts, b.eps.as<float>(), b.Q, rows_, perm_.data(), outD, outI,
+                        b.flags.as<int>());
+            });
+        });
+        KernelTiming::end("tc_argmin_finish", stream);
+        CUDA_CHECK_LAST();
+        return;
+    }
+    // the two selection kernels take the same arguments
+    const auto sel = s.useBisect ? tc_select_bisect_kernel : tc_select_kernel;
+    const size_t listBytes = SmemTopK<int>::bytes(s.LIST, kSelectBuf);
+    const int selWarps = s.useBisect ? kSelWarps : (int)std::max<size_t>(1, std::min<size_t>(8, (48 * 1024) / listBytes));
+    const size_t selSmem = s.useBisect ? sizeof(uint2) * kSelCap * kSelWarps : listBytes * selWarps;
+    CUDA_VERIFY(cudaFuncSetAttribute(sel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)selSmem));
+    KernelTiming::begin("tc_select", stream);
+    sel<<<(unsigned)ceil_div(nq, selWarps), selWarps * 32, selSmem, stream>>>(
+            nq, s.k, s.LIST, r.slices, kParts, arena, r.cap, counts, b.eps.as<float>(), b.baseKey.as<float>(),
+            b.baseId.as<int>(), b.thr.as<float>(), b.flags.as<int>(), contrib, s.kFrac);
+    KernelTiming::end("tc_select", stream);
+    CUDA_CHECK_LAST();
+    if (c.shard) {
+        KernelTiming::begin("tc_pool", stream);
+        // ONE small all-reduce per round (2 floats per query): every shard then filters against a
+        // threshold certified by the pooled evidence of all shards
+        c.shard->comm->allReduceMax(contrib, (size_t)2 * nq, stream);
+        tc_pooled_thr_kernel<<<(unsigned)ceil_div(nq, 256), 256, 0, stream>>>(nq, contrib, b.eps.as<float>(), b.thr.as<float>());
+        KernelTiming::end("tc_pool", stream);
+        CUDA_CHECK_LAST();
+    }
+}
+
+// exact re-rank of the base lists into outD / outI, sorted by (distance, id)
+void FlatTcDatabase::rerank(const Call& c, const Batch& b, float* outD, idx_t* outI) const {
+    const FlatTcSchedule& s = c.s;
+    cudaStream_t stream = c.stream;
+    const int rrWarps = (int)std::max<size_t>(1, std::min<size_t>(8, (48 * 1024) / SmemTopK<int>::bytes(s.KL, 64)));
+    const size_t rrSmem = SmemTopK<int>::bytes(s.KL, 64) * rrWarps;
+    KernelTiming::begin("tc_rerank", stream);
+    withBool(metric_ == METRIC_L2, [&](auto l2) {
+        withBool(yHalf_ != 0, [&](auto yh) {
+            auto kern = tc_rerank_kernel<l2, yh>;
+            CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rrSmem));
+            kern<<<(unsigned)ceil_div(b.nq, rrWarps), rrWarps * 32, rrSmem, stream>>>(
+                    (int)b.nq, d_, s.k, s.LIST, s.KL, b.Q, rows_, perm_.data(), b.baseId.as<int>(), b.baseKey.as<float>(),
+                    c.shard ? b.thr.as<float>() : nullptr, outD, outI);
+        });
+    });
+    KernelTiming::end("tc_rerank", stream);
+    CUDA_CHECK_LAST();
+}
+
+// certificate failures -> exact SIMT recompute into outD / outI; returns their number
+int FlatTcDatabase::recomputeFallbacks(const Call& c, const Batch& b, const uint32_t* rowMask, float* outD, idx_t* outI) const {
+    const int k = c.s.k;
+    const int64_t nq = b.nq;
+    cudaStream_t stream = c.stream;
+    auto list = res_->temp(device_, sizeof(int) * nq);
+    int* countDev = b.flags.as<int>() + nq;
+    tc_collect_flags_kernel<<<(unsigned)ceil_div(nq, 256), 256, 0, stream>>>(b.flags.as<int>(), (int)nq, list.as<int>(), countDev);
+    CUDA_CHECK_LAST();
+    int nflag = 0;
+    CUDA_VERIFY(cudaMemcpyAsync(&nflag, countDev, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    CUDA_VERIFY(cudaStreamSynchronize(stream));
+    if (nflag > 0) {
+        auto fq = res_->temp(device_, sizeof(float) * (size_t)nflag * d_);
+        auto fD = res_->temp(device_, sizeof(float) * (size_t)nflag * k);
+        auto fI = res_->temp(device_, sizeof(idx_t) * (size_t)nflag * k);
+        tc_gather_queries_kernel<<<nflag, 128, 0, stream>>>(b.Q, list.as<int>(), d_, fq.as<float>());
+        CUDA_CHECK_LAST();
+        runFlatExact(
+                res_, device_, fq.as<float>(), nflag, rows_, n_, d_, k, metric_, 0, fD.as<float>(), fI.as<idx_t>(), stream,
+                yHalf_, 0.f, rowMask);
+        tc_scatter_results_kernel<<<nflag, 128, 0, stream>>>(fD.as<float>(), fI.as<idx_t>(), list.as<int>(), k, outD, outI);
+        CUDA_CHECK_LAST();
+        CUDA_VERIFY(cudaStreamSynchronize(stream));
+    }
+    return nflag;
+}
+
+int64_t FlatTcDatabase::search(const float* Q, int64_t nqAll, int k, float* outD, idx_t* outI, cudaStream_t stream,
+                               const FlatTcShard* shard, const uint32_t* rowMask) const {
+    FB_THROW_IF_NOT_MSG(!dirty_, "FlatTcDatabase::search before prepare");
+    if (nqAll == 0)
+        return 0;
+    const float* bias = bias_.data();
+    const float* tileBias = tileBias_.data();
+    GpuMemoryReservation maskedBias, maskedTileBias;
+    if (rowMask) {
+        // an excluded row gets a -inf bias: its score can then never pass a round's threshold, exactly as the
+        // padding rows past n.  maxNorm_ over all rows stays a valid bound for the certificate.
+        maskedBias = res_->temp(device_, sizeof(float) * bias_.size());
+        maskedTileBias = res_->temp(device_, sizeof(float) * tileBias_.size());
+        const int64_t padRows = (int64_t)bias_.size();
+        mask_bias_kernel<<<(unsigned)ceil_div(padRows, (int64_t)256), 256, 0, stream>>>(
+                bias_.data(), perm_.data(), rowMask, n_, padRows, maskedBias.as<float>());
+        CUDA_CHECK_LAST();
+        runTileBias(maskedBias.as<float>(), n_, maskedTileBias.as<float>(), stream);
+        bias = maskedBias.as<float>();
+        tileBias = maskedTileBias.as<float>();
+    }
+    FB_THROW_IF_NOT(flatTcSupported(d_, k, n_));
+    const int KB = dpad_ / kKBlock;
+    const int kSteps = (d_ + 15) / 16;
+    const FlatTcSchedule s = planFlatTcSchedule(
+            n_, k, res_->numSMs(device_), shard ? shard->comm->size() : 0, shard ? shard->maxTiles : 0);
+    const SmemPlan sp = planSmem(KB, kSteps);
+    const Call c{stream, s, KB, kSteps, sp, bias, tileBias, makeTileMap(y16_.data(), n_, dpad_, sp.boxRows, sp.ksplit), shard};
+    int64_t fallbacks = 0;
+    for (int64_t qb = 0; qb < nqAll; qb += s.qBatch) {
+        Batch b;
+        b.Q = Q + qb * d_;
+        b.nq = std::min(s.qBatch, nqAll - qb);
+        b.qPairs = ceil_div(b.nq, kUnitM);
+        prepareQueries(c, b);
+        const FlatTcRounds plan = s.rounds(b.qPairs);
+        auto arena = res_->temp(device_, plan.arenaBytes);
+        auto counts = res_->temp(device_, plan.countBytes);
+        GpuMemoryReservation contrib;
+        if (shard)
+            contrib = res_->temp(device_, sizeof(float) * 2 * b.nq);
+        float* oD = outD + qb * k;
+        idx_t* oI = outI + qb * k;
+        for (const FlatTcRound& r : plan.rounds)
+            runRound(c, b, r, arena.as<uint2>(), counts.as<int>(), contrib.as<float>(), oD, oI);
+        if (!s.streaming)
+            rerank(c, b, oD, oI);
+        fallbacks += recomputeFallbacks(c, b, rowMask, oD, oI);
+    }
+    return fallbacks;
+}
+
+void runFlatTcScoresDebug(const __half* Q16, int64_t nq, const __half* Y16, int64_t n, int dpad, float* S, cudaStream_t stream) {
     FB_THROW_IF_NOT(dpad % kKBlock == 0 && dpad <= kMaxKB * kKBlock);
     const int KB = dpad / kKBlock;
     const int kSteps = dpad / 16; // debug seam: operands arrive padded
@@ -938,354 +1215,18 @@ void runFlatTcScoresDebug(
     CUDA_VERIFY(cudaMallocAsync(&one, sizeof(float), stream));
     float h1 = 1.f;
     CUDA_VERIFY(cudaMemcpyAsync(one, &h1, sizeof(float), cudaMemcpyHostToDevice, stream));
-    TcParams p{};
-    p.slices = 1;
-    p.qPairs = (int)qPairs;
-    p.numUnits = (int)qPairs;
+    // every tile in one slice, unpermuted
+    const FlatTcRound all{0, (int)numTiles, 1, (int)numTiles, 0};
+    TcParams p = roundParams(sp, KB, kSteps, nq, qPairs, all, numTiles, 1, 0, one);
     CUtensorMap mq = makeTileMap(qpad, qPairs * kUnitM, dpad, kTileM);
-    p.tileBegin = 0;
-    p.tileEnd = (int)numTiles;
-    p.tilesPerSlice = (int)numTiles;
-    p.permA = 1;
-    p.permB = 0;
-    p.numTiles = (unsigned long long)numTiles;
-    p.KB = KB;
-    p.ksplit = sp.ksplit;
-    p.kSteps = kSteps;
-    p.yStages = sp.yStages;
-    p.invScalePtr = one;
-    p.bias = nullptr;
-    p.tileMaxBias = nullptr;
-    p.thr = nullptr;
-    p.cand = nullptr;
-    p.cap = 0;
-    p.candCount = nullptr;
     p.dump = S;
     p.dumpLd = numTiles * kTileN; // S must be [nq][numTiles*128]
-    p.nq = (int)nq;
     int dev = 0, sms = 0;
     CUDA_VERIFY(cudaGetDevice(&dev));
     CUDA_VERIFY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     launchTc<true>(mq, my, p, (int)std::min<int64_t>(p.numUnits, sms), sp, stream);
     CUDA_VERIFY(cudaFreeAsync(qpad, stream));
     CUDA_VERIFY(cudaFreeAsync(one, stream));
-}
-
-void runFlatTcSearch(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nqAll,
-        const void* Y,
-        const __half* Y16,
-        const float* bias,
-        const int* perm,
-        const float* tileMaxBias,
-        float yScale,
-        float yMaxNorm,
-        int64_t n,
-        int d,
-        int dpad,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const FlatTcShard* shard,
-        int yHalf,
-        const uint32_t* rowMask) {
-    if (nqAll == 0)
-        return;
-    FB_THROW_IF_NOT(flatTcSupported(d, k, n));
-    const int KB = dpad / kKBlock;
-    const int kSteps = (d + 15) / 16;
-    const SmemPlan sp = planSmem(KB, kSteps);
-    const int sms = res->numSMs(device);
-    const int64_t T = ceil_div(n, kTileN);
-    // Sharded search: every rank runs the SAME number of rounds (one all-reduce per round), so the schedule
-    // is laid out over the largest shard's tile count and clamped to this shard's.  Thresholds are pooled
-    // across ranks after every round, i.e. a round over t local tiles is worth S*t tiles of evidence: the first
-    // round shrinks by S and the rounds grow faster (fewer launches for a 1/S-size shard).
-    const int nShards = shard ? shard->comm->size() : 1;
-    const int64_t Tsched = shard ? std::max<int64_t>(T, shard->maxTiles) : T;
-    const int kFrac = (k + nShards - 1) / nShards;
-    const int LIST = std::max(128, next_pow2(2 * k));
-    const int KL = std::max(64, next_pow2(k));
-
-    // tile permutation: multiplicative hash with a multiplier coprime to T
-    unsigned long long A = (unsigned long long)((double)T * 0.6180339887498949);
-    if (A < 1)
-        A = 1;
-    while (gcd64(A, (unsigned long long)T) != 1)
-        A++;
-    const unsigned long long B = (unsigned long long)(T / 3);
-
-    // error model constants (DESIGN.md): fp16 rounding of both operands + fp32 accumulation slack
-    const float c1 = 1.01f * (ldexpf(1.f, -10) + (float)dpad * ldexpf(1.f, -22));
-    const float c2 = (float)(dpad + 16) * ldexpf(1.f, -24);
-
-    CUtensorMap mapY = makeTileMap(Y16, n, dpad, sp.boxRows, sp.ksplit);
-
-    // first round: ~40 k rows (16 tiles at k = 100).  Every score of round 0 becomes a candidate, so a
-    // fixed 16 tiles would make small-k searches (k-means assignment: k = 1, millions of queries) pay 4096
-    // candidates per query for nothing.
-    int r0Tiles = std::max(std::max(1, (40 * k + kTileN - 1) / kTileN), (k + 127) / 128 * 2);
-    if (nShards > 1) // pooled evidence: nShards * r0Tiles tiles; a shard must still be able to vouch for kFrac rows
-        r0Tiles = std::max<int>((r0Tiles + nShards - 1) / nShards, std::max(2, (2 * kFrac + kTileN - 1) / kTileN));
-    // threshold selection by bisection (no sorted lists) holds kSelCap entries per query and round: the all-pass first
-    // round is sized to 3/4 of that
-    const bool useBisect = LIST <= 256;
-    if (useBisect)
-        r0Tiles = std::min(r0Tiles, std::max(2, kSelCap * 3 / 4 / kTileN));
-    // queries per pass: bounds the candidate arena, whose largest user is the all-pass round 0
-    // (2 KB per query and tile) -- 16384 queries at k = 100, up to 131072 for small k
-    // k = 1 (k-means assignment, the coarse quantiser of an add): streaming mode -- one pass over all tiles with
-    // self-tightening per-thread thresholds (flat_tc_kernel SELF) and a fused select + exact re-rank
-    // (tc_argmin_finish_kernel); no rounds, no all-pass first round, no per-query sorted lists.
-    const bool streaming = k == 1 && !shard;
-    // streaming: a batch is a whole number of waves of the persistent grid (one 128-query unit per CTA and wave)
-    // (large k: the all-pass round covers 40 k rows, so the floor drops to keep the arena near 1 GiB)
-    const int64_t kQFloor = r0Tiles > 64 ? 2048 : 16384;
-    const int64_t kQBatch = streaming ? (int64_t)sms * kUnitM * 4
-                                      : std::min<int64_t>(131072, std::max<int64_t>(kQFloor, (int64_t)262144 / r0Tiles));
-    for (int64_t qb = 0; qb < nqAll; qb += kQBatch) {
-        const int64_t nq = std::min(kQBatch, nqAll - qb);
-        const float* Qb = Q + qb * d;
-        const int64_t qPairs = ceil_div(nq, kUnitM);
-
-        auto q16 = res->temp(device, sizeof(__half) * qPairs * kUnitM * dpad);
-        auto scal = res->temp(device, sizeof(float) * 4); // [absmax, qScale, inv, -]
-        auto eps = res->temp(device, sizeof(float) * nq);
-        auto thr = res->temp(device, sizeof(float) * nq);
-        auto flags = res->temp(device, sizeof(int) * (nq + 1));
-        auto baseKey = res->temp(device, streaming ? sizeof(float) : sizeof(float) * nq * LIST);
-        auto baseId = res->temp(device, streaming ? sizeof(int) : sizeof(int) * nq * LIST);
-
-        CUDA_VERIFY(cudaMemsetAsync(scal.data, 0, sizeof(float) * 4, stream));
-        CUDA_VERIFY(cudaMemsetAsync(flags.data, 0, sizeof(int) * (nq + 1), stream));
-        CUDA_VERIFY(cudaMemsetAsync(q16.data, 0, sizeof(__half) * qPairs * kUnitM * dpad, stream));
-        float* sc = scal.as<float>();
-        runAbsMax(Qb, nq * d, sc + 0, stream);
-        tc_query_scale_kernel<<<1, 1, 0, stream>>>(sc + 0, yScale, sc + 1, sc + 2);
-        CUDA_CHECK_LAST();
-        tc_prepare_queries_kernel<<<(unsigned)ceil_div(nq, 8), 256, 0, stream>>>(
-                Qb, nq, d, dpad, sc + 1, c1, c2, yMaxNorm, q16.as<__half>(), eps.as<float>(), thr.as<float>());
-        CUDA_CHECK_LAST();
-        if (!streaming) {
-            int64_t cnt = nq * LIST;
-            tc_init_base_kernel<<<(unsigned)ceil_div(cnt, 256), 256, 0, stream>>>(
-                    baseKey.as<float>(), baseId.as<int>(), cnt);
-            CUDA_CHECK_LAST();
-        }
-
-        // ---- geometric rounds over the permuted tile order
-        struct Round {
-            int begin, end, slices, tilesPerSlice, cap;
-        };
-        const int parts = kParts;
-        std::vector<Round> rounds;
-        {
-            const double g = nShards > 1 ? std::max(4.0, std::min(8.0, 2.0 * nShards)) : 4.0; // growth per round
-            int64_t seen = 0;
-            while (seen < Tsched) {
-                int64_t end = seen == 0 ? std::min<int64_t>(Tsched, r0Tiles)
-                                        : std::min<int64_t>(Tsched, (int64_t)(seen * g));
-                if (Tsched - end < end / 4)
-                    end = Tsched; // do not leave a sliver for an extra round
-                if (streaming)
-                    end = Tsched; // k = 1: ONE pass, thresholds tighten themselves inside the kernel
-                int64_t tiles = end - seen;
-                // choose the slice count minimising (waves x tiles per slice)
-                int bestS = 1;
-                double bestCost = 1e300;
-                int64_t maxS = std::max<int64_t>(1, std::min<int64_t>(512, tiles / 8));
-                for (int64_t S = 1; S <= maxS; S++) {
-                    int64_t tps = ceil_div(tiles, S);
-                    int64_t units = qPairs * ceil_div(tiles, tps);
-                    int64_t waves = ceil_div(units, sms);
-                    double cost = (double)waves * (double)(tps + 6); // +6: per-unit fixed overhead
-                    if (cost < bestCost * 0.999) {
-                        bestCost = cost;
-                        bestS = (int)S;
-                    }
-                }
-                int64_t tps = ceil_div(tiles, bestS);
-                int S = (int)ceil_div(tiles, tps);
-                int cap;
-                if (streaming) {
-                    // a thread emits ~ln(columns it sees) running maxima plus the near-ties of the maximum
-                    cap = 64;
-                } else if (seen == 0) {
-                    cap = (int)(tps * (kTileN / parts)); // everything passes in round 0
-                } else {
-                    double expect = 1.5 * k * ((double)tps / (double)seen) / parts;
-                    cap = next_pow2((int)std::min<double>(1 << 20, 4.0 * expect + 32.0));
-                    cap = std::max(cap, 32);
-                }
-                rounds.push_back({(int)seen, (int)end, S, (int)tps, cap});
-                seen = end;
-            }
-        }
-        size_t arenaBytes = 0, countBytes = 0;
-        for (auto& r : rounds) {
-            size_t units = (size_t)qPairs * r.slices;
-            arenaBytes = std::max(arenaBytes, units * kSegsPerUnit * (size_t)r.cap * sizeof(uint2));
-            countBytes = std::max(countBytes, units * kSegsPerUnit * sizeof(int));
-        }
-        auto arena = res->temp(device, arenaBytes);
-        auto counts = res->temp(device, countBytes);
-
-        const int selWarps = (int)std::max<size_t>(1, std::min<size_t>(8, (48 * 1024) / SmemTopK<int>::bytes(LIST, kSelectBuf)));
-        const size_t selSmem = SmemTopK<int>::bytes(LIST, kSelectBuf) * selWarps;
-        CUDA_VERIFY(cudaFuncSetAttribute(tc_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)selSmem));
-
-        GpuMemoryReservation contrib;
-        if (shard)
-            contrib = res->temp(device, sizeof(float) * 2 * nq);
-        for (auto& r : rounds) {
-            TcParams p{};
-            p.slices = r.slices;
-            p.qPairs = (int)qPairs;
-            p.numUnits = (int)(qPairs * r.slices);
-            CUtensorMap mapQ = makeTileMap(q16.as<__half>(), qPairs * kUnitM, dpad, kTileM);
-            p.tileBegin = (int)std::min<int64_t>(r.begin, T); // schedule laid out over the largest shard: clamp to ours
-            p.tileEnd = (int)std::min<int64_t>(r.end, T);
-            p.tilesPerSlice = r.tilesPerSlice;
-            p.permA = A;
-            p.permB = B;
-            p.numTiles = (unsigned long long)T;
-            p.KB = KB;
-            p.ksplit = sp.ksplit;
-            p.kSteps = kSteps;
-            p.yStages = sp.yStages;
-            p.invScalePtr = sc + 2;
-            p.bias = bias;
-            p.tileMaxBias = tileMaxBias;
-            p.tileMinBias = tileMaxBias + T + 1; // second half of the array (see tc_tile_max_bias_kernel)
-            p.thr = thr.as<float>();
-            p.eps = eps.as<float>();
-            p.cand = arena.as<uint2>();
-            p.cap = r.cap;
-            p.candCount = counts.as<int>();
-            p.dump = nullptr;
-            p.dumpLd = 0;
-            p.nq = (int)nq;
-            if (p.tileBegin < p.tileEnd) {
-                launchTc<false>(mapQ, mapY, p, std::min(p.numUnits, sms), sp, stream, streaming);
-            } else { // this shard has no tiles in this round of the common schedule: no candidates
-                CUDA_VERIFY(cudaMemsetAsync(counts.data, 0, (size_t)p.numUnits * kSegsPerUnit * sizeof(int), stream));
-            }
-            if (streaming) { // select + exact re-rank fused: one warp per query
-                const int fw = 8;
-                float* oD1 = outD + qb;
-                idx_t* oI1 = outI + qb;
-                KernelTiming::begin("tc_argmin_finish", stream);
-                auto launchFin = [&](auto kern) {
-                    kern<<<(unsigned)ceil_div(nq, fw), fw * 32, 0, stream>>>(
-                            (int)nq, d, r.slices, parts, arena.as<uint2>(), r.cap, counts.as<int>(), eps.as<float>(), Qb, Y, perm,
-                            oD1, oI1, flags.as<int>());
-                };
-                if (metric == METRIC_L2)
-                    yHalf ? launchFin(tc_argmin_finish_kernel<true, true>) : launchFin(tc_argmin_finish_kernel<true, false>);
-                else
-                    yHalf ? launchFin(tc_argmin_finish_kernel<false, true>) : launchFin(tc_argmin_finish_kernel<false, false>);
-                KernelTiming::end("tc_argmin_finish", stream);
-                CUDA_CHECK_LAST();
-                continue;
-            }
-            KernelTiming::begin("tc_select", stream);
-            if (useBisect) {
-                const size_t bsmem = sizeof(uint2) * kSelCap * kSelWarps;
-                CUDA_VERIFY(cudaFuncSetAttribute(tc_select_bisect_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bsmem));
-                tc_select_bisect_kernel<<<(unsigned)ceil_div(nq, kSelWarps), kSelWarps * 32, bsmem, stream>>>(
-                        (int)nq, k, LIST, r.slices, parts, arena.as<uint2>(), r.cap, counts.as<int>(), eps.as<float>(),
-                        baseKey.as<float>(), baseId.as<int>(), thr.as<float>(), flags.as<int>(),
-                        shard ? contrib.as<float>() : nullptr, kFrac);
-            } else {
-                tc_select_kernel<<<(unsigned)ceil_div(nq, selWarps), selWarps * 32, selSmem, stream>>>(
-                        (int)nq,
-                        k,
-                        LIST,
-                        r.slices,
-                        parts,
-                        arena.as<uint2>(),
-                        r.cap,
-                        counts.as<int>(),
-                        eps.as<float>(),
-                        baseKey.as<float>(),
-                        baseId.as<int>(),
-                        thr.as<float>(),
-                        flags.as<int>(),
-                        shard ? contrib.as<float>() : nullptr,
-                        kFrac);
-            }
-            KernelTiming::end("tc_select", stream);
-            CUDA_CHECK_LAST();
-            if (shard) {
-                KernelTiming::begin("tc_pool", stream);
-                // ONE small all-reduce per round (2 floats per query): every shard then filters against a
-                // threshold certified by the pooled evidence of all shards
-                shard->comm->allReduceMax(contrib.as<float>(), (size_t)2 * nq, stream);
-                tc_pooled_thr_kernel<<<(unsigned)ceil_div(nq, 256), 256, 0, stream>>>(
-                        (int)nq, contrib.as<float>(), eps.as<float>(), thr.as<float>());
-                KernelTiming::end("tc_pool", stream);
-                CUDA_CHECK_LAST();
-            }
-        }
-
-        // ---- exact re-rank
-        if (!streaming) {
-            const int rrWarps = (int)std::max<size_t>(1, std::min<size_t>(8, (48 * 1024) / SmemTopK<int>::bytes(KL, 64)));
-            const size_t rrSmem = SmemTopK<int>::bytes(KL, 64) * rrWarps;
-            float* oD = outD + qb * k;
-            idx_t* oI = outI + qb * k;
-            auto launchRr = [&](auto kern) {
-                CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rrSmem));
-                kern<<<(unsigned)ceil_div(nq, rrWarps), rrWarps * 32, rrSmem, stream>>>(
-                        (int)nq, d, k, LIST, KL, Qb, Y, perm, baseId.as<int>(), baseKey.as<float>(),
-                        shard ? thr.as<float>() : nullptr, oD, oI);
-            };
-            KernelTiming::begin("tc_rerank", stream);
-            if (metric == METRIC_L2)
-                yHalf ? launchRr(tc_rerank_kernel<true, true>) : launchRr(tc_rerank_kernel<true, false>);
-            else
-                yHalf ? launchRr(tc_rerank_kernel<false, true>) : launchRr(tc_rerank_kernel<false, false>);
-            KernelTiming::end("tc_rerank", stream);
-            CUDA_CHECK_LAST();
-        }
-
-        // ---- certificate failures -> exact SIMT recompute
-        {
-            auto list = res->temp(device, sizeof(int) * nq);
-            int* countDev = flags.as<int>() + nq;
-            tc_collect_flags_kernel<<<(unsigned)ceil_div(nq, 256), 256, 0, stream>>>(
-                    flags.as<int>(), (int)nq, list.as<int>(), countDev);
-            CUDA_CHECK_LAST();
-            int nflag = 0;
-            CUDA_VERIFY(cudaMemcpyAsync(&nflag, countDev, sizeof(int), cudaMemcpyDeviceToHost, stream));
-            CUDA_VERIFY(cudaStreamSynchronize(stream));
-            if (nflag > 0) {
-                auto fq = res->temp(device, sizeof(float) * (size_t)nflag * d);
-                auto fD = res->temp(device, sizeof(float) * (size_t)nflag * k);
-                auto fI = res->temp(device, sizeof(idx_t) * (size_t)nflag * k);
-                tc_gather_queries_kernel<<<nflag, 128, 0, stream>>>(Qb, list.as<int>(), d, fq.as<float>());
-                CUDA_CHECK_LAST();
-                runFlatExact(
-                        res, device, fq.as<float>(), nflag, Y, n, d, k, metric, 0, fD.as<float>(), fI.as<idx_t>(), stream,
-                        yHalf, 0.f, rowMask);
-                tc_scatter_results_kernel<<<nflag, 128, 0, stream>>>(
-                        fD.as<float>(), fI.as<idx_t>(), list.as<int>(), k, outD + qb * k, outI + qb * k);
-                CUDA_CHECK_LAST();
-                CUDA_VERIFY(cudaStreamSynchronize(stream));
-            }
-            lastFlatTcFallbacks() = nflag;
-        }
-    }
-}
-
-int& lastFlatTcFallbacks() {
-    static thread_local int v = 0;
-    return v;
 }
 
 } // namespace fb200

@@ -22,23 +22,20 @@
 
 #include <cuda_fp16.h>
 
+#include "flat_tc_schedule.h" // kUnitM, kTileN, kParts, kSegsPerUnit
 #include "select.cuh"
 #include "tc_ptx.cuh"
 
 namespace fb200 {
 namespace tc {
 
-constexpr int kTileM = 128;       // queries per work unit (the query tile)
-constexpr int kUnitM = kTileM;
+constexpr int kTileM = kUnitM;    // queries per work unit (the query tile)
 constexpr int kWgM = 64;          // query rows per consumer warpgroup (wgmma M)
-constexpr int kTileN = 256;       // database rows per tile (wgmma N)
 constexpr int kHalfN = kTileN / 2; // PIPE: database rows per ring stage and per MMA chain
 constexpr int kKBlock = 64;       // fp16 elements per 128-byte swizzle row
-constexpr int kParts = 4;         // column parts of a tile per query row (lanes of a quad)
 constexpr int kConsumerWarps = 8; // two warpgroups
 constexpr int kTcThreads = 32 * kConsumerWarps + 32;
 constexpr int kMaxYStages = 6;
-constexpr int kSegsPerUnit = kUnitM * kParts;
 
 struct TcParams {
     int numUnits;

@@ -245,21 +245,6 @@ struct MaskBit {
     }
 };
 
-__global__ void mask_bias_kernel(
-        const float* __restrict__ bias, const int* __restrict__ perm, const uint32_t* __restrict__ mask, int64_t n,
-        int64_t padRows, float* __restrict__ out) {
-    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= padRows)
-        return;
-    float b = -CUDART_INF_F;
-    if (p < n) {
-        const int64_t r = perm ? perm[p] : p;
-        if ((mask[r >> 5] >> (r & 31)) & 1u)
-            b = bias[p];
-    }
-    out[p] = b;
-}
-
 __global__ void remap_labels_kernel(idx_t* labels, int64_t count, const idx_t* __restrict__ ids) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < count && labels[i] >= 0)
@@ -338,11 +323,6 @@ void runRemapLabels(idx_t* labels, int64_t count, const idx_t* ids, cudaStream_t
     if (count == 0)
         return;
     remap_labels_kernel<<<(unsigned)ceil_div(count, (int64_t)256), 256, 0, stream>>>(labels, count, ids);
-    CUDA_CHECK_LAST();
-}
-
-void runMaskBias(const float* bias, const int* perm, const uint32_t* maskDev, int64_t n, int64_t padRows, float* biasOut, cudaStream_t stream) {
-    mask_bias_kernel<<<(unsigned)ceil_div(padRows, (int64_t)256), 256, 0, stream>>>(bias, perm, maskDev, n, padRows, biasOut);
     CUDA_CHECK_LAST();
 }
 

@@ -75,8 +75,4 @@ int64_t runCompactMask(GpuResources* res, int device, const uint32_t* maskDev, i
 // labels of a search over the compacted rows -> row ids (ids[label], -1 stays -1), in place
 void runRemapLabels(idx_t* labels, int64_t count, const idx_t* ids, cudaStream_t stream);
 
-// bias copy with -inf at rows whose mask bit is clear: biasOut[p] = mask[perm[p]] ? bias[p] : -inf for p < n
-// (perm null: identity), -inf for n <= p < padRows
-void runMaskBias(const float* bias, const int* perm, const uint32_t* maskDev, int64_t n, int64_t padRows, float* biasOut, cudaStream_t stream);
-
 } // namespace fb200

@@ -107,11 +107,6 @@ __global__ void half_to_float_kernel(const __half* __restrict__ x, float* __rest
         out[i] = __half2float(x[i]);
 }
 
-__global__ void fill_float_kernel(float* out, int64_t n, float v) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n)
-        out[i] = v;
-}
 __global__ void slice_cols_kernel(const float* x, int64_t n, int d, int c0, int dsub, float* out) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n * dsub) {
@@ -459,12 +454,8 @@ GpuIndexFlat::GpuIndexFlat(
           flatConfig_(config),
           vecs_(resources_.get(), config.device, AllocType::FlatData),
           vecs16_(resources_.get(), config.device, AllocType::FlatData),
-          y16_(resources_.get(), config.device, AllocType::FlatData),
-          bias_(resources_.get(), config.device, AllocType::FlatData),
-          perm_(resources_.get(), config.device, AllocType::FlatData),
-          tileMaxBias_(resources_.get(), config.device, AllocType::FlatData) {
+          tc_(resources_.get(), config.device, dims) {
     this->is_trained = true;
-    dpad_ = (int)round_up(dims, 64);
 }
 
 GpuIndexFlat::~GpuIndexFlat() {}
@@ -473,11 +464,7 @@ void GpuIndexFlat::reset() {
     DeviceScope scope(config_.device);
     vecs_.clear();
     vecs16_.clear();
-    y16_.clear();
-    bias_.clear();
-    perm_.clear();
-    tileMaxBias_.clear();
-    tcDirty_ = true;
+    tc_.clear();
     this->ntotal = 0;
 }
 
@@ -517,7 +504,7 @@ void GpuIndexFlat::addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) {
         vecs_.append(xDev, (size_t)n * d, stream);
     }
     this->ntotal += n;
-    tcDirty_ = true;
+    tc_.invalidate();
 }
 
 const float* GpuIndexFlat::roundedQueries_(idx_t n, const float* xDev, GpuMemoryReservation& hold) const {
@@ -546,48 +533,7 @@ void GpuIndexFlat::replaceVectorsDevice(idx_t n, const float* xDev) {
     if (n > 0)
         CUDA_VERIFY(cudaMemcpyAsync(vecs_.data(), xDev, sizeof(float) * n * d, cudaMemcpyDeviceToDevice, stream));
     this->ntotal = n;
-    tcDirty_ = true;
-}
-
-void GpuIndexFlat::prepareTensorCoreData_() const {
-    if (!tcDirty_)
-        return;
-    auto stream = stream_();
-    const idx_t n = this->ntotal;
-    const int64_t padRows = round_up(n, 256) + 256; // whole 256-row tiles, -inf beyond n
-    y16_.resize((size_t)n * dpad_, stream);
-    bias_.resize((size_t)padRows, stream);
-    tileMaxBias_.resize((size_t)(padRows / 256) * 2, stream); // [T+1] max bias per tile, then [T+1] min bias per tile
-    const MetricType metric = searchMetric_();
-    const bool sorted = metric == METRIC_L2; // IP has no bias: row order is kept
-    if (sorted)
-        perm_.resize((size_t)n, stream);
-    else
-        perm_.clear();
-    auto scal = resources_->temp(config_.device, sizeof(float) * 2);
-    auto norms = resources_->temp(config_.device, sizeof(float) * n);
-    CUDA_VERIFY(cudaMemsetAsync(scal.data, 0, sizeof(float) * 2, stream));
-    runAbsMax(rows_(), n * (int64_t)d, scal.as<float>(), stream, yHalf_());
-    float h[2] = {0.f, 0.f};
-    CUDA_VERIFY(cudaMemcpyAsync(h, scal.data, sizeof(float), cudaMemcpyDeviceToHost, stream));
-    CUDA_VERIFY(cudaStreamSynchronize(stream));
-    float scale = 1.f;
-    if (h[0] > 0.f) {
-        int e;
-        std::frexp(h[0], &e);
-        scale = std::ldexp(1.f, 14 - e); // max |y| * scale in [2^13, 2^14)
-    }
-    fill_float_kernel<<<(unsigned)ceil_div(padRows, 256), 256, 0, stream>>>(bias_.data(), padRows, -INFINITY);
-    CUDA_CHECK_LAST();
-    runFlatTcPrepareRows(
-            resources_.get(), config_.device, rows_(), n, d, dpad_, scale, metric, y16_.data(), bias_.data(),
-            sorted ? perm_.data() : nullptr, tileMaxBias_.data(), norms.as<float>(), stream, yHalf_());
-    runMaxOf(norms.as<float>(), n, scal.as<float>() + 1, stream);
-    CUDA_VERIFY(cudaMemcpyAsync(h, scal.data, sizeof(float) * 2, cudaMemcpyDeviceToHost, stream));
-    CUDA_VERIFY(cudaStreamSynchronize(stream));
-    yScale_ = scale;
-    yMaxNorm_ = std::sqrt(h[1]) * 1.0001f;
-    tcDirty_ = false;
+    tc_.invalidate();
 }
 
 // faiss/gpu/impl/Distance.cuh:223-239.  The reference GPU's p = -1 -> L2 branch is a test hook; the CPU sums
@@ -636,18 +582,20 @@ void GpuIndexFlat::searchCompacted_(idx_t n, const float* xDev, int k, float* dD
     runRemapLabels(iDev, n * k, rows.as<idx_t>(), stream);
 }
 
+void GpuIndexFlat::search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels) const {
+    lastSearchFallbackQueries = 0; // summed over the query pages
+    GpuIndex::search(n, x, k, distances, labels);
+}
+
 void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
     auto stream = stream_();
     lastSearchUsedTensorCores = 0;
-    lastSearchFallbackQueries = 0;
-    const MetricType metric = searchMetric_();
     if (this->ntotal == 0) {
         fillEmpty_(n, k, dDev, iDev);
         return;
     }
-    // the tensor-core path pays a fixed cost per query tile of 128; tiny batches stay exact.  Metrics without a
-    // product form (L1, Linf, Lp, Canberra, ...) always run the exact kernel.
-    const bool tc = flatConfig_.useTensorCores && tensorCoreMetric_() && flatTcSupported(d, k, this->ntotal) && n >= 16;
+    // metrics without a product form (L1, Linf, Lp, Canberra, ...) always run the exact kernel
+    const bool tc = useTensorCores_(k, n);
     GpuMemoryReservation qHold;
     xDev = roundedQueries_(n, xDev, qHold);
     const uint32_t* mask = callMask_;
@@ -663,58 +611,34 @@ void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, i
         }
     }
     if (tc) {
-        prepareTensorCoreData_();
-        const float* bias = bias_.data();
-        const float* tileBias = tileMaxBias_.data();
-        GpuMemoryReservation maskedBias, maskedTileBias;
-        if (mask) {
-            // an excluded row gets a -inf bias: its score can then never pass a round's threshold, exactly as the
-            // padding rows past ntotal.  yMaxNorm_ over all rows stays a valid bound for the certificate.
-            maskedBias = resources_->temp(config_.device, sizeof(float) * bias_.size());
-            maskedTileBias = resources_->temp(config_.device, sizeof(float) * tileMaxBias_.size());
-            runMaskBias(
-                    bias_.data(), metric == METRIC_L2 ? perm_.data() : nullptr, mask, this->ntotal, (int64_t)bias_.size(),
-                    maskedBias.as<float>(), stream);
-            runFlatTcTileBias(maskedBias.as<float>(), this->ntotal, maskedTileBias.as<float>(), stream);
-            bias = maskedBias.as<float>();
-            tileBias = maskedTileBias.as<float>();
-        }
-        runFlatTcSearch(
-                resources_.get(), config_.device, xDev, n, rows_(), y16_.data(), bias,
-                metric == METRIC_L2 ? perm_.data() : nullptr, tileBias, yScale_,
-                yMaxNorm_, this->ntotal, d, dpad_, k, metric, dDev, iDev, stream, nullptr, yHalf_(), mask);
+        tc_.prepare(rows_(), this->ntotal, searchMetric_(), yHalf_(), stream);
+        lastSearchFallbackQueries += (int)tc_.search(xDev, n, k, dDev, iDev, stream, nullptr, mask);
         lastSearchUsedTensorCores = 1;
-        lastSearchFallbackQueries = lastFlatTcFallbacks();
     } else {
         runFlatExact(
-                resources_.get(), config_.device, xDev, n, rows_(), this->ntotal, d, k, metric, 0, dDev, iDev,
+                resources_.get(), config_.device, xDev, n, rows_(), this->ntotal, d, k, searchMetric_(), 0, dDev, iDev,
                 stream, yHalf_(), metric_arg, mask);
     }
 }
 
 bool GpuIndexFlat::shardPoolingEligible(int k, idx_t n) const {
     // pooled thresholds are a tensor-core certificate: other metrics take the plain all-gather + merge path
-    return flatConfig_.useTensorCores && tensorCoreMetric_() && this->ntotal > 0 && flatTcSupported(d, k, this->ntotal) &&
-            n >= 16;
+    return useTensorCores_(k, n);
 }
 
 void GpuIndexFlat::searchShardDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* flatShard) const {
+    lastSearchFallbackQueries = 0;
     if (!flatShard) {
         searchImpl_(n, xDev, k, dDev, iDev);
         return;
     }
     FB_THROW_IF_NOT_MSG(shardPoolingEligible(k, n), "pooled sharded search requested on a shard that cannot take the tensor-core path");
     auto stream = stream_();
-    prepareTensorCoreData_();
+    tc_.prepare(rows_(), this->ntotal, searchMetric_(), yHalf_(), stream);
     GpuMemoryReservation qHold;
     xDev = roundedQueries_(n, xDev, qHold);
-    const MetricType metric = searchMetric_();
-    runFlatTcSearch(
-            resources_.get(), config_.device, xDev, n, rows_(), y16_.data(), bias_.data(),
-            metric == METRIC_L2 ? perm_.data() : nullptr, tileMaxBias_.data(), yScale_, yMaxNorm_, this->ntotal, d,
-            dpad_, k, metric, dDev, iDev, stream, flatShard, yHalf_());
+    lastSearchFallbackQueries = (int)tc_.search(xDev, n, k, dDev, iDev, stream, flatShard);
     lastSearchUsedTensorCores = 1;
-    lastSearchFallbackQueries = lastFlatTcFallbacks();
 }
 
 void GpuIndexFlat::reconstruct(idx_t key, float* out) const {

@@ -9,7 +9,7 @@
 //   faiss::gpu::GpuIndexIVFPQ         faiss/gpu/GpuIndexIVFPQ.h:25-181, GpuIndexIVFPQ.cu:29-622
 //   faiss::Clustering                 faiss/Clustering.h:22-229, Clustering.cpp:60-380
 //   faiss::IndexShards                faiss/IndexShards.h:21-106, IndexShards.cpp:87-264
-// Everything device-side goes through kernels.h.
+// Everything device-side goes through kernels.h and flat_tc.h.
 #pragma once
 
 #include <memory>
@@ -17,81 +17,12 @@
 #include <vector>
 
 #include "common.h"
+#include "flat_tc.h"
 #include "idselector.h"
 #include "kernels.h"
 #include "resources.h"
 
 namespace fb200 {
-
-// ------------------------------------------------------------------------------------------
-// growable device array backed by GpuResources (role of DeviceVector, faiss/gpu/utils/DeviceVector.cuh)
-// ------------------------------------------------------------------------------------------
-template <typename T>
-class DeviceVector {
-   public:
-    DeviceVector(GpuResources* res, int device, AllocType type) : res_(res), device_(device), type_(type) {}
-    ~DeviceVector() {
-        clear();
-    }
-    DeviceVector(const DeviceVector&) = delete;
-    DeviceVector& operator=(const DeviceVector&) = delete;
-
-    T* data() const {
-        return data_;
-    }
-    size_t size() const {
-        return size_;
-    }
-    size_t capacity() const {
-        return cap_;
-    }
-    void clear() {
-        if (data_)
-            res_->deallocMemory(device_, data_);
-        data_ = nullptr;
-        size_ = cap_ = 0;
-    }
-    // ensure capacity >= n (exact if `exact`, else geometric growth), preserving contents
-    void reserve(size_t n, cudaStream_t stream, bool exact = false) {
-        if (n <= cap_)
-            return;
-        size_t ncap = exact ? n : std::max(n, cap_ + cap_ / 2);
-        AllocRequest r;
-        r.type = type_;
-        r.device = device_;
-        r.space = MemorySpace::Device;
-        r.stream = stream;
-        r.size = ncap * sizeof(T);
-        T* nd = (T*)res_->allocMemory(r);
-        if (size_ > 0) {
-            CUDA_VERIFY(cudaMemcpyAsync(nd, data_, size_ * sizeof(T), cudaMemcpyDeviceToDevice, stream));
-            CUDA_VERIFY(cudaStreamSynchronize(stream));
-        }
-        if (data_)
-            res_->deallocMemory(device_, data_);
-        data_ = nd;
-        cap_ = ncap;
-    }
-    void resize(size_t n, cudaStream_t stream) {
-        reserve(n, stream);
-        size_ = n;
-    }
-    // append n elements from a host or device pointer
-    void append(const T* src, size_t n, cudaStream_t stream) {
-        if (n == 0)
-            return;
-        reserve(size_ + n, stream);
-        CUDA_VERIFY(cudaMemcpyAsync(data_ + size_, src, n * sizeof(T), cudaMemcpyDefault, stream));
-        size_ += n;
-    }
-
-   private:
-    GpuResources* res_;
-    int device_;
-    AllocType type_;
-    T* data_ = nullptr;
-    size_t size_ = 0, cap_ = 0;
-};
 
 // ------------------------------------------------------------------------------------------
 // faiss::Index
@@ -253,9 +184,12 @@ class GpuIndexFlat : public GpuIndex {
     void reconstruct_batch(idx_t n, const idx_t* keys, float* out) const override;
     void compute_residual(const float* x, float* residual, idx_t key) const override;
     void compute_residual_n(idx_t n, const float* xs, float* residuals, const idx_t* keys) const override;
+    using GpuIndex::search;
+    void search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels) const override;
 
     // device-pointer entry points used by IVF / clustering (role of FlatIndex::query)
     void searchDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
+        lastSearchFallbackQueries = 0;
         searchImpl_(n, xDev, k, dDev, iDev);
     }
     void searchShardDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* flatShard) const override;
@@ -273,7 +207,7 @@ class GpuIndexFlat : public GpuIndex {
     // replace the whole content by n device rows without giving the storage back (the k-means loop installs a new
     // centroid table every iteration: reset() + add() would free and re-allocate five buffers each time)
     void replaceVectorsDevice(idx_t n, const float* xDev);
-    // diagnostics
+    // diagnostics of the last search (fallback queries: exact recomputes, summed over the whole call)
     mutable int lastSearchUsedTensorCores = 0;
     mutable int lastSearchFallbackQueries = 0;
 
@@ -287,13 +221,16 @@ class GpuIndexFlat : public GpuIndex {
     // the selected rows only: gathered (fp32) and searched with the exact kernel, labels mapped back
     void searchCompacted_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, idx_t selected) const;
     void fillEmpty_(idx_t n, int k, float* dDev, idx_t* iDev) const;
-    void prepareTensorCoreData_() const;
     // the metric the kernels run, read at search time: METRIC_Lp with metric_arg 1 is L1 and with 2 is L2
     // (faiss/gpu/impl/Distance.cuh:223-239); only L2 and inner product can take the tensor-core path
     MetricType searchMetric_() const;
     bool tensorCoreMetric_() const {
         const MetricType m = searchMetric_();
         return m == METRIC_L2 || m == METRIC_INNER_PRODUCT;
+    }
+    // does a search of n queries for k results take the tensor cores?  (tiny batches stay exact)
+    bool useTensorCores_(int k, idx_t n) const {
+        return flatConfig_.useTensorCores && tensorCoreMetric_() && flatTcSupported(d, k, this->ntotal) && n >= 16;
     }
 
     const void* rows_() const { // the stored rows, as the kernels take them (with yHalf_())
@@ -310,15 +247,7 @@ class GpuIndexFlat : public GpuIndex {
     mutable idx_t callSelected_ = 0; // rows selected by callMask_ (counted once per call, in selMask_)
     DeviceVector<float> vecs_;    // fp32 storage (default)
     DeviceVector<__half> vecs16_; // fp16 storage (useFloat16): the only copy of the vectors besides the scoring tiles
-    // tensor-core side data, rebuilt lazily after adds
-    mutable DeviceVector<__half> y16_;
-    mutable DeviceVector<float> bias_;
-    mutable DeviceVector<int> perm_;          // L2: stored (norm-sorted) position -> row id
-    mutable DeviceVector<float> tileMaxBias_; // max bias per 256-row tile
-    mutable bool tcDirty_ = true;
-    mutable float yScale_ = 1.f;
-    mutable float yMaxNorm_ = 0.f;
-    mutable int dpad_ = 0;
+    mutable FlatTcDatabase tc_; // rebuilt lazily after the rows change
 };
 
 class GpuIndexFlatL2 : public GpuIndexFlat {

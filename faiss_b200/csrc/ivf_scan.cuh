@@ -43,16 +43,7 @@ void runIvfScanBatches(
         cudaStream_t stream,
         const std::function<void(const IvfScanBatch&)>& launch);
 
-// runtime value -> compile-time constant for the scan launchers' kernel templates:
-// f(std::true_type{}) or f(std::false_type{}) ...
-template <typename F>
-void withBool(bool b, F&& f) {
-    if (b)
-        f(std::true_type{});
-    else
-        f(std::false_type{});
-}
-// ... and f(std::integral_constant<int, V>{}) for the V of Vs equal to v (v must be one of them)
+// runtime value -> compile-time constant (see withBool): f(std::integral_constant<int, V>{}) for the V of Vs equal to v
 template <int... Vs, typename F>
 void withInt(int v, F&& f) {
     const bool found = ((v == Vs ? (f(std::integral_constant<int, Vs>{}), true) : false) || ...);

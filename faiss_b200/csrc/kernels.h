@@ -1,4 +1,4 @@
-// faiss_b200 -- launcher declarations for every device kernel (L1).  Host code (index objects,
+// faiss_b200 -- launcher declarations for the device kernels (L1; the tensor-core Flat search: flat_tc.h).  Host code (index objects,
 // C ABI) only sees these; all pointers are DEVICE pointers, all work is enqueued on `stream`.
 #pragma once
 
@@ -115,88 +115,6 @@ void runCalcResidual(
         int yHalf = 0);
 // gather rows by id (reconstruct_batch) / by range
 void runGatherRows(const void* src, const idx_t* ids, int64_t n, int d, float* out, cudaStream_t stream, int yHalf = 0);
-
-// ---------------------------------------------------------------- flat_tc.cu  (tensor-core path)
-struct FlatTcPlan; // opaque: tensor maps + scratch sizing for one (index, nq, k) shape
-
-// fp32 rows -> scaled fp16 rows (padded to dpad, multiple of 64) + score bias (bias = -||y||^2/2 for
-// L2, 0 for IP) + per-256-row-tile maximum bias.  With perm != null (L2) the fp16 copy is stored in
-// order of increasing norm: perm[stored position] = row id.  norms[] stays in row order.
-void runFlatTcPrepareRows(
-        GpuResources* res,
-        int device,
-        const void* Y, // fp32 rows, or __half rows when yHalf
-        int64_t n,
-        int d,
-        int dpad,
-        float scale,
-        MetricType metric,
-        __half* Y16,
-        float* bias,
-        int* perm,
-        float* tileMaxBias,
-        float* norms,
-        cudaStream_t stream,
-        int yHalf = 0);
-
-// max |x| over a matrix (device scalar, float) -- used to pick the power-of-two fp16 scale
-void runAbsMax(const void* x, int64_t count, float* out /*device, must be zeroed*/, cudaStream_t stream, int yHalf = 0);
-// max row norm^2
-void runMaxOf(const float* x, int64_t count, float* out /*device, zeroed; x >= 0*/, cudaStream_t stream);
-
-bool flatTcSupported(int d, int k, int64_t n);
-
-// Sharded search (one shard per NCCL rank): thresholds are pooled across the ranks after every round
-// (one all-reduce of 2 floats per query), so a 1/S-size shard filters as tightly as the whole database would
-// and keeps only its share of the global top-k; all ranks must call with the same queries and k.
-class Communicator;
-struct FlatTcShard {
-    const Communicator* comm; // this rank
-    int64_t maxTiles;         // max over ranks of ceil(n_r / 256): the common round schedule
-};
-
-// Full certified search: fp16 wgmma scoring + candidate emission + exact fp32 re-rank, with the
-// exact SIMT kernel as fallback for queries whose certificate fails.  See flat_tc.cu.
-void runFlatTcSearch(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nq,
-        const void* Y,       // stored rows [n,d] (exact re-rank): fp32, or __half when yHalf
-        const __half* Y16,   // fp16 scaled rows [n,dpad], stored order
-        const float* bias,   // [n] stored order
-        const int* perm,     // stored position -> row id (null: identity)
-        const float* tileMaxBias, // [ceil(n/256)]
-        float yScale,        // power of two applied to Y16
-        float yMaxNorm,      // max ||y|| (unscaled)
-        int64_t n,
-        int d,
-        int dpad,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const FlatTcShard* shard = nullptr,
-        int yHalf = 0,
-        const uint32_t* rowMask = nullptr); // passed to the exact recompute of certificate failures
-
-// per-tile max / min of a stored-order bias array [round_up(n, 256) + 256] into tileMaxBias (the layout
-// runFlatTcPrepareRows writes): recomputed after a selector's mask set excluded rows' biases to -inf
-void runFlatTcTileBias(const float* bias, int64_t n, float* tileMaxBias, cudaStream_t stream);
-
-// number of queries the last runFlatTcSearch on this thread recomputed with the exact kernel
-int& lastFlatTcFallbacks();
-
-// debug / unit-test seam: raw fp16 tensor-core score tile  S[nq,n] = Q16 . Y16^T  (fp32 out)
-void runFlatTcScoresDebug(
-        const __half* Q16,
-        int64_t nq,
-        const __half* Y16,
-        int64_t n,
-        int dpad,
-        float* S,
-        cudaStream_t stream);
 
 // ---------------------------------------------------------------- kmeans.cu
 // centroid update (role of compute_centroids, faiss/impl/ClusteringHelpers.cpp:101-172):

@@ -8,6 +8,7 @@
 // (getMemoryInfo).  No cuBLAS handle is created: nothing on the hot path calls a library.
 #pragma once
 
+#include <algorithm>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -233,5 +234,75 @@ struct DeviceScope {
 
 // -1 if host pointer, else device ordinal (faiss/gpu/utils/DeviceUtils.h:64)
 int getDeviceForAddress(const void* p);
+
+// ------------------------------------------------------------------------------------------
+// growable device array backed by GpuResources (role of DeviceVector, faiss/gpu/utils/DeviceVector.cuh)
+// ------------------------------------------------------------------------------------------
+template <typename T>
+class DeviceVector {
+   public:
+    DeviceVector(GpuResources* res, int device, AllocType type) : res_(res), device_(device), type_(type) {}
+    ~DeviceVector() {
+        clear();
+    }
+    DeviceVector(const DeviceVector&) = delete;
+    DeviceVector& operator=(const DeviceVector&) = delete;
+
+    T* data() const {
+        return data_;
+    }
+    size_t size() const {
+        return size_;
+    }
+    size_t capacity() const {
+        return cap_;
+    }
+    void clear() {
+        if (data_)
+            res_->deallocMemory(device_, data_);
+        data_ = nullptr;
+        size_ = cap_ = 0;
+    }
+    // ensure capacity >= n (exact if `exact`, else geometric growth), preserving contents
+    void reserve(size_t n, cudaStream_t stream, bool exact = false) {
+        if (n <= cap_)
+            return;
+        size_t ncap = exact ? n : std::max(n, cap_ + cap_ / 2);
+        AllocRequest r;
+        r.type = type_;
+        r.device = device_;
+        r.space = MemorySpace::Device;
+        r.stream = stream;
+        r.size = ncap * sizeof(T);
+        T* nd = (T*)res_->allocMemory(r);
+        if (size_ > 0) {
+            CUDA_VERIFY(cudaMemcpyAsync(nd, data_, size_ * sizeof(T), cudaMemcpyDeviceToDevice, stream));
+            CUDA_VERIFY(cudaStreamSynchronize(stream));
+        }
+        if (data_)
+            res_->deallocMemory(device_, data_);
+        data_ = nd;
+        cap_ = ncap;
+    }
+    void resize(size_t n, cudaStream_t stream) {
+        reserve(n, stream);
+        size_ = n;
+    }
+    // append n elements from a host or device pointer
+    void append(const T* src, size_t n, cudaStream_t stream) {
+        if (n == 0)
+            return;
+        reserve(size_ + n, stream);
+        CUDA_VERIFY(cudaMemcpyAsync(data_ + size_, src, n * sizeof(T), cudaMemcpyDefault, stream));
+        size_ += n;
+    }
+
+   private:
+    GpuResources* res_;
+    int device_;
+    AllocType type_;
+    T* data_ = nullptr;
+    size_t size_ = 0, cap_ = 0;
+};
 
 } // namespace fb200

@@ -9,7 +9,7 @@ import pytest
 
 
 def _pow2_scale(m):
-    # max|x| * s in [2^13, 2^14)   (tc_query_scale_kernel / prepareTensorCoreData_)
+    # max|x| * s in [2^13, 2^14)   (tc_query_scale_kernel / FlatTcDatabase::prepare)
     if m <= 0:
         return 1.0
     e = np.frexp(np.float32(m))[1]

@@ -139,6 +139,40 @@ def test_tensor_core_adversarial_order_falls_back_correctly(res):
     assert torch.equal(I, Ie) and torch.equal(D, De)
 
 
+def test_fallback_count_covers_every_query_batch(res):
+    """lastSearchInfo()["fallback_queries"] counts the exact recomputes of the whole call, not of its last internal
+    query batch (2048 queries at k = 1024): the certificate-failing queries come first, fillers fill later batches"""
+    import faiss_b200 as fb
+
+    rs = np.random.RandomState(5)
+    d, k = 64, 1024
+    # near-duplicate rows (16 points, 2500 copies each, one coordinate moved by 1): their queries fail the
+    # certificate.  In the opposite orthant, rows and queries with spread-out distances: those queries pass it.
+    base = np.floor(rs.rand(16, d) * 16).astype(np.float32)
+    dup = np.repeat(base, 2500, axis=0)
+    dup[np.arange(len(dup)), rs.randint(0, d, len(dup))] += 1.0
+    far = -np.abs(rs.randn(40000, d) * 8).astype(np.float32)
+    xb = np.vstack([dup, far])
+    failing = base[rs.randint(0, 16, 64)]
+    fillers = -np.abs(rs.randn(3000, d) * 8).astype(np.float32)
+    xq = np.vstack([failing, fillers])
+    idx = fb.GpuIndexFlatL2(res, d)
+    idx.add(xb)
+
+    idx.search(fillers, k)
+    assert idx.lastSearchInfo() == {"tensor_cores": 1, "fallback_queries": 0}
+    idx.search(failing, k)
+    alone = idx.lastSearchInfo()["fallback_queries"]
+    assert alone > 0
+
+    D, I = idx.search(xq, k)
+    info = idx.lastSearchInfo()
+    assert info["tensor_cores"] == 1 and info["fallback_queries"] >= alone
+    idx.setUseTensorCores(False)
+    De, Ie = idx.search(xq, k)
+    assert np.array_equal(I, Ie) and np.array_equal(D, De)
+
+
 def test_tcgen05_raw_scores(res):
     """unit test of the MMA path alone: fp16 operands, fp32 accumulation (wgmma, register accumulators)"""
     import torch

@@ -1,4 +1,4 @@
-"""CPU model of the sharded Flat search protocol (DESIGN.md 4, `runFlatTcSearch` with a FlatTcShard):
+"""CPU model of the sharded Flat search protocol (DESIGN.md 4, `FlatTcDatabase::search` with a FlatTcShard):
 geometric rounds over each shard's rows, per-shard threshold selection on APPROXIMATE scores (|S' - S| <= eps),
 cross-shard pooling of two certified lower bounds per query after every round
     c0 = (shard's k-th best S') - eps        c1 = (shard's ceil(k/S)-th best S') - eps
