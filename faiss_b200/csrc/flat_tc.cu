@@ -11,13 +11,13 @@
 //     model (10 mantissa bits) and the fp32 accumulation.
 //   * Fused filter (flat_tc_kernel.cuh).  A persistent warp-specialised kernel: one TMA producer warp
 //     (the unit's 128-query tile once per work unit, 256-row database tiles through an mbarrier ring) and
-//     two consumer warpgroups that each run 64x256xK wgmma tiles into register accumulators and filter
-//     them in place: each thread holds two query rows and 64 of a tile's 256 columns of each, folds the
+//     two consumer warpgroups that each run 64x256xK wgmma tiles into register accumulators (at
+//     112 < d <= 128: four that each run 64x128xK, one per query half and column half) and filter
+//     them in place: each thread holds two query rows and 64 (or 32) of a tile's 256 columns of each, folds the
 //     RAW accumulators with a max tree and compares one bound per 32 of them against the query's
 //     threshold held in a register -- the fp16 copy
 //     is stored sorted by norm, so the tile's maximum bias bounds every row's bias tightly.  Scores
-//     never reach HBM; only the rare survivors are appended (plain stores, no atomics) to a
-//     thread-private candidate segment.
+//     never reach HBM; only the rare survivors are appended to a per-(query, column part) candidate segment.
 //   * Thresholds come from geometric rounds over a pseudo-randomly permuted tile order: round 0
 //     scans ~40 k rows, round r 3x the rows seen so far; after each round a small kernel folds the new candidates into
 //     a per-query sorted base list and sets threshold = (k-th best approx score) - 2*eps_q, which
@@ -818,26 +818,26 @@ struct SmemPlan {
     int yStages;
     size_t bytes;
     int ksplit; // ring stages hold single K-blocks (see flat_tc_kernel)
-    bool pipe;  // ring stages hold half tiles, for the pipelined consumer (flat_tc_kernel PIPE)
+    bool quad;  // four consumer warpgroups over half-tile ring stages (flat_tc_kernel QUAD)
     int boxRows; // database rows per TMA copy of mapY
 };
 
 constexpr int kMaxKB = 4; // d <= 256: the query tile (16 KB per K-block) + at least three 32 KB K-block stages in 227 KB
 
-// 112 < d <= 128: half-tile stages (32 KB: six of them); other d <= 128: whole-tile stages (64 KB at d = 128: three of
-// them); beyond, K-block stages (see flat_tc_kernel)
+// 112 < d <= 128: half-tile stages (32 KB: six of them, which the QUAD kernel takes as a constant); other d <= 128:
+// whole-tile stages (64 KB at d = 128: three of them); beyond, K-block stages (see flat_tc_kernel)
 SmemPlan planSmem(int KB, int kSteps) {
     FB_THROW_IF_NOT_MSG(KB <= kMaxKB, "dimension too large for the tensor-core Flat kernel");
     const int ksplit = KB > 2 ? 1 : 0;
-    const bool pipe = tc_pipelined(KB, kSteps);
-    const int boxRows = pipe ? kHalfN : kTileN;
+    const bool quad = tc_quad(KB, kSteps);
+    const int boxRows = quad ? kHalfN : kTileN;
     const size_t qtile = (size_t)KB * kTileM * kKBlock * 2;
-    const size_t fixed = 1024 /*align slack*/ + 512 /*barriers*/ + qtile;
+    const size_t fixed = 1024 /*align slack*/ + 512 /*barriers*/ + (quad ? kQuadCountBytes : 0) + qtile;
     const size_t stage = (size_t)(ksplit ? 1 : KB) * boxRows * kKBlock * 2;
-    const size_t budget = 226 * 1024; // 232448 B is the opt-in limit per CTA
+    const size_t budget = 227 * 1024; // the opt-in limit per CTA
     int ys = (int)std::min<size_t>(kMaxYStages, (budget - fixed) / stage);
-    FB_THROW_IF_NOT(ys >= 3);
-    return {ys, fixed + ys * stage, ksplit, pipe, boxRows};
+    FB_THROW_IF_NOT(ys >= 3 && (!quad || ys == kMaxYStages));
+    return {ys, fixed + ys * stage, ksplit, quad, boxRows};
 }
 
 // the kernel's parameters for one round over nq queries (the search's pointers are filled in by the caller)
@@ -853,6 +853,7 @@ TcParams roundParams(const SmemPlan& sp, int KB, int kSteps, int64_t nq, int64_t
     p.permA = permA;
     p.permB = permB;
     p.numTiles = (unsigned long long)T;
+    p.permStep = (int)(permA % (unsigned long long)T);
     p.KB = KB;
     p.ksplit = sp.ksplit;
     p.kSteps = kSteps;
@@ -866,12 +867,14 @@ TcParams roundParams(const SmemPlan& sp, int KB, int kSteps, int64_t nq, int64_t
 template <bool DUMP>
 void launchTc(const CUtensorMap& mq, const CUtensorMap& my, const TcParams& p, int grid, const SmemPlan& sp, cudaStream_t stream, bool self = false) {
     const size_t smem = sp.bytes;
-    auto kern = sp.pipe ? flat_tc_kernel<DUMP, false, true> : flat_tc_kernel<DUMP>;
+    // QUAD: a segment's count is a 16-bit shared-memory counter (flat_tc_kernel.cuh)
+    FB_THROW_IF_NOT_FMT(!sp.quad || p.cap <= kQuadMaxCap, "candidate cap %d too large for the 16-bit segment counts", p.cap);
+    auto kern = sp.quad ? flat_tc_kernel<DUMP, false, true> : flat_tc_kernel<DUMP>;
     if (self && !DUMP) // k = 1 streaming mode (self-tightening thresholds)
-        kern = sp.pipe ? flat_tc_kernel<false, true, true> : flat_tc_kernel<false, true>;
+        kern = sp.quad ? flat_tc_kernel<false, true, true> : flat_tc_kernel<false, true>;
     CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTiming::begin("flat_tc", stream);
-    kern<<<grid, kTcThreads, smem, stream>>>(mq, my, p);
+    kern<<<grid, tc_threads(sp.quad), smem, stream>>>(mq, my, p);
     KernelTiming::end("flat_tc", stream);
     CUDA_CHECK_LAST();
 }

@@ -1,23 +1,28 @@
 // faiss_b200 -- the wgmma Flat scoring + filter kernel (included by flat_tc.cu).
 //
-// Roles in one persistent CTA (2 consumer warpgroups + 1 producer warp = 288 threads, one CTA per SM):
-//   warps 0-7 : two consumer warpgroups.  A work unit is one 128-query tile; warpgroup g owns its query rows
-//               64 g .. 64 g + 63.  For every database tile it issues wgmma.m64n256k16 (fp16 operands straight
-//               from the 128B-swizzled shared-memory stages, fp32 accumulators in registers: 128 per thread),
-//               waits for them, hands the stage back and filters its own accumulator fragment (below).  At
-//               112 < d <= 128 (PIPE) a tile runs as two N = 128 chains, A (columns 0-127) and B (128-255), each
-//               reading its own half-tile stage, and the warpgroup is software-pipelined: it filters A(t) while
-//               B(t) runs and B(t) while A(t + 1) runs, so it always has MMAs of its own in flight.  Otherwise a
-//               warpgroup's own MMAs and filter do not overlap.  The two warpgroups share the ring without
-//               synchronising with each other, so one's tensor work can also overlap the other's filter.  Survivors
-//               (rare) are appended with plain stores to a thread-private candidate segment; scores never reach HBM.
-//   warp 8    : TMA producer -- the unit's query tile once, then database tiles (256 rows x dpad fp16, or PIPE: two
-//               128-row halves of one, 128B-swizzled K-major) through an mbarrier ring.
-// Nine warps put three on one scheduler, which caps a thread at 168 registers: the 128 accumulators plus the filter
-// state fit without spills.
+// Roles in one persistent CTA (one CTA per SM).  A work unit is one 128-query tile.
+//   Two-warpgroup layout (2 consumer warpgroups + 1 producer warp = 288 threads): warpgroup g owns query rows
+//               64 g .. 64 g + 63.  For every database tile it issues wgmma.m64n256k16 (fp16 operands straight from
+//               the 128B-swizzled shared-memory stages, fp32 accumulators in registers: 128 per thread), waits for
+//               them, hands the stage back and filters its own accumulator fragment (below).  Nine warps put three on
+//               one scheduler, which caps a thread at 168 registers: the 128 accumulators plus the filter state fit.
+//   QUAD layout, 112 < d <= 128 (4 consumer warpgroups + 1 producer warp = 544 threads): warpgroup (g, h) owns query
+//               rows 64 g .. 64 g + 63 and columns 128 h .. 128 h + 127 of every database tile.  Ring stages hold
+//               128-row halves of a tile; stage s holds half s % 2 and is read by the two warpgroups with h = s % 2.
+//               A warpgroup runs one wgmma.m64n128k16 chain per tile (64 accumulators per thread), waits for it,
+//               hands the stage back and filters.  While one warpgroup filters, three others have chains to run:
+//               the warp schedulers interleave tensor and filter work with no software pipelining.  Seventeen warps
+//               put five on one scheduler, which caps a thread at 96 registers: 64 accumulators plus the filter state.
+//   The consumer warpgroups share the ring without synchronising with each other.  Survivors (rare) are written to
+//   their candidate segment; scores never reach HBM.
+//   Last warp: TMA producer -- the unit's query tile once, then database tiles (256 rows x dpad fp16, QUAD: two
+//   128-row halves of one, 128B-swizzled K-major) through an mbarrier ring.
 //
-// A thread's fragment holds two query rows (r and r + 8) and, of each, the 64 columns 8 j + 2 (lane % 4) + {0, 1}:
-// the four lanes of a quad split a row's 256 columns, which is why a query row has kParts = 4 candidate segments.
+// A thread's fragment holds two query rows (r and r + 8) and, of each, the columns 8 j + 2 (lane % 4) + {0, 1} of
+// the tile: the four lanes of a quad split a row's 256 columns, which is why a query row has kParts = 4 candidate
+// segments.  In the two-warpgroup layout one thread writes a segment (plain stores, thread-private count).  In the
+// QUAD layout the segment's columns are split between warpgroups (g, 0) and (g, 1), so the two writers take slots
+// from a 16-bit shared-memory counter per segment; the candidate SET of a segment is the same, only its order is not.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -31,11 +36,21 @@ namespace tc {
 
 constexpr int kTileM = kUnitM;    // queries per work unit (the query tile)
 constexpr int kWgM = 64;          // query rows per consumer warpgroup (wgmma M)
-constexpr int kHalfN = kTileN / 2; // PIPE: database rows per ring stage and per MMA chain
+constexpr int kHalfN = kTileN / 2; // QUAD: database rows per ring stage and per MMA chain
 constexpr int kKBlock = 64;       // fp16 elements per 128-byte swizzle row
-constexpr int kConsumerWarps = 8; // two warpgroups
-constexpr int kTcThreads = 32 * kConsumerWarps + 32;
 constexpr int kMaxYStages = 6;
+// QUAD: one 16-bit candidate count per segment of the unit.  A writer stops counting at its first slot >= cap, so a
+// count never exceeds cap + 2 (two writers): caps up to kQuadMaxCap keep it in 16 bits.
+constexpr int kQuadCountBytes = kSegsPerUnit * 2;
+constexpr int kQuadMaxCap = 65533;
+
+// consumer warps of a layout: two or four warpgroups; the producer warp comes after them
+__host__ __device__ constexpr int tc_consumer_warps(bool quad) {
+    return quad ? 16 : 8;
+}
+__host__ __device__ constexpr int tc_threads(bool quad) {
+    return 32 * tc_consumer_warps(quad) + 32;
+}
 
 struct TcParams {
     int numUnits;
@@ -45,6 +60,7 @@ struct TcParams {
     int tileEnd;
     int tilesPerSlice;
     unsigned long long permA, permB, numTiles;
+    int permStep;       // permA % numTiles: the tile id step between consecutive positions
     int KB;             // dpad / 64
     int kSteps;         // ceil(d / 16): 16-wide MMA K-steps that hold data; the zero padding up to dpad is never issued
     int ksplit;         // 1: a ring stage holds ONE 64-wide K-block of a database tile (128 < d <= 256), else a whole tile
@@ -63,10 +79,9 @@ struct TcParams {
     int nq;
 };
 
-// The pipelined consumer (PIPE) needs exactly 8 K-steps in one 2-K-block stage: 112 < d <= 128.  Its K-step count must
-// be a compile-time constant: with a run-time count ptxas cannot tell which wgmma group is in flight and serialises
-// every MMA.
-__host__ __device__ constexpr bool tc_pipelined(int KB, int kSteps) {
+// The QUAD layout runs exactly 8 K-steps over one 2-K-block half-tile stage: 112 < d <= 128.  The K-step count is a
+// compile-time constant there, so the chain is fully unrolled.
+__host__ __device__ constexpr bool tc_quad(int KB, int kSteps) {
     return KB == 2 && kSteps == 2 * kKBlock / 16;
 }
 
@@ -79,6 +94,58 @@ __device__ __forceinline__ int chunk_col(int e) {
     return 8 * (e >> 1) + (e & 1);
 }
 
+// Appends the survivors of one candidate segment (one query row, one part) of the unit.
+// Everything but cnt is recomputed from kernel-wide values where it is used (survivors are rare): the QUAD consumer
+// has 96 registers per thread.
+template <bool QUAD>
+struct SegmentWriter {
+    const TcParams& p;
+    const int& unit;
+    uint32_t sCounts; // QUAD: shared-memory address of the unit's 16-bit segment counts
+    int local;        // the segment within the unit: query row * kParts + part
+    int cnt = 0;      // two-warpgroup layout: the segment's count; QUAD: 1 once this writer has met the cap
+
+    __device__ __forceinline__ long long seg() const {
+        return (long long)unit * kSegsPerUnit + local;
+    }
+    // QUAD: the address of the segment's 16-bit count
+    __device__ __forceinline__ uint32_t countAddr() const {
+        return sCounts + 2u * (uint32_t)local;
+    }
+    __device__ __forceinline__ void operator()(float v, unsigned col) {
+        uint2* buf = p.cand + seg() * p.cap;
+        const uint2 c = make_uint2(__float_as_uint(v), col);
+        if constexpr (QUAD) {
+            if (cnt == 0) {
+                const uint32_t a = countAddr();
+                const uint32_t sh = 8u * (a & 2u); // the count's half of its 32-bit word
+                uint32_t old;
+                asm volatile("atom.shared.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(a & ~3u), "r"(1u << sh) : "memory");
+                const int slot = (int)((old >> sh) & 0xffffu);
+                if (slot < p.cap)
+                    buf[slot] = c;
+                else
+                    cnt = 1; // a count above cap already flags the segment; stop before the 16 bits could wrap
+            }
+        } else {
+            if (cnt < p.cap)
+                buf[cnt] = c;
+            cnt++;
+        }
+    }
+    // the segment's count for candCount; QUAD, once every writer is done: also clears the counter for the next unit
+    __device__ __forceinline__ int take() {
+        if constexpr (QUAD) {
+            const uint32_t a = countAddr();
+            uint16_t n;
+            asm volatile("ld.shared.u16 %0, [%1];" : "=h"(n) : "r"(a) : "memory");
+            asm volatile("st.shared.u16 [%0], %1;" ::"r"(a), "h"((uint16_t)0) : "memory");
+            return n;
+        }
+        return cnt;
+    }
+};
+
 // Filter of one query row against 32 of its columns (database rows).
 //
 // The exact test is  score = fma(acc, inv, bias[row]) > thr.  The database tiles hold rows SORTED BY
@@ -86,8 +153,9 @@ __device__ __forceinline__ int chunk_col(int e) {
 // is a tight upper bound of every score in a group (inv > 0 and rounding are monotonic: no false
 // negatives, bit for bit).  The fast path is therefore a pure max tree over raw accumulators --
 // no bias loads, no per-element FMA -- plus one FMA per 32 columns; the rare group whose bound beats
-// the threshold evaluates the exact test with biases read through L1/L2.
-template <bool DUMP, bool SELF>
+// the threshold evaluates the exact test with biases read through L1/L2 and hands every survivor
+// (score, global row) to emit.
+template <bool DUMP, bool SELF, typename Emit>
 __device__ __forceinline__ void epi_filter32(
         const TcParams& p,
         const float (&r)[32],
@@ -97,9 +165,8 @@ __device__ __forceinline__ void epi_filter32(
         float& thr,  // SELF: tightened in place (running maximum minus the slack)
         float slack, // SELF: 2 * eps of this query
         float maxb,
-        uint2* buf,
-        int& cnt,
-        float minb = 0.f) { // SELF: min bias of the tile
+        float minb,  // SELF: min bias of the tile
+        Emit&& emit) {
     if (DUMP) {
         if (q < p.nq) {
             float* dst = p.dump + (long long)q * p.dumpLd + colBase;
@@ -134,9 +201,7 @@ __device__ __forceinline__ void epi_filter32(
                 for (int j = 8 * g; j < 8 * g + 8; j++) {
                     const float v = fmaf(r[j], inv, __ldg(bias + chunk_col(j)));
                     if (v > thr) {
-                        if (cnt < p.cap)
-                            buf[cnt] = make_uint2(__float_as_uint(v), rowBase + chunk_col(j));
-                        cnt++;
+                        emit(v, rowBase + chunk_col(j));
                         if (SELF) // k = 1: nothing scoring <= v - 2 eps can be the exact argmin any more
                             thr = fmaxf(thr, nextafterf(v - slack, -CUDART_INF_F));
                     }
@@ -147,30 +212,38 @@ __device__ __forceinline__ void epi_filter32(
 }
 
 // SELF (k = 1 streaming mode, used for k-means assignment): one pass over all tiles, every consumer thread keeps
-// a running "best approximate score minus 2 eps" threshold for its two queries and emits only the candidates
-// that beat it -- about ln(columns per thread) plus the near-ties of the maximum.
-// PIPE: tc_pipelined(p.KB, p.kSteps) holds, mapY's box is kHalfN rows and every ring stage holds one half of a tile.
-template <bool DUMP, bool SELF = false, bool PIPE = false>
-__global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
+// a running "best approximate score minus 2 eps" threshold for its two queries over its own columns and emits only
+// the candidates that beat it -- about ln(columns per thread) plus the near-ties of the maximum.
+// QUAD: tc_quad(p.KB, p.kSteps) holds, mapY's box is kHalfN rows, p.yStages == kMaxYStages and every ring stage holds one
+// half of a tile; the dynamic shared memory ends with kQuadCountBytes of segment counters.
+template <bool DUMP, bool SELF = false, bool QUAD = false>
+__global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
         const __grid_constant__ CUtensorMap mapQ,
         const __grid_constant__ CUtensorMap mapY,
         const TcParams p) {
+    constexpr int kConsumerWarps = tc_consumer_warps(QUAD);
     extern __shared__ unsigned char smem_dyn[];
     // 1024-byte aligned carve-up (SWIZZLE_128B atoms need it)
     unsigned char* smem = reinterpret_cast<unsigned char*>(
             (reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
-    const int qBytes = p.KB * kTileM * kKBlock * 2; // the query tile (128 rows)
+    // QUAD runs at KB = 2 with kMaxYStages stages: compile-time sizes spare the consumers registers
+    const int KB = QUAD ? 2 : p.KB;
+    const int yStages = QUAD ? kMaxYStages : p.yStages;
+    const int qBytes = KB * kTileM * kKBlock * 2; // the query tile (128 rows)
     // one ring stage: a whole database tile (256 rows x dpad), or -- K-split mode, dpad > 128, where the query tile
-    // plus several whole-tile stages no longer fit 227 KB -- one 64-wide K-block of it; PIPE: one 128-row half of a
+    // plus several whole-tile stages no longer fit 227 KB -- one 64-wide K-block of it; QUAD: one 128-row half of a
     // tile, laid out [kblock][128 rows][64] like a whole tile (the K-block stride is 16 KB)
-    const int stageBytes = PIPE ? p.KB * kHalfN * kKBlock * 2 : (p.ksplit ? 1 : p.KB) * kTileN * kKBlock * 2;
+    const int stageBytes = QUAD ? KB * kHalfN * kKBlock * 2 : (p.ksplit ? 1 : KB) * kTileN * kKBlock * 2;
     unsigned char* sQ = smem;
     unsigned char* sY = smem + qBytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sY + (size_t)p.yStages * stageBytes);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sY + (size_t)yStages * stageBytes);
     uint64_t* q_full = bars + 0;
     uint64_t* q_empty = bars + 1;
     uint64_t* y_full = bars + 2;
     uint64_t* y_empty = y_full + kMaxYStages;
+    // QUAD: 16-bit candidate counts of the unit's segments, behind the 512 bytes of barriers
+    uint32_t* segCount = reinterpret_cast<uint32_t*>(reinterpret_cast<unsigned char*>(bars) + 512);
+    const uint32_t sCounts = ptx::smem_u32(segCount);
 
     // warp index as a provably warp-uniform value: ptxas then knows every warpgroup reaches its wgmma converged
     // (otherwise it serialises the wgmma chain)
@@ -182,12 +255,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
         ptx::prefetch_tensormap(&mapY);
         ptx::mbar_init(q_full, 1);
         ptx::mbar_init(q_empty, kConsumerWarps);
-        for (int i = 0; i < p.yStages; i++) {
+        for (int i = 0; i < yStages; i++) {
             ptx::mbar_init(&y_full[i], 1);
-            ptx::mbar_init(&y_empty[i], kConsumerWarps);
+            ptx::mbar_init(&y_empty[i], 8); // the eight warps (two warpgroups) that read a stage
         }
         ptx::fence_barrier_init();
     }
+    if (QUAD && !DUMP)
+        for (int i = threadIdx.x; i < kQuadCountBytes / 4; i += blockDim.x)
+            segCount[i] = 0;
     __syncthreads();
 
     if (warp == kConsumerWarps) {
@@ -206,18 +282,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
                 const int pe = min(p.tileEnd, pb + p.tilesPerSlice);
                 for (int pp = pb; pp < pe; pp++) {
                     const int t = perm_tile(p, pp);
-                    // K-split: mapY's box is one K-block; PIPE: it is one half of the tile's rows (the second half of
-                    // the last tile may lie wholly past N: TMA zero-fills it and still counts the full box).  Both
-                    // warpgroups consume every stage.
-                    const int loads = PIPE ? 2 : p.ksplit ? p.KB : 1;
+                    // K-split: mapY's box is one K-block; QUAD: it is one half of the tile's rows (the second half of
+                    // the last tile may lie wholly past N: TMA zero-fills it and still counts the full box)
+                    const int loads = QUAD ? 2 : p.ksplit ? KB : 1;
                     for (int l = 0; l < loads; l++) {
                         ptx::mbar_wait(&y_empty[ys], yphase ^ 1);
                         ptx::mbar_arrive_expect_tx(&y_full[ys], (uint32_t)stageBytes);
-                        if (PIPE)
+                        if (QUAD)
                             ptx::tma_load_3d(sY + (size_t)ys * stageBytes, &mapY, &y_full[ys], 0, t * kTileN + l * kHalfN, 0);
                         else
                             ptx::tma_load_3d(sY + (size_t)ys * stageBytes, &mapY, &y_full[ys], 0, t * kTileN, l);
-                        if (++ys == p.yStages) {
+                        if (++ys == yStages) {
                             ys = 0;
                             yphase ^= 1;
                         }
@@ -230,20 +305,23 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
 
     // ================================ consumers ================================
     const int wg = warp >> 2;
+    const int g = QUAD ? (wg & 1) : wg; // query half
+    const int h = QUAD ? (wg >> 1) : 0; // QUAD: column half of every tile (and of the ring)
     const int part = lane & 3;
-    const int row = wg * kWgM + (warp & 3) * 16 + (lane >> 2); // first of the thread's two rows; the second is row + 8
+    const int row = g * kWgM + (warp & 3) * 16 + (lane >> 2); // first of the thread's two rows; the second is row + 8
     const float inv = *p.invScalePtr;
-    const uint32_t sQaddr = ptx::smem_u32(sQ) + (uint32_t)(wg * kWgM * kKBlock * 2); // this warpgroup's 64 rows
+    const uint32_t sQaddr = ptx::smem_u32(sQ) + (uint32_t)(g * kWgM * kKBlock * 2); // this warpgroup's 64 rows
     const uint32_t sYaddr = ptx::smem_u32(sY);
     const int qkb = kTileM * kKBlock * 2; // bytes per K-block of the query tile
     const int ykb = kTileN * kKBlock * 2; // bytes per K-block of a database tile
-    const int hkb = kHalfN * kKBlock * 2; // PIPE: bytes per K-block of a half-tile stage
-    const int permStep = (int)(p.permA % p.numTiles);
-    float acc[128];
+    const int hkb = kHalfN * kKBlock * 2; // QUAD: bytes per K-block of a half-tile stage
+    constexpr int kAcc = QUAD ? 64 : 128;
+    float acc[kAcc];
 #pragma unroll
-    for (int i = 0; i < 128; i++)
+    for (int i = 0; i < kAcc; i++)
         acc[i] = 0.f;
-    int ys = 0;
+    // QUAD: this warpgroup's sub-ring is stages h, h + 2, h + 4, ...
+    int ys = h;
     uint32_t yphase = 0;
     int it = 0;
     for (int u = blockIdx.x; u < p.numUnits; u += gridDim.x, it++) {
@@ -256,11 +334,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
         float thr1 = (!DUMP && q1 < p.nq) ? p.thr[q1] : CUDART_INF_F;
         const float slack0 = (SELF && q0 < p.nq) ? 2.f * p.eps[q0] : 0.f;
         const float slack1 = (SELF && q1 < p.nq) ? 2.f * p.eps[q1] : 0.f;
-        const long long seg0 = ((long long)u * kUnitM + row) * kParts + part;
-        const long long seg1 = ((long long)u * kUnitM + row + 8) * kParts + part;
-        uint2* buf0 = DUMP ? nullptr : p.cand + seg0 * p.cap;
-        uint2* buf1 = DUMP ? nullptr : p.cand + seg1 * p.cap;
-        int cnt0 = 0, cnt1 = 0;
+        SegmentWriter<QUAD> w0{p, u, sCounts, row * kParts + part};
+        SegmentWriter<QUAD> w1{p, u, sCounts, (row + 8) * kParts + part};
         const int pb = p.tileBegin + sl * p.tilesPerSlice;
         const int pe = min(p.tileEnd, pb + p.tilesPerSlice);
 
@@ -271,14 +346,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
         float minbNext = (SELF && pb < pe) ? __ldg(p.tileMinBias + t) : 0.f;
         ptx::mbar_wait(q_full, it & 1);
 
-        // the tile being filtered: this thread's first column of it and its bias bounds
-        long long colBase = 0;
+        // the tile being filtered and its bias bounds
+        int tile = 0;
         float maxb = 0.f, minb = 0.f;
         auto nextTile = [&](int pp) {
-            colBase = (long long)t * kTileN + 2 * part;
+            tile = t;
             maxb = maxbNext;
             minb = minbNext;
-            t += permStep;
+            t += p.permStep;
             if (t >= (int)p.numTiles)
                 t -= (int)p.numTiles;
             if (!DUMP && pp + 1 < pe)
@@ -286,80 +361,57 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
             if (SELF && pp + 1 < pe)
                 minbNext = __ldg(p.tileMinBias + t);
         };
-        // filter of the tile's columns 128 c .. 128 c + 127 (acc[64 c .. 64 c + 63]) for both of the thread's rows
+        // filter of the 128 columns held in acc[64 c .. 64 c + 63] for both of the thread's rows
         auto filterHalf = [&](int c) {
+            // this thread's first column of them
+            const long long colBase = (long long)tile * kTileN + kHalfN * (h + c) + 2 * part;
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
+            for (int hr = 0; hr < 2; hr++) {
                 float r[32];
 #pragma unroll
                 for (int e = 0; e < 32; e++)
-                    r[e] = acc[4 * (16 * c + (e >> 1)) + 2 * h + (e & 1)];
-                if (h)
-                    epi_filter32<DUMP, SELF>(p, r, q1, colBase + 128 * c, inv, thr1, slack1, maxb, buf1, cnt1, minb);
+                    r[e] = acc[4 * (16 * c + (e >> 1)) + 2 * hr + (e & 1)];
+                if (hr)
+                    epi_filter32<DUMP, SELF>(p, r, q1, colBase, inv, thr1, slack1, maxb, minb, w1);
                 else
-                    epi_filter32<DUMP, SELF>(p, r, q0, colBase + 128 * c, inv, thr0, slack0, maxb, buf0, cnt0, minb);
+                    epi_filter32<DUMP, SELF>(p, r, q0, colBase, inv, thr0, slack0, maxb, minb, w0);
             }
         };
 
-        if constexpr (PIPE) {
-            // ring stages are taken and handed back one half-tile at a time
-            auto acquireStage = [&]() {
+        if constexpr (QUAD) {
+            // the bias bounds are loaded for the tile at hand: the stage wait and the MMA chain hide their latency,
+            // and a bound fetched a tile ahead would cost registers the 96-register budget does not have
+            tile = t;
+            for (int left = pe - pb; left > 0; left--) {
+                maxb = DUMP ? 0.f : __ldg(p.tileMaxBias + tile);
+                minb = SELF ? __ldg(p.tileMinBias + tile) : 0.f;
                 ptx::mbar_wait(&y_full[ys], yphase);
-                const int s = ys;
-                if (++ys == p.yStages) {
-                    ys = 0;
-                    yphase ^= 1;
-                }
-                return s;
-            };
-            auto releaseStage = [&](int s) {
-                __syncwarp();
-                if (lane == 0) // this warp's share of the stage has been read
-                    ptx::mbar_arrive(&y_empty[s]);
-            };
-            // chain c: columns 128 c .. 128 c + 127 of the tile (the half in stage s) into acc[64 c .. 64 c + 63],
-            // committed as one wgmma group.  c must be a compile-time constant at every call.
-            auto issueHalf = [&](int c, int s) {
-                const uint32_t yaddr = sYaddr + (uint32_t)s * (uint32_t)stageBytes;
-                ptx::wgmma_fence_operands<64>(acc + 64 * c);
+                const uint32_t yaddr = sYaddr + (uint32_t)ys * (uint32_t)stageBytes;
+                ptx::wgmma_fence_operands<64>(acc);
                 ptx::wgmma_fence(); // the accumulators were last read by the filter
 #pragma unroll
                 for (int ks = 0; ks < 2 * kKBlock / 16; ks++) {
                     const int kb = ks >> 2, k4 = ks & 3;
                     const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + kb * qkb + k4 * 32);
                     const uint64_t db = ptx::make_smem_desc_sw128(yaddr + kb * hkb + k4 * 32);
-                    ptx::wgmma_m64n128k16_f16_ss(acc + 64 * c, da, db, ks != 0 ? 1u : 0u);
+                    ptx::wgmma_m64n128k16_f16_ss(acc, da, db, ks != 0 ? 1u : 0u);
                 }
                 ptx::wgmma_commit();
-                ptx::wgmma_fence_operands<64>(acc + 64 * c);
-            };
-            // Iteration pp issues A(pp), filters B(pp - 1) while A(pp) runs, then issues B(pp) and filters A(pp) while
-            // B(pp) runs.  Nothing is in flight across the back-edge: ptxas cannot follow a group that is still in
-            // flight there and would serialise every MMA, so B(pp) is waited for at the end of the iteration and
-            // filtered at the start of the next (the unit's last one after the loop).  A half-stage goes back to the
-            // producer as soon as its chain retires.  The filter order per thread -- tile by tile, columns 0-127
-            // first -- is that of the unpipelined loop.
-            for (int pp = pb; pp < pe; pp++) {
-                const int sA = acquireStage();
-                issueHalf(0, sA);
-                // only A(pp) is in flight, so this returns at once; without it ptxas cannot tell that B(pp - 1) has
-                // retired and waits for A(pp) before the filter below
-                ptx::wgmma_wait_all_but_one();
-                if (pp > pb)
-                    filterHalf(1); // B(pp - 1)
-                nextTile(pp);
-                const int sB = acquireStage();
-                issueHalf(1, sB);
-                ptx::wgmma_wait_all_but_one(); // A(pp) retired
+                ptx::wgmma_wait_all();
                 ptx::wgmma_fence_operands<64>(acc);
-                releaseStage(sA);
+                __syncwarp();
+                if (lane == 0) // this warp's share of the stage has been read
+                    ptx::mbar_arrive(&y_empty[ys]);
+                ys += 2;
+                if (ys >= yStages) {
+                    ys -= yStages;
+                    yphase ^= 1;
+                }
                 filterHalf(0);
-                ptx::wgmma_wait_all(); // B(pp) retired
-                ptx::wgmma_fence_operands<64>(acc + 64);
-                releaseStage(sB);
+                tile += p.permStep;
+                if (tile >= (int)p.numTiles)
+                    tile -= (int)p.numTiles;
             }
-            if (pb < pe)
-                filterHalf(1); // B of the unit's last tile
         } else {
             for (int pp = pb; pp < pe; pp++) {
                 nextTile(pp);
@@ -395,12 +447,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) flat_tc_kernel(
                 filterHalf(1);
             }
         }
+        if (QUAD && !DUMP) {
+            // both writers of this query half's segments are done: warpgroup (g, 0) publishes the counts and clears
+            // the counters.  Warpgroup (g, 1) counts again only after the next query tile arrives, which needs this
+            // warp's q_empty arrival below.
+            asm volatile("bar.sync %0, 256;" ::"r"(1 + g) : "memory");
+            if (h == 0) {
+                p.candCount[w0.seg()] = w0.take();
+                p.candCount[w1.seg()] = w1.take();
+            }
+        }
         __syncwarp();
         if (lane == 0) // the query tile may be overwritten
             ptx::mbar_arrive(q_empty);
-        if (!DUMP) {
-            p.candCount[seg0] = cnt0;
-            p.candCount[seg1] = cnt1;
+        if (!QUAD && !DUMP) {
+            p.candCount[w0.seg()] = w0.take();
+            p.candCount[w1.seg()] = w1.take();
         }
     }
 }
