@@ -514,6 +514,12 @@ class GpuIndexFlat(Index):
         check(lib.faiss_GpuIndexFlat_lastSearchInfo(self._h, out))
         return {"tensor_cores": int(out[0]), "fallback_queries": int(out[1])}
 
+    def lastSearchOperandBits(self):
+        """Operand width of the last search's tensor-core scoring: 8 (int8), 16 (fp16), or 0 (exact kernel)."""
+        out = ctypes.c_int(0)
+        check(lib.faiss_GpuIndexFlat_lastSearchOperandBits(self._h, ctypes.byref(out)))
+        return int(out.value)
+
 
 class GpuIndexFlatL2(GpuIndexFlat):
     def __init__(self, res, d, device=0, use_tensor_cores=True, use_float16=False):
@@ -1059,7 +1065,8 @@ def topk_merge(res, D_in, I_in, k, metric=METRIC_L2, id_offsets=None, device=0):
 
 
 def flat_tc_scores_debug(res, Q16, Y16, device=0):
-    """Raw tensor-core fp16 score matrix [nq, roundup(N,256)] (unit-test seam)."""
+    """Raw tensor-core score matrix [nq, roundup(N,256)] (unit-test seam): fp16 rows, or int8 rows of 128 whose
+    scores are the exact integer dot products."""
     import torch
 
     nq, dpad = Q16.shape
@@ -1067,6 +1074,14 @@ def flat_tc_scores_debug(res, Q16, Y16, device=0):
     res.setDefaultStream(device, torch.cuda.current_stream(device).cuda_stream)
     npad = (N + 255) // 256 * 256
     S = torch.zeros((nq, npad), dtype=torch.float32, device=Q16.device)
+    if Q16.dtype == torch.int8:
+        check(
+            lib.b200_flat_tc_scores_debug_s8(
+                res._h, int(device), ctypes.c_void_p(Q16.data_ptr()), ctypes.c_int64(nq), ctypes.c_void_p(Y16.data_ptr()),
+                ctypes.c_int64(N), _ptr(S, _c_f),
+            )
+        )
+        return S
     check(
         lib.b200_flat_tc_scores_debug(
             res._h, int(device), ctypes.c_void_p(Q16.data_ptr()), ctypes.c_int64(nq), ctypes.c_void_p(Y16.data_ptr()),

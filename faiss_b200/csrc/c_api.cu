@@ -352,6 +352,12 @@ int faiss_GpuIndexFlat_lastSearchInfo(const FaissGpuIndex* p, int* out2) {
     }
     CATCH_AND_HANDLE
 }
+int faiss_GpuIndexFlat_lastSearchOperandBits(const FaissGpuIndex* p, int* bits) {
+    try {
+        *bits = AS<GpuIndexFlat>(p, "GpuIndexFlat")->lastSearchOperandBits;
+    }
+    CATCH_AND_HANDLE
+}
 
 // ---------------------------------------------------------------- GpuIndexIVF
 int faiss_GpuIndexIVF_set_nprobe(FaissGpuIndex* p, size_t nprobe) {
@@ -1247,7 +1253,15 @@ int b200_flat_tc_scores_debug(
     try {
         auto res = RES(r);
         DeviceScope s(device);
-        runFlatTcScoresDebug((const __half*)Q16, nq, (const __half*)Y16, N, dpad, S, res->getDefaultStream(device));
+        runFlatTcScoresDebug(Q16, nq, Y16, N, dpad, false, S, res->getDefaultStream(device));
+    }
+    CATCH_AND_HANDLE
+}
+int b200_flat_tc_scores_debug_s8(FaissStandardGpuResources* r, int device, const void* Q8, idx_t nq, const void* Y8, idx_t N, float* S) {
+    try {
+        auto res = RES(r);
+        DeviceScope s(device);
+        runFlatTcScoresDebug(Q8, nq, Y8, N, 128, true, S, res->getDefaultStream(device));
     }
     CATCH_AND_HANDLE
 }

@@ -222,6 +222,185 @@ __global__ void tc_prepare_queries_kernel(
     }
 }
 
+// ---- int8 layout (DESIGN.md 3.1, "int8 scoring").  Centring, quantisation and the certificate's database constants.
+constexpr int kDpad8 = 128; // s8 per stored row: one 128-byte swizzle row
+
+// per-dimension min / max of the rows (order-preserving keys; NaN and inf are ignored); one thread per dimension
+__global__ void tc_col_range_kernel(const void* __restrict__ Y, int yHalf, int64_t n, int d, unsigned* __restrict__ range) {
+    const int j = threadIdx.x;
+    if (j >= d)
+        return;
+    unsigned lo = 0xffffffffu, hi = 0u;
+    for (int64_t r = blockIdx.x; r < n; r += gridDim.x) {
+        const float v = yHalf ? row_load1<true>(Y, r * d + j) : reinterpret_cast<const float*>(Y)[r * d + j];
+        if (v == v && fabsf(v) <= FLT_MAX) {
+            lo = min(lo, float_to_ordered(v));
+            hi = max(hi, float_to_ordered(v));
+        }
+    }
+    atomicMin(range + j, lo);
+    atomicMax(range + d + j, hi);
+}
+
+// centre c = per-dimension midrange (0 for a dimension without a finite value), and the database scale
+// s_y = 127 / max |fl(y - c)| (fl is monotone: the extremes of y give the extremes of fl(y - c)); one block of kDpad8
+__global__ void tc_center_kernel(const unsigned* __restrict__ range, int d, float* __restrict__ center, float* __restrict__ scale) {
+    __shared__ float red[kDpad8 / 32];
+    const int j = threadIdx.x;
+    float a = 0.f;
+    if (j < d) {
+        const unsigned lo = range[j], hi = range[d + j];
+        float c = 0.f;
+        if (lo <= hi) {
+            const float mn = ordered_to_float(lo), mx = ordered_to_float(hi);
+            c = 0.5f * mn + 0.5f * mx;
+            a = fmaxf(mx - c, c - mn);
+        }
+        center[j] = c;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+        a = fmaxf(a, __shfl_xor_sync(kFullMask, a, o));
+    if (lane_id() == 0)
+        red[j >> 5] = a;
+    __syncthreads();
+    if (j == 0) {
+        float m = 0.f;
+        for (int w = 0; w < kDpad8 / 32; w++)
+            m = fmaxf(m, red[w]);
+        *scale = m > 0.f ? 127.f / m : 1.f;
+    }
+}
+
+// one warp per row, lane l holds dimensions 4l .. 4l + 3 of fl(y - c).  Without Y8: the squared centred norm (the sort
+// key) and the plain norm |y| (for the fitness test).  With Y8: the row at stored position `row` (source perm[row])
+// quantised to Y8 = rn(fl(y - c) * s_y) in [-127, 127], zero padded to 128, its bias -|y - c|^2 / 2 and, into
+// stats[0..2] (max of non-negative floats as ints), |Y8 / s_y|^2, |fl(y - c) - Y8 / s_y|^2 and |y - c|^2.
+__global__ void tc_prepare_rows8_kernel(
+        const void* __restrict__ Y,
+        int yHalf,
+        int64_t n,
+        int d,
+        const float* __restrict__ center,
+        const float* __restrict__ scale,
+        const int* __restrict__ perm,
+        int8_t* __restrict__ Y8,
+        float* __restrict__ bias,
+        float* __restrict__ keys,
+        float* __restrict__ norms,
+        float* __restrict__ stats) {
+    const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= n)
+        return;
+    const int64_t src = (perm ? (int64_t)perm[row] : row) * d;
+    const float sy = *scale;
+    float yc2 = 0.f, y2 = 0.f, r2 = 0.f;
+    int h2 = 0;
+    uint32_t packed = 0;
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+        const int i = 4 * lane_id() + u;
+        float y = 0.f, v = 0.f;
+        if (i < d) {
+            y = yHalf ? row_load1<true>(Y, src + i) : reinterpret_cast<const float*>(Y)[src + i];
+            v = y - center[i];
+        }
+        yc2 = fmaf(v, v, yc2);
+        y2 = fmaf(y, y, y2);
+        const int c = (int)fminf(127.f, fmaxf(-127.f, rintf(v * sy)));
+        h2 += c * c;
+        const float r = v - (float)c / sy;
+        r2 = fmaf(r, r, r2);
+        packed |= (uint32_t)(uint8_t)(int8_t)c << (8 * u);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        yc2 += __shfl_xor_sync(kFullMask, yc2, o);
+        y2 += __shfl_xor_sync(kFullMask, y2, o);
+        r2 += __shfl_xor_sync(kFullMask, r2, o);
+        h2 += __shfl_xor_sync(kFullMask, h2, o);
+    }
+    if (!Y8) {
+        if (lane_id() == 0) {
+            keys[row] = yc2;
+            norms[row] = sqrtf(y2);
+        }
+        return;
+    }
+    reinterpret_cast<uint32_t*>(Y8 + row * kDpad8)[lane_id()] = packed;
+    if (lane_id() == 0) {
+        bias[row] = -0.5f * yc2;
+        const float hn = (float)h2 / (sy * sy);
+        atomicMax(reinterpret_cast<int*>(stats + 0), __float_as_int(hn));
+        atomicMax(reinterpret_cast<int*>(stats + 1), __float_as_int(r2));
+        atomicMax(reinterpret_cast<int*>(stats + 2), __float_as_int(yc2));
+    }
+}
+
+// int8 query preparation, one warp per query (lane l: dimensions 4l .. 4l + 3): q_c = fl(q - c), its own scale
+// s_q = 127 / max|q_c|, Q8 = rn(q_c * s_q), inv = fl(1 / (s_q * s_y)) and the certificate (DESIGN.md 3.1)
+//   eps = |q^|*maxR + |r_q|*maxY^ + |r_q|*maxR   (quantisation; q^ = Q8 / s_q, r_q = q_c - q^)
+//       + 2^-20 * |q^| * maxY^                     (inv and the FMA's rounding of acc * inv, residuals computed in fp32)
+//       + c2 * (|q_c| + maxYc)^2                    (bias, centring, the FMA's rounding of the bias, the exact kernel)
+__global__ void tc_prepare_queries8_kernel(
+        const float* __restrict__ Q,
+        int64_t nq,
+        int d,
+        const float* __restrict__ center,
+        const float* __restrict__ yScale,
+        float maxYhat,
+        float maxRy,
+        float maxYc,
+        float c2,
+        int8_t* __restrict__ Q8,
+        float* __restrict__ invQ,
+        float* __restrict__ eps,
+        float* __restrict__ thr) {
+    const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= nq)
+        return;
+    float v[4];
+    float a = 0.f;
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+        const int i = 4 * lane_id() + u;
+        v[u] = i < d ? Q[row * d + i] - center[i] : 0.f;
+        a = fmaxf(a, fabsf(v[u]));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+        a = fmaxf(a, __shfl_xor_sync(kFullMask, a, o));
+    const float sq = a > 0.f ? 127.f / a : 1.f;
+    float qc2 = 0.f, r2 = 0.f;
+    int h2 = 0;
+    uint32_t packed = 0;
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+        const int c = (int)fminf(127.f, fmaxf(-127.f, rintf(v[u] * sq)));
+        qc2 = fmaf(v[u], v[u], qc2);
+        h2 += c * c;
+        const float r = v[u] - (float)c / sq;
+        r2 = fmaf(r, r, r2);
+        packed |= (uint32_t)(uint8_t)(int8_t)c << (8 * u);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        qc2 += __shfl_xor_sync(kFullMask, qc2, o);
+        r2 += __shfl_xor_sync(kFullMask, r2, o);
+        h2 += __shfl_xor_sync(kFullMask, h2, o);
+    }
+    reinterpret_cast<uint32_t*>(Q8 + row * kDpad8)[lane_id()] = packed;
+    if (lane_id() == 0) {
+        const float qh = sqrtf((float)h2) / sq * 1.0001f;
+        const float rq = sqrtf(r2) * 1.0001f;
+        const float qc = sqrtf(qc2) * 1.0001f;
+        const float s = qc + maxYc;
+        eps[row] = (qh * maxRy + rq * maxYhat + rq * maxRy) * 1.0001f + ldexpf(1.f, -20) * qh * maxYhat + c2 * s * s;
+        invQ[row] = 1.f / (sq * *yScale);
+        thr[row] = -CUDART_INF_F;
+    }
+}
+
 // pending-candidate buffer of the select kernel: a round brings ~(growth-1)*k candidates per query, and
 // the cost of a flush is dominated by the merge into the 2k-entry list -- fewer, larger flushes
 constexpr int kSelectBuf = 128;
@@ -384,7 +563,7 @@ __global__ void __launch_bounds__(kSelWarps * 32) tc_select_bisect_kernel(
     float* bk = baseKey + (int64_t)q * LIST;
     int* bi = baseId + (int64_t)q * LIST;
     {
-        constexpr int kMaxListIter = 8; // LIST <= 256
+        constexpr int kMaxListIter = 16; // LIST <= 512 (int8 scoring: 4k entries at k <= 128)
         int ids[kMaxListIter];
         float scs[kMaxListIter];
 #pragma unroll
@@ -814,20 +993,49 @@ CUtensorMap makeTileMap(const __half* base, int64_t rows, int dpad, int boxRows,
     return m;
 }
 
+// int8 matrix [rows][128] viewed as (128, rows, 1); one box = 128 bytes x boxRows rows, 128-byte swizzle
+CUtensorMap makeTileMap8(const int8_t* base, int64_t rows, int boxRows) {
+    CUtensorMap m;
+    cuuint64_t dims[3] = {(cuuint64_t)kDpad8, (cuuint64_t)rows, 1};
+    cuuint64_t strides[2] = {(cuuint64_t)kDpad8, (cuuint64_t)rows * kDpad8};
+    cuuint32_t box[3] = {(cuuint32_t)kDpad8, (cuuint32_t)boxRows, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = getEncodeTiled()(
+            &m,
+            CU_TENSOR_MAP_DATA_TYPE_UINT8,
+            3,
+            const_cast<int8_t*>(base),
+            dims,
+            strides,
+            box,
+            estr,
+            CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B,
+            CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    FB_THROW_IF_NOT_FMT(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with %d", (int)r);
+    return m;
+}
+
 struct SmemPlan {
     int yStages;
     size_t bytes;
     int ksplit; // ring stages hold single K-blocks (see flat_tc_kernel)
     bool quad;  // four consumer warpgroups over half-tile ring stages (flat_tc_kernel QUAD)
     int boxRows; // database rows per TMA copy of mapY
+    bool s8;    // int8 operands (flat_tc_kernel S8)
 };
 
 constexpr int kMaxKB = 4; // d <= 256: the query tile (16 KB per K-block) + at least three 32 KB K-block stages in 227 KB
 
 // 112 < d <= 128: half-tile stages (32 KB: six of them, which the QUAD kernel takes as a constant); other d <= 128:
 // whole-tile stages (64 KB at d = 128: three of them); beyond, K-block stages (see flat_tc_kernel)
-SmemPlan planSmem(int KB, int kSteps) {
+SmemPlan planSmem(int KB, int kSteps, bool s8 = false) {
     FB_THROW_IF_NOT_MSG(KB <= kMaxKB, "dimension too large for the tensor-core Flat kernel");
+    if (s8) { // int8, QUAD: 16 KB query tile and half-tile stages
+        const size_t fixed = 1024 + 512 + kQuadCountBytes + (size_t)kTileM * kDpad8;
+        return {kS8Stages, fixed + (size_t)kS8Stages * kHalfN * kDpad8, 0, true, kHalfN, true};
+    }
     const int ksplit = KB > 2 ? 1 : 0;
     const bool quad = tc_quad(KB, kSteps);
     const int boxRows = quad ? kHalfN : kTileN;
@@ -837,7 +1045,7 @@ SmemPlan planSmem(int KB, int kSteps) {
     const size_t budget = 227 * 1024; // the opt-in limit per CTA
     int ys = (int)std::min<size_t>(kMaxYStages, (budget - fixed) / stage);
     FB_THROW_IF_NOT(ys >= 3 && (!quad || ys == kMaxYStages));
-    return {ys, fixed + ys * stage, ksplit, quad, boxRows};
+    return {ys, fixed + ys * stage, ksplit, quad, boxRows, false};
 }
 
 // the kernel's parameters for one round over nq queries (the search's pointers are filled in by the caller)
@@ -872,6 +1080,8 @@ void launchTc(const CUtensorMap& mq, const CUtensorMap& my, const TcParams& p, i
     auto kern = sp.quad ? flat_tc_kernel<DUMP, false, true> : flat_tc_kernel<DUMP>;
     if (self && !DUMP) // k = 1 streaming mode (self-tightening thresholds)
         kern = sp.quad ? flat_tc_kernel<false, true, true> : flat_tc_kernel<false, true>;
+    if (sp.s8)
+        kern = flat_tc_kernel<DUMP, false, true, true>;
     CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTiming::begin("flat_tc", stream);
     kern<<<grid, tc_threads(sp.quad), smem, stream>>>(mq, my, p);
@@ -914,19 +1124,43 @@ FlatTcDatabase::FlatTcDatabase(GpuResources* res, int device, int d)
           y16_(res, device, AllocType::FlatData),
           bias_(res, device, AllocType::FlatData),
           perm_(res, device, AllocType::FlatData),
-          tileBias_(res, device, AllocType::FlatData) {}
+          tileBias_(res, device, AllocType::FlatData),
+          y8_(res, device, AllocType::FlatData),
+          bias8_(res, device, AllocType::FlatData),
+          perm8_(res, device, AllocType::FlatData),
+          tileBias8_(res, device, AllocType::FlatData),
+          center_(res, device, AllocType::FlatData) {}
 
 void FlatTcDatabase::clear() {
     y16_.clear();
     bias_.clear();
     perm_.clear();
     tileBias_.clear();
+    y8_.clear();
+    bias8_.clear();
+    perm8_.clear();
+    tileBias8_.clear();
+    center_.clear();
     dirty_ = true;
 }
 
-void FlatTcDatabase::prepare(const void* rows, int64_t n, MetricType metric, int yHalf, cudaStream_t stream) {
+void FlatTcDatabase::prepare(const void* rows, int64_t n, MetricType metric, int yHalf, cudaStream_t) {
     if (!dirty_)
         return;
+    rows_ = rows;
+    n_ = n;
+    metric_ = metric;
+    yHalf_ = yHalf;
+    fp16Ready_ = false;
+    int8Ready_ = false;
+    dirty_ = false;
+}
+
+void FlatTcDatabase::prepareFp16(cudaStream_t stream) {
+    const void* rows = rows_;
+    const int64_t n = n_;
+    const MetricType metric = metric_;
+    const int yHalf = yHalf_;
     const int d = d_, dpad = dpad_;
     const int64_t padRows = round_up(n, 256) + 256; // whole 256-row tiles, -inf beyond n
     y16_.resize((size_t)n * dpad, stream);
@@ -982,11 +1216,85 @@ void FlatTcDatabase::prepare(const void* rows, int64_t n, MetricType metric, int
     CUDA_VERIFY(cudaStreamSynchronize(stream));
     scale_ = scale;
     maxNorm_ = std::sqrt(h[1]) * 1.0001f;
-    rows_ = rows;
-    n_ = n;
-    metric_ = metric;
-    yHalf_ = yHalf;
-    dirty_ = false;
+    fp16Ready_ = true;
+}
+
+// Fitness of the int8 layout.  The int8 certificate's database term for a query q is about |q|*max|r_y|, the fp16
+// one c1*|q|*|y|: the int8 path is taken while max|r_y| <= kInt8Fitness * c1 * (mean |y|).  Uniform data gives about
+// 2.2, where the base list of 4k entries holds every entry within 2 eps of the k-th best with room to spare (DESIGN.md
+// 3.1); an outlier coordinate that collapses s_y makes max|r_y| as large as the ordinary rows themselves and fails.
+constexpr float kInt8Fitness = 4.f;
+
+void FlatTcDatabase::prepareInt8(cudaStream_t stream) {
+    const int64_t n = n_;
+    const int d = d_;
+    const int64_t padRows = round_up(n, 256) + 256;
+    y8_.resize((size_t)n * kDpad8, stream);
+    bias8_.resize((size_t)padRows, stream);
+    tileBias8_.resize((size_t)(padRows / 256) * 2, stream);
+    perm8_.resize((size_t)n, stream);
+    center_.resize((size_t)d, stream);
+    // [0, 2d): column range keys; then s_y, the three stats maxima and the sum of row norms
+    auto scratch = res_->temp(device_, sizeof(unsigned) * 2 * d + sizeof(float) * 8);
+    unsigned* range = scratch.as<unsigned>();
+    float* sc = reinterpret_cast<float*>(range + 2 * d); // [s_y, max|y^|^2, max|r_y|^2, max|y_c|^2, sum |y|]
+    CUDA_VERIFY(cudaMemsetAsync(range, 0xff, sizeof(unsigned) * d, stream));
+    CUDA_VERIFY(cudaMemsetAsync(range + d, 0, sizeof(unsigned) * d + sizeof(float) * 8, stream));
+    tc_col_range_kernel<<<(unsigned)std::min<int64_t>(4096, std::max<int64_t>(1, n)), kDpad8, 0, stream>>>(rows_, yHalf_, n, d, range);
+    CUDA_CHECK_LAST();
+    tc_center_kernel<<<1, kDpad8, 0, stream>>>(range, d, center_.data(), sc);
+    CUDA_CHECK_LAST();
+    auto keys = res_->temp(device_, sizeof(float) * n);
+    auto norms = res_->temp(device_, sizeof(float) * n);
+    const int warps = 8;
+    const unsigned rowBlocks = (unsigned)ceil_div(n, warps);
+    tc_prepare_rows8_kernel<<<rowBlocks, warps * 32, 0, stream>>>(
+            rows_, yHalf_, n, d, center_.data(), sc, nullptr, nullptr, nullptr, keys.as<float>(), norms.as<float>(), nullptr);
+    CUDA_CHECK_LAST();
+    {
+        // stored order = rows sorted by the centred norm, which enters the bias
+        auto keysOut = res_->temp(device_, sizeof(float) * n);
+        auto valsIn = res_->temp(device_, sizeof(int) * n);
+        tc_iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, stream>>>(valsIn.as<int>(), n);
+        CUDA_CHECK_LAST();
+        size_t sortBytes = 0, sumBytes = 0;
+        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
+                nullptr, sortBytes, keys.as<float>(), keysOut.as<float>(), valsIn.as<int>(), perm8_.data(), (int)n, 0, 32, stream));
+        CUDA_VERIFY(cub::DeviceReduce::Sum(nullptr, sumBytes, norms.as<float>(), sc + 4, (int)n, stream));
+        auto tmp = res_->temp(device_, std::max(sortBytes, sumBytes));
+        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
+                tmp.data, sortBytes, keys.as<float>(), keysOut.as<float>(), valsIn.as<int>(), perm8_.data(), (int)n, 0, 32, stream));
+        CUDA_VERIFY(cub::DeviceReduce::Sum(tmp.data, sumBytes, norms.as<float>(), sc + 4, (int)n, stream));
+    }
+    fill_float_kernel<<<(unsigned)ceil_div(padRows, 256), 256, 0, stream>>>(bias8_.data(), padRows, -INFINITY);
+    CUDA_CHECK_LAST();
+    tc_prepare_rows8_kernel<<<rowBlocks, warps * 32, 0, stream>>>(
+            rows_, yHalf_, n, d, center_.data(), sc, perm8_.data(), y8_.data(), bias8_.data(), nullptr, nullptr, sc + 1);
+    CUDA_CHECK_LAST();
+    runTileBias(bias8_.data(), n, tileBias8_.data(), stream);
+    float h[5];
+    CUDA_VERIFY(cudaMemcpyAsync(h, sc, sizeof(h), cudaMemcpyDeviceToHost, stream));
+    CUDA_VERIFY(cudaStreamSynchronize(stream));
+    scale8_ = h[0];
+    maxYhat_ = std::sqrt(h[1]) * 1.0001f;
+    maxRy_ = std::sqrt(h[2]) * 1.0001f;
+    maxYc_ = std::sqrt(h[3]) * 1.0001f;
+    const float c1 = 1.01f * (ldexpf(1.f, -10) + (float)kDpad8 * ldexpf(1.f, -22));
+    const float meanNorm = h[4] / (float)n;
+    int8Fit_ = maxRy_ <= kInt8Fitness * c1 * meanNorm && std::isfinite(maxYc_) && std::isfinite(maxYhat_);
+    int8Ready_ = true;
+    if (!int8Fit_) { // the fp16 layout serves this database: give the memory back
+        y8_.clear();
+        bias8_.clear();
+        perm8_.clear();
+        tileBias8_.clear();
+    }
+}
+
+bool FlatTcDatabase::int8Eligible(int k, const FlatTcShard* shard) const {
+    // sharded searches pool thresholds across ranks, and centred scores of shards with different centres differ by a
+    // per-query offset: they stay fp16
+    return metric_ == METRIC_L2 && d_ > 112 && d_ <= kDpad8 && k >= 2 && k <= 128 && shard == nullptr;
 }
 
 // one search call: the schedule, the launch configuration and the bias arrays (the masked copies under a row mask)
@@ -999,6 +1307,8 @@ struct FlatTcDatabase::Call {
     const float* tileBias;
     CUtensorMap mapY;
     const FlatTcShard* shard;
+    bool int8;       // the int8 layout
+    const int* perm; // the layout's stored position -> row id (null: identity)
 };
 
 // device state of one query batch
@@ -1006,14 +1316,15 @@ struct FlatTcDatabase::Batch {
     const float* Q; // [nq][d]
     int64_t nq, qPairs;
     GpuMemoryReservation q16, scal, eps, thr, flags, baseKey, baseId;
+    GpuMemoryReservation invQ; // int8: per-query 1 / (s_q * s_y)
     CUtensorMap mapQ;
 };
 
-// the batch's queries -> scaled fp16 tiles, eps and thresholds; empty base lists
+// the batch's queries -> scaled fp16 (int8: centred, quantised) tiles, eps and thresholds; empty base lists
 void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
     const int64_t nq = b.nq, qPairs = b.qPairs;
     cudaStream_t stream = c.stream;
-    b.q16 = res_->temp(device_, sizeof(__half) * qPairs * kUnitM * dpad_);
+    b.q16 = res_->temp(device_, c.int8 ? (size_t)qPairs * kUnitM * kDpad8 : sizeof(__half) * qPairs * kUnitM * dpad_);
     b.scal = res_->temp(device_, sizeof(float) * 4); // [absmax, qScale, inv, -]
     b.eps = res_->temp(device_, sizeof(float) * nq);
     b.thr = res_->temp(device_, sizeof(float) * nq);
@@ -1027,20 +1338,30 @@ void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
 
     CUDA_VERIFY(cudaMemsetAsync(b.scal.data, 0, sizeof(float) * 4, stream));
     CUDA_VERIFY(cudaMemsetAsync(b.flags.data, 0, sizeof(int) * (nq + 1), stream));
-    CUDA_VERIFY(cudaMemsetAsync(b.q16.data, 0, sizeof(__half) * qPairs * kUnitM * dpad_, stream));
-    float* sc = b.scal.as<float>();
-    runAbsMax(b.Q, nq * d_, sc + 0, stream);
-    tc_query_scale_kernel<<<1, 1, 0, stream>>>(sc + 0, scale_, sc + 1, sc + 2);
-    CUDA_CHECK_LAST();
-    tc_prepare_queries_kernel<<<(unsigned)ceil_div(nq, 8), 256, 0, stream>>>(
-            b.Q, nq, d_, dpad_, sc + 1, c1, c2, maxNorm_, b.q16.as<__half>(), b.eps.as<float>(), b.thr.as<float>());
-    CUDA_CHECK_LAST();
+    CUDA_VERIFY(cudaMemsetAsync(b.q16.data, 0, b.q16.size, stream));
+    if (c.int8) {
+        b.invQ = res_->temp(device_, sizeof(float) * nq);
+        CUDA_VERIFY(cudaMemcpyAsync(b.scal.data, &scale8_, sizeof(float), cudaMemcpyHostToDevice, stream));
+        tc_prepare_queries8_kernel<<<(unsigned)ceil_div(nq, 8), 256, 0, stream>>>(
+                b.Q, nq, d_, center_.data(), b.scal.as<float>(), maxYhat_, maxRy_, maxYc_, c2, b.q16.as<int8_t>(),
+                b.invQ.as<float>(), b.eps.as<float>(), b.thr.as<float>());
+        CUDA_CHECK_LAST();
+    } else {
+        float* sc = b.scal.as<float>();
+        runAbsMax(b.Q, nq * d_, sc + 0, stream);
+        tc_query_scale_kernel<<<1, 1, 0, stream>>>(sc + 0, scale_, sc + 1, sc + 2);
+        CUDA_CHECK_LAST();
+        tc_prepare_queries_kernel<<<(unsigned)ceil_div(nq, 8), 256, 0, stream>>>(
+                b.Q, nq, d_, dpad_, sc + 1, c1, c2, maxNorm_, b.q16.as<__half>(), b.eps.as<float>(), b.thr.as<float>());
+        CUDA_CHECK_LAST();
+    }
     if (!c.s.streaming) {
         int64_t cnt = nq * c.s.LIST;
         tc_init_base_kernel<<<(unsigned)ceil_div(cnt, 256), 256, 0, stream>>>(b.baseKey.as<float>(), b.baseId.as<int>(), cnt);
         CUDA_CHECK_LAST();
     }
-    b.mapQ = makeTileMap(b.q16.as<__half>(), qPairs * kUnitM, dpad_, kTileM);
+    b.mapQ = c.int8 ? makeTileMap8(b.q16.as<int8_t>(), qPairs * kUnitM, kTileM)
+                    : makeTileMap(b.q16.as<__half>(), qPairs * kUnitM, dpad_, kTileM);
 }
 
 // One round: score its tiles and emit candidates, then fold them into the base lists and thresholds (and, sharded,
@@ -1056,6 +1377,7 @@ void FlatTcDatabase::runRound(const Call& c, const Batch& b, const FlatTcRound& 
     p.tileMinBias = c.tileBias + s.T + 1; // second half of the array (see tc_tile_max_bias_kernel)
     p.thr = b.thr.as<float>();
     p.eps = b.eps.as<float>();
+    p.invQ = c.int8 ? b.invQ.as<float>() : nullptr;
     p.cand = arena;
     p.candCount = counts;
     if (p.tileBegin < p.tileEnd) {
@@ -1112,7 +1434,7 @@ void FlatTcDatabase::rerank(const Call& c, const Batch& b, float* outD, idx_t* o
             auto kern = tc_rerank_kernel<l2, yh>;
             CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rrSmem));
             kern<<<(unsigned)ceil_div(b.nq, rrWarps), rrWarps * 32, rrSmem, stream>>>(
-                    (int)b.nq, d_, s.k, s.LIST, s.KL, b.Q, rows_, perm_.data(), b.baseId.as<int>(), b.baseKey.as<float>(),
+                    (int)b.nq, d_, s.k, s.LIST, s.KL, b.Q, rows_, c.perm, b.baseId.as<int>(), b.baseKey.as<float>(),
                     c.shard ? b.thr.as<float>() : nullptr, outD, outI);
         });
     });
@@ -1149,33 +1471,45 @@ int FlatTcDatabase::recomputeFallbacks(const Call& c, const Batch& b, const uint
 }
 
 int64_t FlatTcDatabase::search(const float* Q, int64_t nqAll, int k, float* outD, idx_t* outI, cudaStream_t stream,
-                               const FlatTcShard* shard, const uint32_t* rowMask) const {
+                               const FlatTcShard* shard, const uint32_t* rowMask) {
     FB_THROW_IF_NOT_MSG(!dirty_, "FlatTcDatabase::search before prepare");
     if (nqAll == 0)
         return 0;
-    const float* bias = bias_.data();
-    const float* tileBias = tileBias_.data();
+    FB_THROW_IF_NOT(flatTcSupported(d_, k, n_));
+    bool int8 = int8Eligible(k, shard);
+    if (int8 && !int8Ready_)
+        prepareInt8(stream);
+    int8 = int8 && int8Fit_;
+    if (!int8 && !fp16Ready_)
+        prepareFp16(stream);
+    lastBits_ = int8 ? 8 : 16;
+    const DeviceVector<float>& biasL = int8 ? bias8_ : bias_;
+    const DeviceVector<float>& tileBiasL = int8 ? tileBias8_ : tileBias_;
+    const int* perm = int8 ? perm8_.data() : perm_.data();
+    const float* bias = biasL.data();
+    const float* tileBias = tileBiasL.data();
     GpuMemoryReservation maskedBias, maskedTileBias;
     if (rowMask) {
         // an excluded row gets a -inf bias: its score can then never pass a round's threshold, exactly as the
-        // padding rows past n.  maxNorm_ over all rows stays a valid bound for the certificate.
-        maskedBias = res_->temp(device_, sizeof(float) * bias_.size());
-        maskedTileBias = res_->temp(device_, sizeof(float) * tileBias_.size());
-        const int64_t padRows = (int64_t)bias_.size();
+        // padding rows past n.  The certificate's maxima over all rows stay valid bounds.
+        maskedBias = res_->temp(device_, sizeof(float) * biasL.size());
+        maskedTileBias = res_->temp(device_, sizeof(float) * tileBiasL.size());
+        const int64_t padRows = (int64_t)biasL.size();
         mask_bias_kernel<<<(unsigned)ceil_div(padRows, (int64_t)256), 256, 0, stream>>>(
-                bias_.data(), perm_.data(), rowMask, n_, padRows, maskedBias.as<float>());
+                bias, perm, rowMask, n_, padRows, maskedBias.as<float>());
         CUDA_CHECK_LAST();
         runTileBias(maskedBias.as<float>(), n_, maskedTileBias.as<float>(), stream);
         bias = maskedBias.as<float>();
         tileBias = maskedTileBias.as<float>();
     }
-    FB_THROW_IF_NOT(flatTcSupported(d_, k, n_));
     const int KB = dpad_ / kKBlock;
     const int kSteps = (d_ + 15) / 16;
     const FlatTcSchedule s = planFlatTcSchedule(
-            n_, k, res_->numSMs(device_), shard ? shard->comm->size() : 0, shard ? shard->maxTiles : 0);
-    const SmemPlan sp = planSmem(KB, kSteps);
-    const Call c{stream, s, KB, kSteps, sp, bias, tileBias, makeTileMap(y16_.data(), n_, dpad_, sp.boxRows, sp.ksplit), shard};
+            n_, k, res_->numSMs(device_), shard ? shard->comm->size() : 0, shard ? shard->maxTiles : 0, int8);
+    const SmemPlan sp = planSmem(KB, kSteps, int8);
+    const CUtensorMap mapY = int8 ? makeTileMap8(y8_.data(), n_, sp.boxRows)
+                                  : makeTileMap(y16_.data(), n_, dpad_, sp.boxRows, sp.ksplit);
+    const Call c{stream, s, KB, kSteps, sp, bias, tileBias, mapY, shard, int8, perm};
     int64_t fallbacks = 0;
     for (int64_t qb = 0; qb < nqAll; qb += s.qBatch) {
         Batch b;
@@ -1200,19 +1534,23 @@ int64_t FlatTcDatabase::search(const float* Q, int64_t nqAll, int k, float* outD
     return fallbacks;
 }
 
-void runFlatTcScoresDebug(const __half* Q16, int64_t nq, const __half* Y16, int64_t n, int dpad, float* S, cudaStream_t stream) {
+void runFlatTcScoresDebug(const void* Q, int64_t nq, const void* Y, int64_t n, int dpad, bool s8, float* S,
+                          cudaStream_t stream) {
     FB_THROW_IF_NOT(dpad % kKBlock == 0 && dpad <= kMaxKB * kKBlock);
+    FB_THROW_IF_NOT_MSG(!s8 || dpad == kDpad8, "int8 scores take rows of 128");
     const int KB = dpad / kKBlock;
     const int kSteps = dpad / 16; // debug seam: operands arrive padded
-    SmemPlan sp = planSmem(KB, kSteps);
-    CUtensorMap my = makeTileMap(Y16, n, dpad, sp.boxRows, sp.ksplit);
+    SmemPlan sp = planSmem(KB, kSteps, s8);
+    const size_t rowBytes = s8 ? (size_t)kDpad8 : sizeof(__half) * dpad;
+    CUtensorMap my = s8 ? makeTileMap8((const int8_t*)Y, n, sp.boxRows)
+                        : makeTileMap((const __half*)Y, n, dpad, sp.boxRows, sp.ksplit);
     const int64_t numTiles = ceil_div(n, kTileN);
     const int64_t qPairs = ceil_div(nq, kUnitM);
     // the kernel reads whole 128-row query tiles: zero-padded private copy
-    __half* qpad = nullptr;
-    CUDA_VERIFY(cudaMallocAsync(&qpad, sizeof(__half) * qPairs * kUnitM * dpad, stream));
-    CUDA_VERIFY(cudaMemsetAsync(qpad, 0, sizeof(__half) * qPairs * kUnitM * dpad, stream));
-    CUDA_VERIFY(cudaMemcpyAsync(qpad, Q16, sizeof(__half) * nq * dpad, cudaMemcpyDeviceToDevice, stream));
+    void* qpad = nullptr;
+    CUDA_VERIFY(cudaMallocAsync(&qpad, rowBytes * qPairs * kUnitM, stream));
+    CUDA_VERIFY(cudaMemsetAsync(qpad, 0, rowBytes * qPairs * kUnitM, stream));
+    CUDA_VERIFY(cudaMemcpyAsync(qpad, Q, rowBytes * nq, cudaMemcpyDeviceToDevice, stream));
     // scale (1.0) for the debug run; the dump path never reads biases
     float* one = nullptr;
     CUDA_VERIFY(cudaMallocAsync(&one, sizeof(float), stream));
@@ -1221,7 +1559,8 @@ void runFlatTcScoresDebug(const __half* Q16, int64_t nq, const __half* Y16, int6
     // every tile in one slice, unpermuted
     const FlatTcRound all{0, (int)numTiles, 1, (int)numTiles, 0};
     TcParams p = roundParams(sp, KB, kSteps, nq, qPairs, all, numTiles, 1, 0, one);
-    CUtensorMap mq = makeTileMap(qpad, qPairs * kUnitM, dpad, kTileM);
+    CUtensorMap mq = s8 ? makeTileMap8((const int8_t*)qpad, qPairs * kUnitM, kTileM)
+                        : makeTileMap((const __half*)qpad, qPairs * kUnitM, dpad, kTileM);
     p.dump = S;
     p.dumpLd = numTiles * kTileN; // S must be [nq][numTiles*128]
     int dev = 0, sms = 0;

@@ -27,6 +27,8 @@
 
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "flat_tc_schedule.h" // kUnitM, kTileN, kParts, kSegsPerUnit
 #include "select.cuh"
 #include "tc_ptx.cuh"
@@ -39,6 +41,9 @@ constexpr int kWgM = 64;          // query rows per consumer warpgroup (wgmma M)
 constexpr int kHalfN = kTileN / 2; // QUAD: database rows per ring stage and per MMA chain
 constexpr int kKBlock = 64;       // fp16 elements per 128-byte swizzle row
 constexpr int kMaxYStages = 6;
+// S8 (int8 operands, QUAD only): a 128-byte swizzle row holds 128 s8, so the query tile and a half-tile stage are 16 KB
+// each and twelve stages fit beside them
+constexpr int kS8Stages = 12;
 // QUAD: one 16-bit candidate count per segment of the unit.  A writer stops counting at its first slot >= cap, so a
 // count never exceeds cap + 2 (two writers): caps up to kQuadMaxCap keep it in 16 bits.
 constexpr int kQuadCountBytes = kSegsPerUnit * 2;
@@ -77,6 +82,7 @@ struct TcParams {
     float* dump;        // debug: raw accumulators [nq][dumpLd]
     long long dumpLd;
     int nq;
+    const float* invQ;  // S8: [nq] per-query 1 / (s_q * s_y)
 };
 
 // The QUAD layout runs exactly 8 K-steps over one 2-K-block half-tile stage: 112 < d <= 128.  The K-step count is a
@@ -146,7 +152,8 @@ struct SegmentWriter {
     }
 };
 
-// Filter of one query row against 32 of its columns (database rows).
+// Filter of one query row against 32 of its columns (database rows).  T is the accumulator type: float (fp16 operands)
+// or int (s8 operands, where the fast path is an integer max tree and one exact int -> float conversion: |acc| < 2^24).
 //
 // The exact test is  score = fma(acc, inv, bias[row]) > thr.  The database tiles hold rows SORTED BY
 // NORM, so the biases of a tile are nearly equal and  bound = fma(max acc, inv, max bias of the tile)
@@ -155,10 +162,17 @@ struct SegmentWriter {
 // no bias loads, no per-element FMA -- plus one FMA per 32 columns; the rare group whose bound beats
 // the threshold evaluates the exact test with biases read through L1/L2 and hands every survivor
 // (score, global row) to emit.
-template <bool DUMP, bool SELF, typename Emit>
+__device__ __forceinline__ float tc_max(float a, float b) {
+    return fmaxf(a, b);
+}
+__device__ __forceinline__ int tc_max(int a, int b) {
+    return max(a, b);
+}
+
+template <bool DUMP, bool SELF, typename T, typename Emit>
 __device__ __forceinline__ void epi_filter32(
         const TcParams& p,
-        const float (&r)[32],
+        const T (&r)[32],
         int q,
         long long colBase, // global (sorted) row index of element 0 of this chunk
         float inv,
@@ -172,19 +186,19 @@ __device__ __forceinline__ void epi_filter32(
             float* dst = p.dump + (long long)q * p.dumpLd + colBase;
 #pragma unroll
             for (int j = 0; j < 32; j++)
-                dst[chunk_col(j)] = r[j];
+                dst[chunk_col(j)] = (float)r[j];
         }
         return;
     }
-    float mg[4];
+    T mg[4];
 #pragma unroll
     for (int g = 0; g < 4; g++) {
         const int o = 8 * g;
-        const float a = fmaxf(fmaxf(r[o + 0], r[o + 1]), fmaxf(r[o + 2], r[o + 3]));
-        const float c = fmaxf(fmaxf(r[o + 4], r[o + 5]), fmaxf(r[o + 6], r[o + 7]));
-        mg[g] = fmaxf(a, c);
+        const T a = tc_max(tc_max(r[o + 0], r[o + 1]), tc_max(r[o + 2], r[o + 3]));
+        const T c = tc_max(tc_max(r[o + 4], r[o + 5]), tc_max(r[o + 6], r[o + 7]));
+        mg[g] = tc_max(a, c);
     }
-    const float m = fmaxf(fmaxf(mg[0], mg[1]), fmaxf(mg[2], mg[3]));
+    const float m = (float)tc_max(tc_max(mg[0], mg[1]), tc_max(mg[2], mg[3]));
     if (SELF) {
         // the chunk's best row scores at least fma(m, inv, min bias of the tile) (monotone rounding, bias >= minb):
         // the running "best - 2 eps" threshold can be raised BEFORE any per-element work, so the slow path below
@@ -196,10 +210,10 @@ __device__ __forceinline__ void epi_filter32(
         const unsigned rowBase = (unsigned)colBase;
 #pragma unroll
         for (int g = 0; g < 4; g++) {
-            if (fmaf(mg[g], inv, maxb) > thr) {
+            if (fmaf((float)mg[g], inv, maxb) > thr) {
 #pragma unroll
                 for (int j = 8 * g; j < 8 * g + 8; j++) {
-                    const float v = fmaf(r[j], inv, __ldg(bias + chunk_col(j)));
+                    const float v = fmaf((float)r[j], inv, __ldg(bias + chunk_col(j)));
                     if (v > thr) {
                         emit(v, rowBase + chunk_col(j));
                         if (SELF) // k = 1: nothing scoring <= v - 2 eps can be the exact argmin any more
@@ -216,7 +230,9 @@ __device__ __forceinline__ void epi_filter32(
 // the candidates that beat it -- about ln(columns per thread) plus the near-ties of the maximum.
 // QUAD: tc_quad(p.KB, p.kSteps) holds, mapY's box is kHalfN rows, p.yStages == kMaxYStages and every ring stage holds one
 // half of a tile; the dynamic shared memory ends with kQuadCountBytes of segment counters.
-template <bool DUMP, bool SELF = false, bool QUAD = false>
+// S8 (QUAD, not SELF): int8 operands, 128 per swizzle row (one K-block: d <= 128), kS8Stages stages of 16 KB, four
+// m64n128k32 K-steps per half-tile, exact int32 accumulators, a per-query p.invQ in place of p.invScalePtr.
+template <bool DUMP, bool SELF = false, bool QUAD = false, bool S8 = false>
 __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
         const __grid_constant__ CUtensorMap mapQ,
         const __grid_constant__ CUtensorMap mapY,
@@ -227,9 +243,11 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
     unsigned char* smem = reinterpret_cast<unsigned char*>(
             (reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
     // QUAD runs at KB = 2 with kMaxYStages stages: compile-time sizes spare the consumers registers
-    const int KB = QUAD ? 2 : p.KB;
-    const int yStages = QUAD ? kMaxYStages : p.yStages;
-    const int qBytes = KB * kTileM * kKBlock * 2; // the query tile (128 rows)
+    static_assert(!S8 || (QUAD && !SELF), "int8 scoring runs the QUAD layout outside streaming mode");
+    constexpr int kStages = S8 ? kS8Stages : kMaxYStages; // barrier slots
+    const int KB = S8 ? 1 : QUAD ? 2 : p.KB;
+    const int yStages = QUAD ? kStages : p.yStages;
+    const int qBytes = KB * kTileM * kKBlock * 2; // the query tile (128 rows; S8: 128 rows x 128 s8)
     // one ring stage: a whole database tile (256 rows x dpad), or -- K-split mode, dpad > 128, where the query tile
     // plus several whole-tile stages no longer fit 227 KB -- one 64-wide K-block of it; QUAD: one 128-row half of a
     // tile, laid out [kblock][128 rows][64] like a whole tile (the K-block stride is 16 KB)
@@ -240,7 +258,7 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
     uint64_t* q_full = bars + 0;
     uint64_t* q_empty = bars + 1;
     uint64_t* y_full = bars + 2;
-    uint64_t* y_empty = y_full + kMaxYStages;
+    uint64_t* y_empty = y_full + kStages;
     // QUAD: 16-bit candidate counts of the unit's segments, behind the 512 bytes of barriers
     uint32_t* segCount = reinterpret_cast<uint32_t*>(reinterpret_cast<unsigned char*>(bars) + 512);
     const uint32_t sCounts = ptx::smem_u32(segCount);
@@ -309,17 +327,18 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
     const int h = QUAD ? (wg >> 1) : 0; // QUAD: column half of every tile (and of the ring)
     const int part = lane & 3;
     const int row = g * kWgM + (warp & 3) * 16 + (lane >> 2); // first of the thread's two rows; the second is row + 8
-    const float inv = *p.invScalePtr;
+    const float inv = S8 ? 0.f : *p.invScalePtr;
     const uint32_t sQaddr = ptx::smem_u32(sQ) + (uint32_t)(g * kWgM * kKBlock * 2); // this warpgroup's 64 rows
     const uint32_t sYaddr = ptx::smem_u32(sY);
     const int qkb = kTileM * kKBlock * 2; // bytes per K-block of the query tile
     const int ykb = kTileN * kKBlock * 2; // bytes per K-block of a database tile
     const int hkb = kHalfN * kKBlock * 2; // QUAD: bytes per K-block of a half-tile stage
     constexpr int kAcc = QUAD ? 64 : 128;
-    float acc[kAcc];
+    using Acc = std::conditional_t<S8, int, float>;
+    Acc acc[kAcc];
 #pragma unroll
     for (int i = 0; i < kAcc; i++)
-        acc[i] = 0.f;
+        acc[i] = 0;
     // QUAD: this warpgroup's sub-ring is stages h, h + 2, h + 4, ...
     int ys = h;
     uint32_t yphase = 0;
@@ -334,6 +353,8 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
         float thr1 = (!DUMP && q1 < p.nq) ? p.thr[q1] : CUDART_INF_F;
         const float slack0 = (SELF && q0 < p.nq) ? 2.f * p.eps[q0] : 0.f;
         const float slack1 = (SELF && q1 < p.nq) ? 2.f * p.eps[q1] : 0.f;
+        const float inv0 = S8 ? (!DUMP && q0 < p.nq ? p.invQ[q0] : 0.f) : inv;
+        const float inv1 = S8 ? (!DUMP && q1 < p.nq ? p.invQ[q1] : 0.f) : inv;
         SegmentWriter<QUAD> w0{p, u, sCounts, row * kParts + part};
         SegmentWriter<QUAD> w1{p, u, sCounts, (row + 8) * kParts + part};
         const int pb = p.tileBegin + sl * p.tilesPerSlice;
@@ -367,14 +388,14 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
             const long long colBase = (long long)tile * kTileN + kHalfN * (h + c) + 2 * part;
 #pragma unroll
             for (int hr = 0; hr < 2; hr++) {
-                float r[32];
+                Acc r[32];
 #pragma unroll
                 for (int e = 0; e < 32; e++)
                     r[e] = acc[4 * (16 * c + (e >> 1)) + 2 * hr + (e & 1)];
                 if (hr)
-                    epi_filter32<DUMP, SELF>(p, r, q1, colBase, inv, thr1, slack1, maxb, minb, w1);
+                    epi_filter32<DUMP, SELF>(p, r, q1, colBase, inv1, thr1, slack1, maxb, minb, w1);
                 else
-                    epi_filter32<DUMP, SELF>(p, r, q0, colBase, inv, thr0, slack0, maxb, minb, w0);
+                    epi_filter32<DUMP, SELF>(p, r, q0, colBase, inv0, thr0, slack0, maxb, minb, w0);
             }
         };
 
@@ -389,12 +410,21 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
                 const uint32_t yaddr = sYaddr + (uint32_t)ys * (uint32_t)stageBytes;
                 ptx::wgmma_fence_operands<64>(acc);
                 ptx::wgmma_fence(); // the accumulators were last read by the filter
+                if constexpr (S8) {
 #pragma unroll
-                for (int ks = 0; ks < 2 * kKBlock / 16; ks++) {
-                    const int kb = ks >> 2, k4 = ks & 3;
-                    const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + kb * qkb + k4 * 32);
-                    const uint64_t db = ptx::make_smem_desc_sw128(yaddr + kb * hkb + k4 * 32);
-                    ptx::wgmma_m64n128k16_f16_ss(acc, da, db, ks != 0 ? 1u : 0u);
+                    for (int ks = 0; ks < 4; ks++) { // 4 x k32 over the 128-byte row
+                        const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + ks * 32);
+                        const uint64_t db = ptx::make_smem_desc_sw128(yaddr + ks * 32);
+                        ptx::wgmma_m64n128k32_s8_ss(acc, da, db, ks != 0 ? 1u : 0u);
+                    }
+                } else {
+#pragma unroll
+                    for (int ks = 0; ks < 2 * kKBlock / 16; ks++) {
+                        const int kb = ks >> 2, k4 = ks & 3;
+                        const uint64_t da = ptx::make_smem_desc_sw128(sQaddr + kb * qkb + k4 * 32);
+                        const uint64_t db = ptx::make_smem_desc_sw128(yaddr + kb * hkb + k4 * 32);
+                        ptx::wgmma_m64n128k16_f16_ss(acc, da, db, ks != 0 ? 1u : 0u);
+                    }
                 }
                 ptx::wgmma_commit();
                 ptx::wgmma_wait_all();

@@ -50,7 +50,7 @@ struct FlatTcSchedule {
     int kFrac;        // ceil(k / nShards): the rows a shard must vouch for
     int LIST;         // base-list entries per query
     int KL;           // re-rank list size (pow2 >= k, >= 64)
-    bool useBisect;   // threshold selection by bisection (LIST <= 256), else sorted base lists
+    bool useBisect;   // threshold selection by bisection (fp16: LIST <= 256; int8: k <= 128), else sorted base lists
     bool streaming;   // k = 1 without sharding: one pass with self-tightening thresholds and a fused finish
     int64_t T;        // this database's tiles
     int64_t Tsched;   // tiles the rounds are laid out over (the largest shard's in a sharded search)
@@ -108,8 +108,11 @@ struct FlatTcSchedule {
 };
 
 // n database rows, k results per query, sms SMs.  shardRanks = 0: a plain search; otherwise a sharded search over
-// shardRanks ranks whose largest shard holds shardMaxTiles tiles.
-inline FlatTcSchedule planFlatTcSchedule(int64_t n, int k, int sms, int shardRanks = 0, int64_t shardMaxTiles = 0) {
+// shardRanks ranks whose largest shard holds shardMaxTiles tiles.  int8: the scores come from the int8 tensor cores,
+// whose certificate margin is about twice the fp16 one: more entries lie within 2 eps of the k-th best, so the base list
+// holds 4k entries instead of 2k.
+inline FlatTcSchedule planFlatTcSchedule(int64_t n, int k, int sms, int shardRanks = 0, int64_t shardMaxTiles = 0,
+                                         bool int8 = false) {
     FlatTcSchedule s;
     s.k = k;
     s.sms = sms;
@@ -122,7 +125,7 @@ inline FlatTcSchedule planFlatTcSchedule(int64_t n, int k, int sms, int shardRan
     s.nShards = sharded ? shardRanks : 1;
     s.Tsched = sharded ? std::max<int64_t>(s.T, shardMaxTiles) : s.T;
     s.kFrac = (k + s.nShards - 1) / s.nShards;
-    s.LIST = std::max(128, tcNextPow2(2 * k));
+    s.LIST = std::max(128, tcNextPow2((int8 ? 4 : 2) * k));
     s.KL = std::max(64, tcNextPow2(k));
 
     // tile permutation: multiplicative hash with a multiplier coprime to T
@@ -142,7 +145,7 @@ inline FlatTcSchedule planFlatTcSchedule(int64_t n, int k, int sms, int shardRan
         r0Tiles = std::max<int>((r0Tiles + s.nShards - 1) / s.nShards, std::max(2, (2 * s.kFrac + kTileN - 1) / kTileN));
     // threshold selection by bisection (no sorted lists) holds kSelCap entries per query and round: the all-pass first
     // round is sized to 3/4 of that
-    s.useBisect = s.LIST <= 256;
+    s.useBisect = int8 ? k <= 128 : s.LIST <= 256;
     if (s.useBisect)
         r0Tiles = std::min(r0Tiles, std::max(2, kSelCap * 3 / 4 / kTileN));
     s.r0Tiles = r0Tiles;

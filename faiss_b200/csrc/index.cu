@@ -590,6 +590,7 @@ void GpuIndexFlat::search(idx_t n, const float* x, idx_t k, float* distances, id
 void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
     auto stream = stream_();
     lastSearchUsedTensorCores = 0;
+    lastSearchOperandBits = 0;
     if (this->ntotal == 0) {
         fillEmpty_(n, k, dDev, iDev);
         return;
@@ -614,6 +615,7 @@ void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, i
         tc_.prepare(rows_(), this->ntotal, searchMetric_(), yHalf_(), stream);
         lastSearchFallbackQueries += (int)tc_.search(xDev, n, k, dDev, iDev, stream, nullptr, mask);
         lastSearchUsedTensorCores = 1;
+        lastSearchOperandBits = tc_.lastOperandBits();
     } else {
         runFlatExact(
                 resources_.get(), config_.device, xDev, n, rows_(), this->ntotal, d, k, searchMetric_(), 0, dDev, iDev,
@@ -639,6 +641,7 @@ void GpuIndexFlat::searchShardDevice(idx_t n, const float* xDev, int k, float* d
     xDev = roundedQueries_(n, xDev, qHold);
     lastSearchFallbackQueries = (int)tc_.search(xDev, n, k, dDev, iDev, stream, flatShard);
     lastSearchUsedTensorCores = 1;
+    lastSearchOperandBits = tc_.lastOperandBits();
 }
 
 void GpuIndexFlat::reconstruct(idx_t key, float* out) const {

@@ -210,6 +210,7 @@ class GpuIndexFlat : public GpuIndex {
     // diagnostics of the last search (fallback queries: exact recomputes, summed over the whole call)
     mutable int lastSearchUsedTensorCores = 0;
     mutable int lastSearchFallbackQueries = 0;
+    mutable int lastSearchOperandBits = 0; // tensor-core operand width of the last search: 8 or 16; 0: exact kernel
 
    protected:
     bool addImplRequiresIDs_() const override {

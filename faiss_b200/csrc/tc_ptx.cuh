@@ -137,6 +137,12 @@ __device__ __forceinline__ void wgmma_fence_operands(float* d) {
     for (int i = 0; i < N; i++)
         asm volatile("" : "+f"(d[i])::"memory");
 }
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operands(int* d) {
+#pragma unroll
+    for (int i = 0; i < N; i++)
+        asm volatile("" : "+r"(d[i])::"memory");
+}
 // D[64 x 256, registers] (+)= A[smem desc, 64 x 16] * B[smem desc, 256 x 16]^T, fp16 inputs, fp32 accumulate,
 // both operands K-major.  Fragment of D held by thread t of the warpgroup (warp w = t / 32, lane l):
 //   d[4 j + 2 h + b] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + b]   (j < 32, h, b < 2)
@@ -194,6 +200,29 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16_ss(float* d, uint64_t desc_
               "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
               "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
               "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
+// D[64 x 128, registers] (+)= A[smem desc, 64 x 32] * B[smem desc, 128 x 32]^T, s8 inputs, exact s32 accumulate, both
+// operands K-major (32 s8 = 32 bytes per K-step, the same stride as an fp16 k16 step).  Same fragment layout as above.
+// Integer wgmma takes no scale or transpose immediates.
+__device__ __forceinline__ void wgmma_m64n128k32_s8_ss(int* d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %66, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+            "%64, %65, p;\n"
+            "}\n"
+            : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+              "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+              "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+              "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+              "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+              "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+              "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+              "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
             : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 

@@ -124,6 +124,8 @@ FB200_API int faiss_GpuIndexFlat_setUseTensorCores(FaissGpuIndex* index, int ena
 /* diagnostics of the last search on this index: out[0] = tensor-core path used, out[1] = queries
    recomputed by the exact kernel because their certificate failed */
 FB200_API int faiss_GpuIndexFlat_lastSearchInfo(const FaissGpuIndex* index, int* out2);
+/* operand width of the last search's tensor-core scoring: 8 (int8), 16 (fp16), or 0 when it ran the exact kernel */
+FB200_API int faiss_GpuIndexFlat_lastSearchOperandBits(const FaissGpuIndex* index, int* bits);
 
 /* ---- GpuIndexIVF (faiss/gpu/GpuIndexIVF.h:40-167) ---- */
 FB200_API int faiss_GpuIndexIVF_set_nprobe(FaissGpuIndex* index, size_t nprobe);
@@ -319,6 +321,8 @@ FB200_API int b200_flat_search_exact(FaissStandardGpuResources* res, int device,
 FB200_API int b200_topk_merge(FaissStandardGpuResources* res, int device, const float* D_in, const idx_t* I_in, idx_t nq, int nshard, int k_in, const idx_t* id_offsets /* device, [nshard] or NULL */, int k, FaissMetricType metric, float* D, idx_t* I);
 /* unit-test seam for the tensor-core path: S[nq, roundup(N,256)] = Q16 . Y16^T (fp16 inputs) */
 FB200_API int b200_flat_tc_scores_debug(FaissStandardGpuResources* res, int device, const void* Q16, idx_t nq, const void* Y16, idx_t N, int dpad, float* S);
+/* the same for int8 rows of 128: S = the exact int32 dot products Q8 . Y8^T, as floats */
+FB200_API int b200_flat_tc_scores_debug_s8(FaissStandardGpuResources* res, int device, const void* Q8, idx_t nq, const void* Y8, idx_t N, float* S);
 /* role of IVFBase::searchCoarseQuantizer_ (faiss/gpu/impl/IVFBase.cu:509-545): nprobe nearest centroids per query */
 FB200_API int b200_ivf_coarse(FaissStandardGpuResources* res, int device, const float* centroids, idx_t nlist, int d, const float* Q, idx_t nq, int nprobe, FaissMetricType metric, float* coarse_dis, idx_t* coarse_ids);
 /* role of Clustering's index.search(n, x, 1) (faiss/Clustering.cpp:270-290): nearest centroid of every point */
