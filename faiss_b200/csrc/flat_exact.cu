@@ -193,8 +193,15 @@ struct OpGower {
     __device__ static float finish(const Acc& a, float) { return a.a / a.b; }
 };
 
+// What a CTA does with its distance tile:
+//   List    offer it to per-query shared-memory top-k lists (k > 1)
+//   Argmin  keep the best (key, row) per query with a packed atomicMin (k = 1)
+//   Store   write every Op::finish value to D[q * ldD + row] (all-pairs distances, no selection, no lists);
+//           the raw distance, not the key, and NaN as computed
+enum class Epi { List, Argmin, Store };
+
 // MASK: only rows whose bit is set in rowMask (bit r & 31 of word r >> 5) enter the results (SearchParameters::sel)
-template <int TQ, int TN, class Op, bool K1, bool MASK>
+template <int TQ, int TN, class Op, Epi E, bool MASK>
 __global__ void __launch_bounds__(256) flat_exact_kernel(
         const float* __restrict__ Q,
         int nq,
@@ -206,10 +213,13 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
         int LIST,
         int64_t rowsPerSplit,
         float arg,                  // metric_arg (the exponent of METRIC_Lp)
-        float* __restrict__ partD,  // [nq, nsplit, k]   keys ("smaller is better")
+        float* __restrict__ partD,  // [nq, nsplit, k]   keys ("smaller is better"); Store: D [nq][ldD]
         idx_t* __restrict__ partI,  // [nq, nsplit, k]   row index (or -1)
-        const uint32_t* __restrict__ rowMask)
+        const uint32_t* __restrict__ rowMask,
+        int64_t ldD)
 {
+    constexpr bool K1 = E == Epi::Argmin;
+    constexpr bool STORE = E == Epi::Store;
     using C = ExactCfg<TQ, TN>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* Qs = reinterpret_cast<float*>(smem_raw);            // [kDK][QS]
@@ -218,7 +228,7 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
     float* thrS = reinterpret_cast<float*>(cntS + TQ);         // [TQ]
     unsigned long long* best = reinterpret_cast<unsigned long long*>(thrS + TQ); // [TQ] (K1)
     unsigned char* listBase = reinterpret_cast<unsigned char*>(best + TQ);
-    const size_t perQuery = K1 ? 0 : SmemTopK<int>::bytes(LIST, C::BUF);
+    const size_t perQuery = E == Epi::List ? SmemTopK<int>::bytes(LIST, C::BUF) : 0;
 
     const int tid = threadIdx.x;
     const int tx = tid % C::TXN;
@@ -243,12 +253,12 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
         return s;
     };
 
-    if (tid < TQ) {
+    if (!STORE && tid < TQ) {
         cntS[tid] = 0;
         thrS[tid] = CUDART_INF_F;
         best[tid] = ~0ull;
     }
-    if (!K1) {
+    if (E == Epi::List) {
         for (int q = warp; q < TQ; q += 8) {
             SmemTopK<int> s = queueOf(q);
             s.init();
@@ -351,60 +361,84 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
             __syncthreads();
         }
 
-        // ---- offer the tile to the per-query lists
+        if constexpr (STORE) {
+            // this thread's 4 consecutive rows of each of its query rows: one 16-byte streaming store when the
+            // 4 are in range and D's rows keep 16-byte alignment (nb - r0 and tx * 4 are multiples of 4)
+            const int64_t c0 = nb + tx * 4;
+            const bool vecStore = (ldD & 3) == 0 && (reinterpret_cast<uintptr_t>(partD) & 15) == 0 && c0 + 3 < r1;
 #pragma unroll
-        for (int r = 0; r < C::RQ; r++) {
-            const int q = ty * C::RQ + r;
-            if (q0 + q >= nq)
-                continue;
-            if (K1) {
-                unsigned long long mine = ~0ull;
+            for (int r = 0; r < C::RQ; r++) {
+                const int q = ty * C::RQ + r;
+                if (q0 + q >= nq)
+                    continue;
+                float* out = partD + (int64_t)(q0 + q) * ldD + c0;
+                if (vecStore) {
+                    __stcs(reinterpret_cast<float4*>(out),
+                           make_float4(Op::finish(acc[r][0], arg), Op::finish(acc[r][1], arg), Op::finish(acc[r][2], arg),
+                                       Op::finish(acc[r][3], arg)));
+                } else {
 #pragma unroll
-                for (int c = 0; c < 4; c++) {
-                    int64_t row = nb + tx * 4 + c;
-                    if (row < r1 && (!MASK || ((rowMask[row >> 5] >> (row & 31)) & 1u))) {
+                    for (int c = 0; c < 4; c++)
+                        if (c0 + c < r1)
+                            __stcs(out + c, Op::finish(acc[r][c], arg));
+                }
+            }
+        } else {
+            // ---- offer the tile to the per-query lists
+#pragma unroll
+            for (int r = 0; r < C::RQ; r++) {
+                const int q = ty * C::RQ + r;
+                if (q0 + q >= nq)
+                    continue;
+                if (K1) {
+                    unsigned long long mine = ~0ull;
+#pragma unroll
+                    for (int c = 0; c < 4; c++) {
+                        int64_t row = nb + tx * 4 + c;
+                        if (row < r1 && (!MASK || ((rowMask[row >> 5] >> (row & 31)) & 1u))) {
+                            const float dist = Op::finish(acc[r][c], arg);
+                            float key = Op::kSimilarity ? -dist : dist;
+                            if (key == key && (!Op::kSentinel || key < FLT_MAX)) { // NaN never wins
+                                unsigned long long p =
+                                        ((unsigned long long)float_to_ordered(key) << 32) | (unsigned)(row - r0);
+                                mine = min(mine, p);
+                            }
+                        }
+                    }
+                    if (mine < best[q])
+                        atomicMin(&best[q], mine);
+                } else {
+                    const float thr = thrS[q];
+                    SmemTopK<int> s = queueOf(q);
+#pragma unroll
+                    for (int c = 0; c < 4; c++) {
+                        int64_t row = nb + tx * 4 + c;
                         const float dist = Op::finish(acc[r][c], arg);
                         float key = Op::kSimilarity ? -dist : dist;
-                        if (key == key && (!Op::kSentinel || key < FLT_MAX)) { // NaN never wins
-                            unsigned long long p =
-                                    ((unsigned long long)float_to_ordered(key) << 32) | (unsigned)(row - r0);
-                            mine = min(mine, p);
+                        if (row < r1 && key <= thr && (!Op::kSentinel || key < FLT_MAX) &&
+                            (!MASK || ((rowMask[row >> 5] >> (row & 31)) & 1u))) {
+                            int pos = atomicAdd(&cntS[q], 1);
+                            s.keys[LIST + pos] = key;
+                            s.ids[LIST + pos] = (int)(row - r0);
                         }
                     }
                 }
-                if (mine < best[q])
-                    atomicMin(&best[q], mine);
-            } else {
-                const float thr = thrS[q];
-                SmemTopK<int> s = queueOf(q);
-#pragma unroll
-                for (int c = 0; c < 4; c++) {
-                    int64_t row = nb + tx * 4 + c;
-                    const float dist = Op::finish(acc[r][c], arg);
-                    float key = Op::kSimilarity ? -dist : dist;
-                    if (row < r1 && key <= thr && (!Op::kSentinel || key < FLT_MAX) &&
-                        (!MASK || ((rowMask[row >> 5] >> (row & 31)) & 1u))) {
-                        int pos = atomicAdd(&cntS[q], 1);
-                        s.keys[LIST + pos] = key;
-                        s.ids[LIST + pos] = (int)(row - r0);
+            }
+            if (!K1) {
+                __syncthreads();
+                for (int q = warp; q < TQ; q += 8) {
+                    int c = cntS[q];
+                    if (c > TN) {
+                        SmemTopK<int> s = queueOf(q);
+                        s.flush(c);
+                        if (lane_id() == 0) {
+                            cntS[q] = 0;
+                            thrS[q] = s.threshold();
+                        }
                     }
                 }
+                __syncthreads();
             }
-        }
-        if (!K1) {
-            __syncthreads();
-            for (int q = warp; q < TQ; q += 8) {
-                int c = cntS[q];
-                if (c > TN) {
-                    SmemTopK<int> s = queueOf(q);
-                    s.flush(c);
-                    if (lane_id() == 0) {
-                        cntS[q] = 0;
-                        thrS[q] = s.threshold();
-                    }
-                }
-            }
-            __syncthreads();
         }
     }
 
@@ -422,7 +456,7 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
                 partI[o] = r0 + (int64_t)(unsigned)(b & 0xffffffffu);
             }
         }
-    } else {
+    } else if (E == Epi::List) {
         for (int q = warp; q < TQ; q += 8) {
             if (q0 + q >= nq)
                 continue;
@@ -590,7 +624,7 @@ void runMergeTopKKeyspace(
 // ------------------------------------------------------------------------------------------
 // host driver
 // ------------------------------------------------------------------------------------------
-template <int TQ, int TN, bool K1>
+template <int TQ, int TN, Epi E>
 static void launchExact(
         const float* Q,
         int64_t nq,
@@ -607,22 +641,28 @@ static void launchExact(
         float* partD,
         idx_t* partI,
         const uint32_t* rowMask,
-        cudaStream_t stream) {
+        cudaStream_t stream,
+        int64_t ldD = 0) {
     using C = ExactCfg<TQ, TN>;
-    size_t smem = sizeof(float) * kDK * (C::QS + C::YS) + TQ * (sizeof(int) + sizeof(float) + sizeof(unsigned long long));
-    if (!K1)
+    size_t smem = sizeof(float) * kDK * (C::QS + C::YS);
+    if (E != Epi::Store)
+        smem += TQ * (sizeof(int) + sizeof(float) + sizeof(unsigned long long));
+    if (E == Epi::List)
         smem += SmemTopK<int>::bytes(LIST, C::BUF) * TQ;
     dim3 grid((unsigned)ceil_div(nq, TQ), (unsigned)nsplit);
     auto launch = [&](auto kern) {
         CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, C::kThreads, smem, stream>>>(Q, (int)nq, Y, yHalf, n, d, k, LIST, rowsPerSplit, metricArg, partD, partI, rowMask);
+        kern<<<grid, C::kThreads, smem, stream>>>(
+                Q, (int)nq, Y, yHalf, n, d, k, LIST, rowsPerSplit, metricArg, partD, partI, rowMask, ldD);
     };
     auto launchOp = [&](auto op) {
         using Op = decltype(op);
-        if (rowMask)
-            launch(flat_exact_kernel<TQ, TN, Op, K1, true>);
+        if constexpr (E == Epi::Store)
+            launch(flat_exact_kernel<TQ, TN, Op, E, false>);
+        else if (rowMask)
+            launch(flat_exact_kernel<TQ, TN, Op, E, true>);
         else
-            launch(flat_exact_kernel<TQ, TN, Op, K1, false>);
+            launch(flat_exact_kernel<TQ, TN, Op, E, false>);
     };
     // METRIC_Lp arrives here with p != 1, 2: GpuIndexFlat::searchMetric_ sends those to L1 / L2
     switch (metric) {
@@ -660,6 +700,18 @@ static void launchExact(
             FB_THROW_FMT("unimplemented metric type %d", (int)metric); // faiss/gpu/impl/Distance.cuh:289
     }
     CUDA_CHECK_LAST();
+}
+
+// database split (gridDim.y): enough blocks to fill the chip (2 waves), slices of >= 8 tiles, < 2^31 rows
+static void databaseSplit(int64_t ctas, int64_t nq, int TQ, int64_t n, int TN, int64_t& nsplit, int64_t& rowsPerSplit) {
+    int64_t qTiles = ceil_div(nq, TQ);
+    int64_t wantSplit = std::max<int64_t>(1, (ctas + qTiles - 1) / qTiles);
+    int64_t maxSplit = std::max<int64_t>(1, n / (8 * TN));
+    nsplit = std::min(wantSplit, maxSplit);
+    nsplit = std::max(nsplit, ceil_div(n, (int64_t(1) << 30)));
+    nsplit = std::min<int64_t>(nsplit, 65535);
+    rowsPerSplit = n > 0 ? round_up(ceil_div(n, nsplit), TN) : TN;
+    nsplit = n > 0 ? ceil_div(n, rowsPerSplit) : 1;
 }
 
 static void flatExactImpl(
@@ -707,31 +759,23 @@ static void flatExactImpl(
             LIST = p2;
         }
     }
-    // database split: enough blocks to fill the chip (2 waves), slices of >= 8 tiles, < 2^31 rows
-    int sms = res->numSMs(device);
-    int64_t qTiles = ceil_div(nq, TQ);
-    int64_t wantSplit = std::max<int64_t>(1, (2 * sms + qTiles - 1) / qTiles);
-    int64_t maxSplit = std::max<int64_t>(1, n / (8 * TN));
-    int64_t nsplit = std::min(wantSplit, maxSplit);
-    nsplit = std::max(nsplit, ceil_div(n, (int64_t(1) << 30)));
-    nsplit = std::min<int64_t>(nsplit, 65535);
-    int64_t rowsPerSplit = n > 0 ? round_up(ceil_div(n, nsplit), TN) : TN;
-    nsplit = n > 0 ? ceil_div(n, rowsPerSplit) : 1;
+    int64_t nsplit, rowsPerSplit;
+    databaseSplit(2 * res->numSMs(device), nq, TQ, n, TN, nsplit, rowsPerSplit);
 
     auto partD = res->temp(device, sizeof(float) * nq * nsplit * k);
     auto partI = res->temp(device, sizeof(idx_t) * nq * nsplit * k);
 
-#define LAUNCH(TQ_, TN_, K1_)                                                                        \
-    launchExact<TQ_, TN_, K1_>(                                                                      \
+#define LAUNCH(TQ_, TN_, E_)                                                                         \
+    launchExact<TQ_, TN_, E_>(                                                                       \
             Q, nq, Y, yHalf, n, d, k, LIST, metric, metricArg, (int)nsplit, rowsPerSplit, partD.as<float>(), partI.as<idx_t>(), rowMask, stream)
     if (K1) {
-        LAUNCH(32, 64, true);
+        LAUNCH(32, 64, Epi::Argmin);
     } else if (TQ == 32) {
-        LAUNCH(32, 64, false);
+        LAUNCH(32, 64, Epi::List);
     } else if (TQ == 16) {
-        LAUNCH(16, 64, false);
+        LAUNCH(16, 64, Epi::List);
     } else {
-        LAUNCH(8, 128, false);
+        LAUNCH(8, 128, Epi::List);
     }
 #undef LAUNCH
     runMergeTopKKeyspace(
@@ -778,6 +822,31 @@ void runFlatArgmin(
         outD = tmp.as<float>();
     }
     flatExactImpl(res, device, Q, nq, Y, 0, n, d, 1, metric, 0.f, 0, outD, outI, nullptr, stream);
+}
+
+void runFlatPairwise(
+        GpuResources* res,
+        int device,
+        const float* Q,
+        int64_t nq,
+        const float* Y,
+        int64_t n,
+        int d,
+        MetricType metric,
+        float metricArg,
+        float* D,
+        int64_t ldD,
+        cudaStream_t stream) {
+    if (!is_implemented_metric(metric))
+        FB_THROW_FMT("unimplemented metric type %d", (int)metric);
+    if (nq == 0 || n == 0)
+        return;
+    FB_THROW_IF_NOT_MSG(nq < (int64_t(1) << 31), "too many queries in one call");
+    // every CTA does the same work, so a split finer than the k-NN's keeps the last wave's imbalance small
+    int64_t nsplit, rowsPerSplit;
+    databaseSplit(32 * res->numSMs(device), nq, 32, n, 64, nsplit, rowsPerSplit);
+    launchExact<32, 64, Epi::Store>(
+            Q, nq, Y, 0, n, d, 0, 0, metric, metricArg, (int)nsplit, rowsPerSplit, D, nullptr, nullptr, stream, ldD);
 }
 
 // ------------------------------------------------------------------------------------------

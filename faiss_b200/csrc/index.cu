@@ -42,51 +42,6 @@ void validateNProbe(size_t nprobe) {
             nprobe);
 }
 
-// RAII: a pointer that is guaranteed device-resident on `device` (copies host data in)
-template <typename T>
-struct DeviceView {
-    DeviceView(GpuResources* res, int device, const T* p, size_t count, cudaStream_t stream) {
-        if (!p || count == 0) {
-            ptr = nullptr;
-            return;
-        }
-        int dev = getDeviceForAddress(p);
-        if (dev == device) {
-            ptr = p;
-        } else {
-            hold = res->temp(device, count * sizeof(T));
-            CUDA_VERIFY(cudaMemcpyAsync(hold.data, p, count * sizeof(T), cudaMemcpyDefault, stream));
-            ptr = hold.as<T>();
-        }
-    }
-    const T* ptr;
-    GpuMemoryReservation hold;
-};
-
-// output staging: device buffer that is copied back to a host pointer on `finish`
-template <typename T>
-struct DeviceOut {
-    DeviceOut(GpuResources* res, int device, T* p, size_t count) : user(p), n(count) {
-        int dev = getDeviceForAddress(p);
-        if (dev == device) {
-            ptr = p;
-        } else {
-            hold = res->temp(device, count * sizeof(T));
-            ptr = hold.as<T>();
-            staged = true;
-        }
-    }
-    void finish(cudaStream_t stream) {
-        if (staged)
-            CUDA_VERIFY(cudaMemcpyAsync(user, ptr, n * sizeof(T), cudaMemcpyDefault, stream));
-    }
-    T* user;
-    T* ptr;
-    size_t n;
-    bool staged = false;
-    GpuMemoryReservation hold;
-};
-
 __global__ void iota_ids_kernel(idx_t* out, idx_t n, idx_t base) {
     idx_t i = (idx_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n)
@@ -529,21 +484,22 @@ void GpuIndexFlat::replaceVectorsDevice(idx_t n, const float* xDev) {
             addImpl_(n, xDev, nullptr);
         return;
     }
-    vecs_.resize((size_t)n * d, stream); // keeps the allocation when it is large enough
+    float* rows = resizeVectorsDevice(n);
     if (n > 0)
-        CUDA_VERIFY(cudaMemcpyAsync(vecs_.data(), xDev, sizeof(float) * n * d, cudaMemcpyDeviceToDevice, stream));
-    this->ntotal = n;
-    tc_.invalidate();
+        CUDA_VERIFY(cudaMemcpyAsync(rows, xDev, sizeof(float) * n * d, cudaMemcpyDeviceToDevice, stream));
 }
 
-// faiss/gpu/impl/Distance.cuh:223-239.  The reference GPU's p = -1 -> L2 branch is a test hook; the CPU sums
-// |a-b|^-1 there, and so does the Lp kernel.
+float* GpuIndexFlat::resizeVectorsDevice(idx_t n) {
+    FB_THROW_IF_NOT_MSG(!flatConfig_.useFloat16, "fp32 row access on a float16 GpuIndexFlat");
+    DeviceScope scope(config_.device);
+    vecs_.resize((size_t)n * d, stream_()); // keeps the allocation when it is large enough
+    this->ntotal = n;
+    tc_.invalidate();
+    return vecs_.data();
+}
+
 MetricType GpuIndexFlat::searchMetric_() const {
-    if (metric_type == METRIC_Lp && metric_arg == 1.f)
-        return METRIC_L1;
-    if (metric_type == METRIC_Lp && metric_arg == 2.f)
-        return METRIC_L2;
-    return metric_type;
+    return flatKernelMetric(metric_type, metric_arg);
 }
 
 // faiss/gpu/impl/Distance.cu:152-164: fill with "no result"

@@ -207,6 +207,9 @@ class GpuIndexFlat : public GpuIndex {
     // replace the whole content by n device rows without giving the storage back (the k-means loop installs a new
     // centroid table every iteration: reset() + add() would free and re-allocate five buffers each time)
     void replaceVectorsDevice(idx_t n, const float* xDev);
+    // the fp32 storage resized to n rows, contents undefined, for the caller to fill on the default stream (bfKnn
+    // converts fp16 / bf16 / column-major vectors straight into it); not available under useFloat16
+    float* resizeVectorsDevice(idx_t n);
     // diagnostics of the last search (fallback queries: exact recomputes, summed over the whole call)
     mutable int lastSearchUsedTensorCores = 0;
     mutable int lastSearchFallbackQueries = 0;

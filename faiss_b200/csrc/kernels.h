@@ -55,6 +55,35 @@ void runFlatArgmin(
         idx_t* outI,
         cudaStream_t stream);
 
+// All-pairs distances with the arithmetic of runFlatExact (role of allPairwiseDistanceOnDevice,
+// faiss/gpu/impl/Distance.cuh:167-292): D[i * ldD + j] = distance(Q[i], Y[j]) for i < nq, j < n, the value the
+// k-NN path returns for that pair, bit for bit.  Inner product and Jaccard are the raw similarity; NaN is written
+// as computed.  `metric` is what the kernel runs: METRIC_Lp with p = 1 / 2 is mapped by flatKernelMetric first.
+void runFlatPairwise(
+        GpuResources* res,
+        int device,
+        const float* Q,
+        int64_t nq,
+        const float* Y,
+        int64_t n,
+        int d,
+        MetricType metric,
+        float metricArg,
+        float* D,
+        int64_t ldD,
+        cudaStream_t stream);
+
+// the metric the exact kernel runs for (metric, metricArg): METRIC_Lp with p = 1 is L1 and with p = 2 is L2
+// (faiss/gpu/impl/Distance.cuh:223-239); the reference GPU's p = -1 -> L2 branch is a test hook, and the CPU sums
+// |a-b|^-1 there, as the Lp kernel does
+inline MetricType flatKernelMetric(MetricType metric, float metricArg) {
+    if (metric == METRIC_Lp && metricArg == 1.f)
+        return METRIC_L1;
+    if (metric == METRIC_Lp && metricArg == 2.f)
+        return METRIC_L2;
+    return metric;
+}
+
 // Row-wise top-k over candidate lists (role of runBlockSelectPair / merge_knn_results,
 // faiss/gpu/utils/BlockSelectFloat.cu:98, faiss/utils/Heap.cpp:166-238).
 //   inD/inI: [rows, nlists, kin]; ids == -1 are skipped; idOffsets (optional, [nlists]) is added to

@@ -235,6 +235,51 @@ struct DeviceScope {
 // -1 if host pointer, else device ordinal (faiss/gpu/utils/DeviceUtils.h:64)
 int getDeviceForAddress(const void* p);
 
+// RAII: a pointer that is guaranteed device-resident on `device` (copies host data in)
+template <typename T>
+struct DeviceView {
+    DeviceView(GpuResources* res, int device, const T* p, size_t count, cudaStream_t stream) {
+        if (!p || count == 0) {
+            ptr = nullptr;
+            return;
+        }
+        int dev = getDeviceForAddress(p);
+        if (dev == device) {
+            ptr = p;
+        } else {
+            hold = res->temp(device, count * sizeof(T));
+            CUDA_VERIFY(cudaMemcpyAsync(hold.data, p, count * sizeof(T), cudaMemcpyDefault, stream));
+            ptr = hold.as<T>();
+        }
+    }
+    const T* ptr;
+    GpuMemoryReservation hold;
+};
+
+// output staging: device buffer that is copied back to a host pointer on `finish`
+template <typename T>
+struct DeviceOut {
+    DeviceOut(GpuResources* res, int device, T* p, size_t count) : user(p), n(count) {
+        int dev = getDeviceForAddress(p);
+        if (dev == device) {
+            ptr = p;
+        } else {
+            hold = res->temp(device, count * sizeof(T));
+            ptr = hold.as<T>();
+            staged = true;
+        }
+    }
+    void finish(cudaStream_t stream) {
+        if (staged)
+            CUDA_VERIFY(cudaMemcpyAsync(user, ptr, n * sizeof(T), cudaMemcpyDefault, stream));
+    }
+    T* user;
+    T* ptr;
+    size_t n;
+    bool staged = false;
+    GpuMemoryReservation hold;
+};
+
 // ------------------------------------------------------------------------------------------
 // growable device array backed by GpuResources (role of DeviceVector, faiss/gpu/utils/DeviceVector.cuh)
 // ------------------------------------------------------------------------------------------

@@ -293,11 +293,57 @@ FB200_API int faiss_b200_kmeans_sharded(FaissStandardGpuResources* res, int devi
 FB200_API int faiss_b200_pq_train(FaissStandardGpuResources* res, int device, size_t d, size_t M, size_t n, const float* x, int niter, int seed, float* centroids_out);
 
 /* bfKnn (faiss/gpu/GpuDistance.h:33-181): brute-force k-NN of `queries` in `vectors` (both row-major fp32, host or
-   device), any metric GpuIndexFlat takes; outputs host or device.  (Column-major inputs, fp16/bf16 vectors and
-   bfKnn_tiling are not on the path.) */
+   device), any metric GpuIndexFlat takes; outputs host or device.  fp16 / bf16 and column-major inputs, int32 ids,
+   all pairwise distances (k = -1) and tiling: faiss_b200_bfKnn_params / faiss_b200_bfKnn_tiling below. */
 FB200_API int faiss_b200_bfKnn(FaissStandardGpuResources* res, int device, FaissMetricType metric, idx_t k, int dims, const float* vectors, idx_t num_vectors, const float* queries, idx_t num_queries, float* out_distances, idx_t* out_indices);
 /* the same with GpuDistanceParams::metricArg (faiss/gpu/GpuDistance.h:41), the exponent of METRIC_Lp */
 FB200_API int faiss_b200_bfKnn_ex(FaissStandardGpuResources* res, int device, FaissMetricType metric, float metric_arg, idx_t k, int dims, const float* vectors, idx_t num_vectors, const float* queries, idx_t num_queries, float* out_distances, idx_t* out_indices);
+
+/* faiss::gpu::DistanceDataType / IndicesDataType (faiss/gpu/GpuDistance.h:18-29), same values */
+typedef enum FaissDistanceDataType {
+    FaissDistanceDataType_F32 = 1,
+    FaissDistanceDataType_F16 = 2,
+    FaissDistanceDataType_BF16 = 3
+} FaissDistanceDataType;
+typedef enum FaissIndicesDataType {
+    FaissIndicesDataType_I64 = 1,
+    FaissIndicesDataType_I32 = 2
+} FaissIndicesDataType;
+
+/* faiss::gpu::GpuDistanceParams (faiss/gpu/GpuDistance.h:32-152): the reference's field names, in its order, for the
+   fields implemented here (no vectorNorms, ignoreOutDistances, use_cuvs; device is an ordinal, not -1).
+   - k in [1, 2048]: k-NN, outDistances / outIndices [numQueries][k].  k = -1: all pairwise distances,
+     outDistances [numQueries][numVectors], outIndices unused.  Every distance is the one GpuIndexFlat returns, bit for
+     bit (a direct-form sum in dimension order, no ||x||^2 + ||y||^2 - 2<x, y> expansion); for inner product and
+     Jaccard the raw similarity; NaN as the CPU computes it.
+   - vectorType == queryType is required.  fp16 / bf16 inputs are widened to fp32 exactly on the device.
+   - *RowMajor = 0: the input is [dims][num], num innermost.
+   - outIndicesType I32 is refused when numVectors > INT32_MAX (the reference narrows silently).
+   - Any pointer may be host or device resident.  A host-resident k = -1 matrix is computed in blocks of <= 256 MiB. */
+typedef struct FaissGpuDistanceParams {
+    FaissMetricType metric;
+    float metricArg;
+    int k;
+    int dims;
+    const void* vectors;
+    FaissDistanceDataType vectorType;
+    int vectorsRowMajor;
+    idx_t numVectors;
+    const void* queries;
+    FaissDistanceDataType queryType;
+    int queriesRowMajor;
+    idx_t numQueries;
+    float* outDistances;
+    FaissIndicesDataType outIndicesType;
+    void* outIndices;
+    int device;
+} FaissGpuDistanceParams;
+/* faiss::gpu::bfKnn(res, params).  Arguments are validated before any CUDA call: -2 with a message. */
+FB200_API int faiss_b200_bfKnn_params(FaissStandardGpuResources* res, const FaissGpuDistanceParams* params);
+/* faiss::gpu::bfKnn_tiling (faiss/gpu/GpuDistance.cu:457-570): vectors / queries cut into shards of at most
+   vectorsMemoryLimit / queriesMemoryLimit bytes (0: no limit).  The sharded input must be host-resident and row-major,
+   k > 0.  The result equals faiss_b200_bfKnn_params's bit for bit. */
+FB200_API int faiss_b200_bfKnn_tiling(FaissStandardGpuResources* res, const FaissGpuDistanceParams* params, size_t vectorsMemoryLimit, size_t queriesMemoryLimit);
 
 /* ---- instrumentation (bench.py): kernels launched by this library so far; optional CUDA-event
    timing of a named kernel ("flat_tc") on its launching stream ---- */
@@ -317,6 +363,8 @@ FB200_API int faiss_b200_merge_knn_results_host(idx_t n, idx_t k, int nshard, Fa
 FB200_API int b200_l2_norms(FaissStandardGpuResources* res, int device, const float* x, idx_t n, int d, float* norms);
 /* role of bfKnnOnDevice (faiss/gpu/impl/Distance.cuh:300), exact SIMT arithmetic */
 FB200_API int b200_flat_search_exact(FaissStandardGpuResources* res, int device, const float* Y, idx_t N, int d, const float* Q, idx_t nq, int k, FaissMetricType metric, float* D, idx_t* I);
+/* faiss_b200_bfKnn_params for k = -1 into a host-resident matrix, with a block budget of page_bytes instead of 256 MiB */
+FB200_API int b200_pairwise_paged(FaissStandardGpuResources* res, const FaissGpuDistanceParams* params, size_t page_bytes);
 /* role of merge_knn_results (faiss/utils/Heap.cpp:166-238) on the device: in [nq, nshard, k] */
 FB200_API int b200_topk_merge(FaissStandardGpuResources* res, int device, const float* D_in, const idx_t* I_in, idx_t nq, int nshard, int k_in, const idx_t* id_offsets /* device, [nshard] or NULL */, int k, FaissMetricType metric, float* D, idx_t* I);
 /* unit-test seam for the tensor-core path: S[nq, roundup(N,256)] = Q16 . Y16^T (fp16 inputs) */
