@@ -1032,8 +1032,8 @@ constexpr int kMaxKB = 4; // d <= 256: the query tile (16 KB per K-block) + at l
 // whole-tile stages (64 KB at d = 128: three of them); beyond, K-block stages (see flat_tc_kernel)
 SmemPlan planSmem(int KB, int kSteps, bool s8 = false) {
     FB_THROW_IF_NOT_MSG(KB <= kMaxKB, "dimension too large for the tensor-core Flat kernel");
-    if (s8) { // int8, QUAD: 16 KB query tile and half-tile stages
-        const size_t fixed = 1024 + 512 + kQuadCountBytes + (size_t)kTileM * kDpad8;
+    if (s8) { // int8, QUAD: 16 KB query tile and half-tile stages, and the bias ring
+        const size_t fixed = 1024 + 512 + kQuadCountBytes + (size_t)kTileM * kDpad8 + (size_t)kS8BiasSlots * kS8BiasSlotBytes;
         return {kS8Stages, fixed + (size_t)kS8Stages * kHalfN * kDpad8, 0, true, kHalfN, true};
     }
     const int ksplit = KB > 2 ? 1 : 0;
@@ -1077,6 +1077,8 @@ void launchTc(const CUtensorMap& mq, const CUtensorMap& my, const TcParams& p, i
     const size_t smem = sp.bytes;
     // QUAD: a segment's count is a 16-bit shared-memory counter (flat_tc_kernel.cuh)
     FB_THROW_IF_NOT_FMT(!sp.quad || p.cap <= kQuadMaxCap, "candidate cap %d too large for the 16-bit segment counts", p.cap);
+    // the int8 search bulk-copies each half-tile's biases into shared memory, which takes a 16-byte aligned source
+    FB_THROW_IF_NOT_MSG(!sp.s8 || DUMP || reinterpret_cast<uintptr_t>(p.bias) % 16 == 0, "int8 search: bias array not 16-byte aligned");
     auto kern = sp.quad ? flat_tc_kernel<DUMP, false, true> : flat_tc_kernel<DUMP>;
     if (self && !DUMP) // k = 1 streaming mode (self-tightening thresholds)
         kern = sp.quad ? flat_tc_kernel<false, true, true> : flat_tc_kernel<false, true>;

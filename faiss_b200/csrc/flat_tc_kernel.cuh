@@ -44,6 +44,14 @@ constexpr int kMaxYStages = 6;
 // S8 (int8 operands, QUAD only): a 128-byte swizzle row holds 128 s8, so the query tile and a half-tile stage are 16 KB
 // each and twelve stages fit beside them
 constexpr int kS8Stages = 12;
+// S8 search: the fp32 biases of a stage's 128 rows are copied with its codes, on its y_full barrier, so the filter's
+// exact test reads them from shared memory (a bias read from global memory is an HBM round trip the whole warpgroup
+// waits on).  The stage's n-th fill (pass n over the ring, yphase = n % 2) puts them in bias slot stage + kS8Stages *
+// yphase: twice as many slots as stages, so a warp can hand its stage back before its filter, as without the slots.
+// The fill that next writes a slot is two passes later, and it waits for the release of the fill one pass later,
+// which every reader of the slot gives only after the MMAs of that fill, which come after its filter of this one.
+constexpr int kS8BiasSlotBytes = kHalfN * 4;
+constexpr int kS8BiasSlots = 2 * kS8Stages;
 // QUAD: one 16-bit candidate count per segment of the unit.  A writer stops counting at its first slot >= cap, so a
 // count never exceeds cap + 2 (two writers): caps up to kQuadMaxCap keep it in 16 bits.
 constexpr int kQuadCountBytes = kSegsPerUnit * 2;
@@ -71,7 +79,7 @@ struct TcParams {
     int ksplit;         // 1: a ring stage holds ONE 64-wide K-block of a database tile (128 < d <= 256), else a whole tile
     int yStages;
     const float* invScalePtr; // device scalar: 1 / (qScale * yScale)
-    const float* bias;  // [numTiles*256], -inf padded (read on the slow path only)
+    const float* bias;  // [numTiles*256], -inf padded (read on the slow path only; S8 search: staged, 16-byte aligned)
     const float* tileMaxBias; // [numTiles] max bias of the tile's rows (rows are stored sorted by norm)
     const float* tileMinBias; // [numTiles] min bias of the tile's rows (SELF mode: a lower bound of the chunk's best score)
     const float* thr;   // [nq]  pass if score > thr
@@ -160,7 +168,8 @@ struct SegmentWriter {
 // is a tight upper bound of every score in a group (inv > 0 and rounding are monotonic: no false
 // negatives, bit for bit).  The fast path is therefore a pure max tree over raw accumulators --
 // no bias loads, no per-element FMA -- plus one FMA per 32 columns; the rare group whose bound beats
-// the threshold evaluates the exact test with biases read through L1/L2 and hands every survivor
+// the threshold evaluates the exact test with biases read through L1/L2 (SMEM_BIAS: from the bias slot at shared
+// address sBias, which holds the 128 rows from colBase rounded down to a multiple of 128) and hands every survivor
 // (score, global row) to emit.
 __device__ __forceinline__ float tc_max(float a, float b) {
     return fmaxf(a, b);
@@ -169,7 +178,7 @@ __device__ __forceinline__ int tc_max(int a, int b) {
     return max(a, b);
 }
 
-template <bool DUMP, bool SELF, typename T, typename Emit>
+template <bool DUMP, bool SELF, bool SMEM_BIAS = false, typename T, typename Emit>
 __device__ __forceinline__ void epi_filter32(
         const TcParams& p,
         const T (&r)[32],
@@ -180,7 +189,8 @@ __device__ __forceinline__ void epi_filter32(
         float slack, // SELF: 2 * eps of this query
         float maxb,
         float minb,  // SELF: min bias of the tile
-        Emit&& emit) {
+        Emit&& emit,
+        uint32_t sBias = 0) {
     if (DUMP) {
         if (q < p.nq) {
             float* dst = p.dump + (long long)q * p.dumpLd + colBase;
@@ -211,9 +221,20 @@ __device__ __forceinline__ void epi_filter32(
 #pragma unroll
         for (int g = 0; g < 4; g++) {
             if (fmaf((float)mg[g], inv, maxb) > thr) {
+                // SMEM_BIAS: elements j, j + 1 (neighbouring columns) take their biases as one pair
+                const uint32_t slotCol0 = sBias + 4u * (rowBase % kHalfN);
+                float2 pair;
 #pragma unroll
                 for (int j = 8 * g; j < 8 * g + 8; j++) {
-                    const float v = fmaf((float)r[j], inv, __ldg(bias + chunk_col(j)));
+                    float b;
+                    if constexpr (SMEM_BIAS) {
+                        if ((j & 1) == 0)
+                            pair = ptx::lds64f(slotCol0 + 4u * (uint32_t)chunk_col(j));
+                        b = (j & 1) ? pair.y : pair.x;
+                    } else {
+                        b = __ldg(bias + chunk_col(j));
+                    }
+                    const float v = fmaf((float)r[j], inv, b);
                     if (v > thr) {
                         emit(v, rowBase + chunk_col(j));
                         if (SELF) // k = 1: nothing scoring <= v - 2 eps can be the exact argmin any more
@@ -231,7 +252,9 @@ __device__ __forceinline__ void epi_filter32(
 // QUAD: tc_quad(p.KB, p.kSteps) holds, mapY's box is kHalfN rows, p.yStages == kMaxYStages and every ring stage holds one
 // half of a tile; the dynamic shared memory ends with kQuadCountBytes of segment counters.
 // S8 (QUAD, not SELF): int8 operands, 128 per swizzle row (one K-block: d <= 128), kS8Stages stages of 16 KB, four
-// m64n128k32 K-steps per half-tile, exact int32 accumulators, a per-query p.invQ in place of p.invScalePtr.
+// m64n128k32 K-steps per half-tile, exact int32 accumulators, a per-query p.invQ in place of p.invScalePtr.  The search
+// (not DUMP) copies each half-tile's 128 biases into the bias ring, kS8BiasSlots slots of kS8BiasSlotBytes behind the
+// segment counters at the end of the dynamic shared memory.
 template <bool DUMP, bool SELF = false, bool QUAD = false, bool S8 = false>
 __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
         const __grid_constant__ CUtensorMap mapQ,
@@ -262,6 +285,9 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
     // QUAD: 16-bit candidate counts of the unit's segments, behind the 512 bytes of barriers
     uint32_t* segCount = reinterpret_cast<uint32_t*>(reinterpret_cast<unsigned char*>(bars) + 512);
     const uint32_t sCounts = ptx::smem_u32(segCount);
+    // S8 search: the bias ring behind the counts (the raw-score dump reads no biases)
+    constexpr bool kStageBias = S8 && !DUMP;
+    unsigned char* sBias = reinterpret_cast<unsigned char*>(segCount) + kQuadCountBytes;
 
     // warp index as a provably warp-uniform value: ptxas then knows every warpgroup reaches its wgmma converged
     // (otherwise it serialises the wgmma chain)
@@ -305,11 +331,14 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
                     const int loads = QUAD ? 2 : p.ksplit ? KB : 1;
                     for (int l = 0; l < loads; l++) {
                         ptx::mbar_wait(&y_empty[ys], yphase ^ 1);
-                        ptx::mbar_arrive_expect_tx(&y_full[ys], (uint32_t)stageBytes);
+                        ptx::mbar_arrive_expect_tx(&y_full[ys], (uint32_t)(stageBytes + (kStageBias ? kS8BiasSlotBytes : 0)));
                         if (QUAD)
                             ptx::tma_load_3d(sY + (size_t)ys * stageBytes, &mapY, &y_full[ys], 0, t * kTileN + l * kHalfN, 0);
                         else
                             ptx::tma_load_3d(sY + (size_t)ys * stageBytes, &mapY, &y_full[ys], 0, t * kTileN, l);
+                        if constexpr (kStageBias)
+                            ptx::bulk_load_1d(sBias + (ys + kS8Stages * yphase) * kS8BiasSlotBytes,
+                                              p.bias + (size_t)t * kTileN + l * kHalfN, kS8BiasSlotBytes, &y_full[ys]);
                         if (++ys == yStages) {
                             ys = 0;
                             yphase ^= 1;
@@ -382,8 +411,9 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
             if (SELF && pp + 1 < pe)
                 minbNext = __ldg(p.tileMinBias + t);
         };
-        // filter of the 128 columns held in acc[64 c .. 64 c + 63] for both of the thread's rows
-        auto filterHalf = [&](int c) {
+        // filter of the 128 columns held in acc[64 c .. 64 c + 63] for both of the thread's rows; kStageBias: their
+        // biases are in the bias slot at shared address sb
+        auto filterHalf = [&](int c, uint32_t sb) {
             // this thread's first column of them
             const long long colBase = (long long)tile * kTileN + kHalfN * (h + c) + 2 * part;
 #pragma unroll
@@ -393,9 +423,9 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
                 for (int e = 0; e < 32; e++)
                     r[e] = acc[4 * (16 * c + (e >> 1)) + 2 * hr + (e & 1)];
                 if (hr)
-                    epi_filter32<DUMP, SELF>(p, r, q1, colBase, inv1, thr1, slack1, maxb, minb, w1);
+                    epi_filter32<DUMP, SELF, kStageBias>(p, r, q1, colBase, inv1, thr1, slack1, maxb, minb, w1, sb);
                 else
-                    epi_filter32<DUMP, SELF>(p, r, q0, colBase, inv0, thr0, slack0, maxb, minb, w0);
+                    epi_filter32<DUMP, SELF, kStageBias>(p, r, q0, colBase, inv0, thr0, slack0, maxb, minb, w0, sb);
             }
         };
 
@@ -429,6 +459,7 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
                 ptx::wgmma_commit();
                 ptx::wgmma_wait_all();
                 ptx::wgmma_fence_operands<64>(acc);
+                const uint32_t sb = kStageBias ? ptx::smem_u32(sBias) + (uint32_t)((ys + kS8Stages * yphase) * kS8BiasSlotBytes) : 0u;
                 __syncwarp();
                 if (lane == 0) // this warp's share of the stage has been read
                     ptx::mbar_arrive(&y_empty[ys]);
@@ -437,7 +468,7 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
                     ys -= yStages;
                     yphase ^= 1;
                 }
-                filterHalf(0);
+                filterHalf(0, sb);
                 tile += p.permStep;
                 if (tile >= (int)p.numTiles)
                     tile -= (int)p.numTiles;
@@ -473,8 +504,8 @@ __global__ void __launch_bounds__(tc_threads(QUAD), 1) flat_tc_kernel(
                         yphase ^= 1;
                     }
                 }
-                filterHalf(0);
-                filterHalf(1);
+                filterHalf(0, 0u);
+                filterHalf(1, 0u);
             }
         }
         if (QUAD && !DUMP) {
