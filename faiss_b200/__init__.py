@@ -92,7 +92,7 @@ def _empty_like_residency(x, shape, dtype):
     if _is_torch(x) and x.is_cuda:
         import torch
 
-        tdt = {np.float32: torch.float32, np.int64: torch.int64}[dtype]
+        tdt = {np.float32: torch.float32, np.int64: torch.int64, np.uint8: torch.uint8}[dtype]
         return torch.empty(shape, dtype=tdt, device=x.device)
     return np.empty(shape, dtype=dtype)
 
@@ -280,6 +280,24 @@ class Index:
             )
         )
         return D, I
+
+    def search_and_reconstruct(self, x, k, params=None):
+        """faiss::Index::search_and_reconstruct -> (D, I, R), R [n, k, d] the stored vector of each result (all 0xFF
+        bytes where I is -1); outputs follow x's residency.  GpuIndexFlat and the IVF indexes."""
+        x = self._check_x(x)
+        n = x.shape[0]
+        D = _empty_like_residency(x, (n, k), np.float32)
+        I = _empty_like_residency(x, (n, k), np.int64)
+        R = _empty_like_residency(x, (n, k, self.d), np.float32)
+        self._use_torch_stream(x, D, I, R)
+        rc = lib.faiss_Index_search_and_reconstruct(
+            self._h, ctypes.c_int64(n), _ptr(x, _c_f), ctypes.c_int64(k), params._h if params is not None else None,
+            _ptr(D, _c_f), _ptr(I, _c_i64), _ptr(R, _c_f)
+        )
+        if params is not None and getattr(params, "sel", None) is not None:
+            params.sel._raise_pending()
+        check(rc)
+        return D, I, R
 
     def assign(self, x, k=1):
         x = self._check_x(x)
@@ -603,6 +621,32 @@ class GpuIndexIVF(Index):
 
     def setIsTrained(self, v=True):
         check(lib.faiss_GpuIndexIVF_set_is_trained(self._h, int(bool(v))))
+
+    def code_sizes(self):
+        """(coarse_code_size, code_size): IndexIVF's list-number and code byte widths"""
+        c, s = ctypes.c_int(), ctypes.c_int()
+        check(lib.faiss_GpuIndexIVF_code_sizes(self._h, ctypes.byref(c), ctypes.byref(s)))
+        return c.value, s.value
+
+    def search_and_return_codes(self, x, k, include_listnos=False, params=None):
+        """faiss::IndexIVF::search_and_return_codes -> (D, I, codes), codes [n, k, (coarse_code_size if include_listnos)
+        + code_size] uint8: the CPU inverted-list bytes of each result, prefixed by its list number (little-endian);
+        all 0xFF where I is -1.  Outputs follow x's residency."""
+        x = self._check_x(x)
+        n = x.shape[0]
+        ccs, cs = self.code_sizes()
+        D = _empty_like_residency(x, (n, k), np.float32)
+        I = _empty_like_residency(x, (n, k), np.int64)
+        C = _empty_like_residency(x, (n, k, (ccs if include_listnos else 0) + cs), np.uint8)
+        self._use_torch_stream(x, D, I, C)
+        rc = lib.faiss_GpuIndexIVF_search_and_return_codes(
+            self._h, ctypes.c_int64(n), _ptr(x, _c_f), ctypes.c_int64(k), params._h if params is not None else None,
+            _ptr(D, _c_f), _ptr(I, _c_i64), _ptr(C, _c_u8), int(bool(include_listnos))
+        )
+        if params is not None and getattr(params, "sel", None) is not None:
+            params.sel._raise_pending()
+        check(rc)
+        return D, I, C
 
     def search_preassigned(self, x, k, assign, centroid_dis=None):
         x = self._check_x(x)

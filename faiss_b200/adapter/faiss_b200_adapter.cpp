@@ -112,6 +112,23 @@ void B200Index::search(
     faiss_SearchParameters_free(sp);
     ck(rc);
 }
+void B200Index::search_and_reconstruct(
+        faiss::idx_t n, const float* x, faiss::idx_t k, float* distances, faiss::idx_t* labels, float* recons,
+        const faiss::SearchParameters* params) const {
+    if (!params || !params->sel) {
+        ck(faiss_Index_search_and_reconstruct(h_, n, x, k, nullptr, distances, labels, recons));
+        return;
+    }
+    SelectorHandles sel;
+    FaissSearchParameters* sp = nullptr;
+    ck(faiss_SearchParameters_new(&sp, sel.convert(params->sel)));
+    int rc = faiss_Index_search_and_reconstruct(h_, n, x, k, sp, distances, labels, recons);
+    faiss_SearchParameters_free(sp);
+    ck(rc);
+}
+void B200Index::reconstruct_batch(faiss::idx_t n, const faiss::idx_t* keys, float* recons) const {
+    ck(faiss_Index_reconstruct_batch(h_, n, keys, recons));
+}
 void B200Index::reset() {
     ck(faiss_Index_reset(h_));
     sync_();
@@ -151,8 +168,10 @@ void B200IndexFlat::copyTo(faiss::IndexFlat* index) const { // faiss/gpu/GpuInde
 }
 
 // ---------------------------------------------------------------- IVF
-void B200IndexIVF::search(
-        faiss::idx_t n, const float* x, faiss::idx_t k, float* distances, faiss::idx_t* labels, const faiss::SearchParameters* params) const {
+// search (recons == null) or search_and_reconstruct with the index's nprobe or the SearchParametersIVF's
+void B200IndexIVF::search_(
+        faiss::idx_t n, const float* x, faiss::idx_t k, float* distances, faiss::idx_t* labels, float* recons,
+        const faiss::SearchParameters* params) const {
     size_t use_nprobe = nprobe;
     size_t max_codes = 0;
     SelectorHandles sel;
@@ -167,9 +186,19 @@ void B200IndexIVF::search(
     }
     FaissSearchParametersIVF* sp = nullptr;
     ck(faiss_SearchParametersIVF_new_with_sel(&sp, selHandle, use_nprobe, max_codes));
-    int rc = faiss_Index_search_with_params(h_, n, x, k, sp, distances, labels);
+    int rc = recons ? faiss_Index_search_and_reconstruct(h_, n, x, k, sp, distances, labels, recons)
+                    : faiss_Index_search_with_params(h_, n, x, k, sp, distances, labels);
     faiss_SearchParameters_free(sp);
     ck(rc);
+}
+void B200IndexIVF::search(
+        faiss::idx_t n, const float* x, faiss::idx_t k, float* distances, faiss::idx_t* labels, const faiss::SearchParameters* params) const {
+    search_(n, x, k, distances, labels, nullptr, params);
+}
+void B200IndexIVF::search_and_reconstruct(
+        faiss::idx_t n, const float* x, faiss::idx_t k, float* distances, faiss::idx_t* labels, float* recons,
+        const faiss::SearchParameters* params) const {
+    search_(n, x, k, distances, labels, recons, params);
 }
 
 void B200IndexIVF::copyListsFrom_(const faiss::IndexIVF* index) {

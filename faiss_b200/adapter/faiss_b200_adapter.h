@@ -58,6 +58,18 @@ class B200Index : public faiss::Index {
     void reset() override;
     void reconstruct(faiss::idx_t key, float* recons) const override;
     void reconstruct_n(faiss::idx_t i0, faiss::idx_t ni, float* recons) const override;
+    // one call for all keys (faiss::Index's default is one reconstruct per key)
+    void reconstruct_batch(faiss::idx_t n, const faiss::idx_t* keys, float* recons) const override;
+    // one call on the device: R is the entry each result was scored on, not the per-label reconstruct of
+    // faiss::Index's default (which resolves an id stored twice to one fixed entry)
+    void search_and_reconstruct(
+            faiss::idx_t n,
+            const float* x,
+            faiss::idx_t k,
+            float* distances,
+            faiss::idx_t* labels,
+            float* recons,
+            const faiss::SearchParameters* params = nullptr) const override;
     FaissIndex_H* handle() const {
         return h_;
     }
@@ -92,9 +104,25 @@ class B200IndexIVF : public B200Index { // faiss::gpu::GpuIndexIVF (faiss/gpu/Gp
             float* distances,
             faiss::idx_t* labels,
             const faiss::SearchParameters* params = nullptr) const override;
+    void search_and_reconstruct(
+            faiss::idx_t n,
+            const float* x,
+            faiss::idx_t k,
+            float* distances,
+            faiss::idx_t* labels,
+            float* recons,
+            const faiss::SearchParameters* params = nullptr) const override;
 
    protected:
     B200IndexIVF(int d, faiss::MetricType metric, size_t nlist_, int device) : B200Index(d, metric, device), nlist(nlist_) {}
+    void search_(
+            faiss::idx_t n,
+            const float* x,
+            faiss::idx_t k,
+            float* distances,
+            faiss::idx_t* labels,
+            float* recons,
+            const faiss::SearchParameters* params) const;
     void copyListsFrom_(const faiss::IndexIVF* index);
     void copyListsTo_(faiss::IndexIVF* index) const;
 };

@@ -816,6 +816,31 @@ int faiss_Index_search_with_params(
     }
     CATCH_AND_HANDLE
 }
+int faiss_Index_search_and_reconstruct(
+        const FaissIndex* p, idx_t n, const float* x, idx_t k, const FaissSearchParameters* params, float* D, idx_t* I,
+        float* recons) {
+    try {
+        IX(p)->search_and_reconstruct(n, x, k, D, I, recons, params ? params->p : nullptr);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexIVF_search_and_return_codes(
+        const FaissGpuIndex* p, idx_t n, const float* x, idx_t k, const FaissSearchParameters* params, float* D, idx_t* I,
+        uint8_t* codes, int include_listno) {
+    try {
+        AS<GpuIndexIVF>(p, "GpuIndexIVF")
+                ->search_and_return_codes(n, x, k, D, I, codes, include_listno != 0, params ? params->p : nullptr);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexIVF_code_sizes(const FaissGpuIndex* p, int* coarse_code_size, int* code_size) {
+    try {
+        auto* ivf = AS<GpuIndexIVF>(p, "GpuIndexIVF");
+        *coarse_code_size = ivf->coarse_code_size();
+        *code_size = ivf->code_size();
+    }
+    CATCH_AND_HANDLE
+}
 void faiss_b200_set_interrupt_callback(int (*want_interrupt)(void*), void* ctx) {
     InterruptCallback::set(want_interrupt, ctx);
 }

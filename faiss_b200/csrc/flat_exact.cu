@@ -893,19 +893,22 @@ __global__ void gather_rows_kernel(
         const idx_t* __restrict__ ids,
         int64_t n,
         int d,
-        float* __restrict__ out) {
+        float* __restrict__ out,
+        bool missingAllOnes) {
     int64_t i = blockIdx.x;
     idx_t a = ids[i];
     for (int j = threadIdx.x; j < d; j += blockDim.x) {
-        out[i * d + j] = a < 0 ? CUDART_NAN_F : row_elem(src, yHalf, a * d + j);
+        out[i * d + j] = a < 0 ? (missingAllOnes ? __int_as_float(-1) : CUDART_NAN_F) : row_elem(src, yHalf, a * d + j);
     }
 }
 
-void runGatherRows(const void* src, const idx_t* ids, int64_t n, int d, float* out, cudaStream_t stream, int yHalf) {
+void runGatherRows(
+        const void* src, const idx_t* ids, int64_t n, int d, float* out, cudaStream_t stream, int yHalf, bool missingAllOnes) {
     if (n == 0)
         return;
     FB_THROW_IF_NOT(n < (int64_t(1) << 31));
-    gather_rows_kernel<<<(unsigned)n, std::min(d, 256), 0, stream>>>(src, yHalf, ids, n, d, out);
+    gather_rows_kernel<<<(unsigned)n, std::min(d, 256), 0, stream>>>(
+            src, yHalf, ids, n, d, out, missingAllOnes);
     CUDA_CHECK_LAST();
 }
 

@@ -2,6 +2,7 @@
 #include "index.h"
 
 #include "comm.h"
+#include "ivf_layout.cuh"
 
 #include <algorithm>
 #include <cfloat>
@@ -111,6 +112,19 @@ __global__ void copy_lists_kernel(
         dstIds[dstStart[l] + i] = srcIds[srcStart[l] + i];
 }
 
+// an output that may live on the host and whose rows are only partly written: the device staging starts as a copy
+// of the caller's contents
+template <typename T>
+struct DeviceInOut : DeviceOut<T> {
+    DeviceInOut(GpuResources* res, int device, T* p, size_t count, cudaStream_t stream) : DeviceOut<T>(res, device, p, count) {
+        if (this->staged)
+            CUDA_VERIFY(cudaMemcpyAsync(this->ptr, p, count * sizeof(T), cudaMemcpyDefault, stream));
+    }
+};
+
+// outputs of a retrieval call are staged per page of at most this many bytes
+constexpr size_t kRetrievalPageBytes = size_t(256) << 20;
+
 } // namespace
 
 // ------------------------------------------------------------------------------------------
@@ -133,6 +147,9 @@ void Index::reconstruct_batch(idx_t n, const idx_t* keys, float* recons) const {
 void Index::reconstruct_n(idx_t i0, idx_t ni, float* recons) const {
     for (idx_t i = 0; i < ni; i++)
         reconstruct(i0 + i, recons + (size_t)i * d);
+}
+void Index::search_and_reconstruct(idx_t, const float*, idx_t, float*, idx_t*, float*, const SearchParameters*) const {
+    FB_THROW_MSG("search_and_reconstruct not implemented for this type of index");
 }
 void Index::compute_residual(const float* x, float* residual, idx_t key) const {
     reconstruct(key, residual);
@@ -598,6 +615,27 @@ void GpuIndexFlat::searchShardDevice(idx_t n, const float* xDev, int k, float* d
     lastSearchFallbackQueries = (int)tc_.search(xDev, n, k, dDev, iDev, stream, flatShard);
     lastSearchUsedTensorCores = 1;
     lastSearchOperandBits = tc_.lastOperandBits();
+}
+
+void GpuIndexFlat::search_and_reconstruct(
+        idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, float* recons, const SearchParameters* params) const {
+    search(n, x, k, distances, labels, params);
+    if (n == 0)
+        return;
+    FB_THROW_IF_NOT_MSG(recons, "null pointer passed to search_and_reconstruct");
+    DeviceScope scope(config_.device);
+    auto stream = stream_();
+    // labels are row numbers: gather the rows, a page of results at a time
+    const idx_t total = n * k;
+    const idx_t pageRows = std::max<idx_t>(1, (idx_t)(kRetrievalPageBytes / (sizeof(float) * d)));
+    for (idx_t r0 = 0; r0 < total; r0 += pageRows) {
+        const idx_t nr = std::min(pageRows, total - r0);
+        DeviceView<idx_t> lv(resources_.get(), config_.device, labels + r0, nr, stream);
+        DeviceOut<float> rv(resources_.get(), config_.device, recons + (size_t)r0 * d, (size_t)nr * d);
+        runGatherRows(rows_(), lv.ptr, nr, d, rv.ptr, stream, yHalf_(), true);
+        rv.finish(stream);
+        CUDA_VERIFY(cudaStreamSynchronize(stream));
+    }
 }
 
 void GpuIndexFlat::reconstruct(idx_t key, float* out) const {
@@ -1426,6 +1464,161 @@ void GpuIndexIVF::search_preassigned(
     CUDA_VERIFY(cudaStreamSynchronize(stream));
 }
 
+// ---- retrieval: ids -> arena slots -> decoded entries (ivf_reconstruct.cu)
+IvfStoredLayout GpuIndexIVF::listLayout_() const {
+    IvfStoredLayout a;
+    a.d = d;
+    a.codeSize = lists_->codeSize();
+    a.interleaved = lists_->interleaved();
+    a.listStart = lists_->dStart();
+    a.listLen = lists_->dLen();
+    a.nlist = nlist;
+    a.arenaElems = lists_->arenaElems();
+    a.codes = lists_->codes();
+    a.ids = lists_->ids();
+    return a;
+}
+
+int GpuIndexIVF::coarse_code_size() const {
+    int nbyte = 0;
+    for (idx_t nl = nlist - 1; nl > 0; nl >>= 8)
+        nbyte++;
+    return nbyte;
+}
+
+// rows per call of the ids -> slots pass: all of them for a device output; pages of kRetrievalPageBytes for a host
+// output, so the device staging stays bounded (each page repeats the pass over the stored ids)
+idx_t GpuIndexIVF::retrievalPageRows_(const float* out, idx_t n) const {
+    if (getDeviceForAddress(out) == config_.device)
+        return std::max<idx_t>(n, 1);
+    return std::max<idx_t>(1, (idx_t)(kRetrievalPageBytes / (sizeof(float) * d)));
+}
+
+void GpuIndexIVF::reconstruct_n(idx_t i0, idx_t ni, float* recons) const {
+    FB_THROW_IF_NOT(ni == 0 || (i0 >= 0 && i0 + ni <= this->ntotal));
+    if (ni == 0)
+        return;
+    DeviceScope scope(config_.device);
+    auto stream = stream_();
+    const IvfStoredLayout a = storedLayout_();
+    const idx_t page = retrievalPageRows_(recons, ni);
+    for (idx_t r0 = 0; r0 < ni; r0 += page) {
+        const idx_t nr = std::min(page, ni - r0);
+        auto slots = resources_->temp(config_.device, sizeof(idx_t) * nr);
+        runIvfSlotsOfRange(a, i0 + r0, nr, slots.as<idx_t>(), stream);
+        // rows of ids not stored keep the caller's contents: a staged page starts as a copy of them
+        DeviceInOut<float> out(resources_.get(), config_.device, recons + (size_t)r0 * d, (size_t)nr * d, stream);
+        runIvfReconstruct(a, slots.as<idx_t>(), nr, false, out.ptr, stream);
+        out.finish(stream);
+        CUDA_VERIFY(cudaStreamSynchronize(stream));
+    }
+}
+
+void GpuIndexIVF::reconstruct_batch(idx_t n, const idx_t* keys, float* recons) const {
+    if (n == 0)
+        return;
+    DeviceScope scope(config_.device);
+    auto stream = stream_();
+    const IvfStoredLayout a = storedLayout_();
+    DeviceView<idx_t> kv(resources_.get(), config_.device, keys, (size_t)n, stream);
+    auto slots = resources_->temp(config_.device, sizeof(idx_t) * n);
+    // every key is resolved before any row is written
+    FB_THROW_IF_NOT_MSG(
+            runIvfSlotsOfKeys(resources_.get(), config_.device, a, kv.ptr, n, slots.as<idx_t>(), stream), "key not found");
+    const idx_t page = retrievalPageRows_(recons, n);
+    for (idx_t r0 = 0; r0 < n; r0 += page) {
+        const idx_t nr = std::min(page, n - r0);
+        DeviceOut<float> out(resources_.get(), config_.device, recons + (size_t)r0 * d, (size_t)nr * d);
+        runIvfReconstruct(a, slots.as<idx_t>() + r0, nr, true, out.ptr, stream);
+        out.finish(stream);
+        CUDA_VERIFY(cudaStreamSynchronize(stream));
+    }
+}
+
+void GpuIndexIVF::reconstruct(idx_t key, float* recons) const {
+    reconstruct_batch(1, &key, recons);
+}
+
+void GpuIndexIVF::searchWithSlots_(
+        idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, const SearchParameters* params,
+        size_t resultBytes, const std::function<void(idx_t, idx_t, const idx_t*)>& page) const {
+    DeviceScope scope(config_.device);
+    FB_THROW_IF_NOT_MSG(this->is_trained, "Index not trained");
+    validateKSelect(k);
+    if (n == 0)
+        return;
+    FB_THROW_IF_NOT_MSG(x && distances && labels, "null pointer passed to search");
+    struct Guard {
+        const SearchParameters*& params;
+        const uint32_t*& mask;
+        const IvfSlotOutput*& slots;
+        ~Guard() {
+            params = nullptr;
+            mask = nullptr;
+            slots = nullptr;
+        }
+    } guard{callParams_, callMask_, callSlots_};
+    callParams_ = params;
+    GpuMemoryReservation mask;
+    if (params && params->sel && this->ntotal > 0) {
+        mask = selMask_(*params->sel);
+        callMask_ = mask.as<uint32_t>();
+    }
+    auto stream = stream_();
+    const int64_t slotsTotal = lists_->arenaElems();
+    auto identity = resources_->device_alloc(config_.device, sizeof(idx_t) * std::max<int64_t>(1, slotsTotal), AllocType::Other);
+    runIvfIdentitySlots(identity.as<idx_t>(), slotsTotal, stream);
+    // query pages: search()'s bound on the result staging, and a bound on the page's decoded output
+    idx_t maxQ = std::min<idx_t>(idx_t(1) << 18, (idx_t)((size_t(1) << 30) / ((size_t)k * 12 * 8)));
+    maxQ = std::min<idx_t>(maxQ, (idx_t)(kRetrievalPageBytes / ((size_t)k * resultBytes)));
+    maxQ = std::max<idx_t>(maxQ, 1);
+    for (idx_t i0 = 0; i0 < n; i0 += maxQ) {
+        InterruptCallback::check(); // between query pages
+        const idx_t nb = std::min(maxQ, n - i0);
+        DeviceView<float> xv(resources_.get(), config_.device, x + (size_t)i0 * d, (size_t)nb * d, stream);
+        DeviceOut<float> dv(resources_.get(), config_.device, distances + (size_t)i0 * k, (size_t)nb * k);
+        DeviceOut<idx_t> lv(resources_.get(), config_.device, labels + (size_t)i0 * k, (size_t)nb * k);
+        auto slots = resources_->temp(config_.device, sizeof(idx_t) * nb * k);
+        const IvfSlotOutput so{identity.as<idx_t>(), lists_->ids(), slots.as<idx_t>()};
+        callSlots_ = &so;
+        searchImpl_(nb, xv.ptr, (int)k, dv.ptr, lv.ptr);
+        callSlots_ = nullptr;
+        page(i0, nb, slots.as<idx_t>());
+        dv.finish(stream);
+        lv.finish(stream);
+        CUDA_VERIFY(cudaStreamSynchronize(stream));
+    }
+}
+
+void GpuIndexIVF::search_and_reconstruct(
+        idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, float* recons, const SearchParameters* params) const {
+    FB_THROW_IF_NOT_MSG(n == 0 || recons, "null pointer passed to search_and_reconstruct");
+    const IvfStoredLayout a = storedLayout_();
+    searchWithSlots_(n, x, k, distances, labels, params, sizeof(float) * d, [&](idx_t i0, idx_t nb, const idx_t* slots) {
+        auto stream = stream_();
+        DeviceOut<float> rv(resources_.get(), config_.device, recons + (size_t)i0 * k * d, (size_t)nb * k * d);
+        runIvfReconstruct(a, slots, nb * k, true, rv.ptr, stream);
+        rv.finish(stream);
+        CUDA_VERIFY(cudaStreamSynchronize(stream)); // the staging buffer dies here
+    });
+}
+
+void GpuIndexIVF::search_and_return_codes(
+        idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, uint8_t* codes, bool include_listno,
+        const SearchParameters* params) const {
+    FB_THROW_IF_NOT_MSG(n == 0 || codes, "null pointer passed to search_and_return_codes");
+    const IvfStoredLayout a = listLayout_();
+    const int listnoBytes = include_listno ? coarse_code_size() : 0;
+    const size_t rowBytes = (size_t)listnoBytes + a.codeSize;
+    searchWithSlots_(n, x, k, distances, labels, params, rowBytes, [&](idx_t i0, idx_t nb, const idx_t* slots) {
+        auto stream = stream_();
+        DeviceOut<uint8_t> cv(resources_.get(), config_.device, codes + (size_t)i0 * k * rowBytes, (size_t)nb * k * rowBytes);
+        runIvfGatherCodes(a, slots, nb * k, listnoBytes, cv.ptr, stream);
+        cv.finish(stream);
+        CUDA_VERIFY(cudaStreamSynchronize(stream)); // the staging buffer dies here
+    });
+}
+
 // ------------------------------------------------------------------------------------------
 // GpuIndexIVFFlat
 // ------------------------------------------------------------------------------------------
@@ -1463,8 +1656,14 @@ void GpuIndexIVFFlat::scanImpl_(
         idx_t* iDev) const {
     runIvfFlatScan(
             resources_.get(), config_.device, xDev, n, d, probes, np, lists_->dStart(), lists_->dLen(),
-            reinterpret_cast<const float*>(lists_->codes()), lists_->ids(), lists_->arenaElems(), k, metric_type, dDev,
-            iDev, stream_(), callMask_);
+            reinterpret_cast<const float*>(lists_->codes()), scanIds_(), lists_->arenaElems(), k, metric_type, dDev,
+            iDev, stream_(), callMask_, callSlots_);
+}
+
+IvfStoredLayout GpuIndexIVFFlat::storedLayout_() const {
+    IvfStoredLayout a = listLayout_();
+    a.kind = IVF_STORED_FLAT;
+    return a;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1689,14 +1888,26 @@ void GpuIndexIVFPQ::scanImpl_(
         runIvfPqScanInterleaved(
                 resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np, quantizer->vectorsDevice(),
                 pqCentroidsT_.data(), precomputedActive_() ? (ensureTerm2_(), term2_.data()) : nullptr,
-                lists_->codeSize(), nibbleLayout_(), lists_->dStart(), lists_->dLen(), lists_->codes(), lists_->ids(),
-                lists_->arenaElems(), k, metric_type, dDev, iDev, stream_(), callMask_);
+                lists_->codeSize(), nibbleLayout_(), lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(),
+                lists_->arenaElems(), k, metric_type, dDev, iDev, stream_(), callMask_, callSlots_);
         return;
     }
     runIvfPqScan(
             resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np, quantizer->vectorsDevice(),
-            pqCentroids_.data(), M_, nbits_, lists_->dStart(), lists_->dLen(), lists_->codes(), lists_->ids(), k,
-            metric_type, dDev, iDev, stream_(), callMask_);
+            pqCentroids_.data(), M_, nbits_, lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(), k,
+            metric_type, dDev, iDev, stream_(), callMask_, callSlots_);
+}
+
+// IndexIVFPQ::reconstruct_from_offset (faiss/IndexIVFPQ.cpp:358-372): pq.decode, then + the list's centroid
+IvfStoredLayout GpuIndexIVFPQ::storedLayout_() const {
+    FB_THROW_IF_NOT_MSG(pqCentroids_.size() > 0, "PQ not trained");
+    IvfStoredLayout a = listLayout_();
+    a.kind = IVF_STORED_PQ;
+    a.M = M_;
+    a.nbits = nbits_;
+    a.pq = pqCentroids_.data();
+    a.centroids = quantizer->vectorsDevice();
+    return a;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1889,8 +2100,23 @@ void GpuIndexIVFScalarQuantizer::scanImpl_(
     runIvfSqScan(
             resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np,
             needCentroids ? quantizer->vectorsDevice() : nullptr, by_residual, qtype_, params_.data() + 2 * d,
-            lists_->dStart(), lists_->dLen(), lists_->codes(), lists_->ids(), lists_->arenaElems(), lists_->codeSize(), k,
-            metric_type, dDev, iDev, stream_(), callMask_);
+            lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(), lists_->arenaElems(), lists_->codeSize(), k,
+            metric_type, dDev, iDev, stream_(), callMask_, callSlots_);
+}
+
+// IndexIVFScalarQuantizer::reconstruct_from_offset (faiss/IndexScalarQuantizer.cpp:400-425): sq.decode, then + the
+// list's centroid when by_residual
+IvfStoredLayout GpuIndexIVFScalarQuantizer::storedLayout_() const {
+    FB_THROW_IF_NOT_MSG(params_.size() == (size_t)4 * d, "scalar quantizer not trained");
+    IvfStoredLayout a = listLayout_();
+    a.kind = IVF_STORED_SQ;
+    const bool nibble = qtype_ == SQ_QT_4bit || qtype_ == SQ_QT_4bit_uniform;
+    a.sqCodec = nibble ? SQC_NIBBLE : qtype_ == SQ_QT_6bit ? SQC_SIX : qtype_ == SQ_QT_fp16 ? SQC_HALF : SQC_BYTE;
+    a.levels = qtype_ == SQ_QT_fp16 || qtype_ == SQ_QT_8bit_direct ? 0.f : nibble ? 15.f : qtype_ == SQ_QT_6bit ? 63.f : 255.f;
+    a.vmin = params_.data();
+    a.vdiff = params_.data() + d;
+    a.centroids = by_residual ? quantizer->vectorsDevice() : nullptr;
+    return a;
 }
 
 // ------------------------------------------------------------------------------------------

@@ -12,6 +12,7 @@
 // Everything device-side goes through kernels.h and flat_tc.h.
 #pragma once
 
+#include <functional>
 #include <memory>
 #include <string>
 #include <vector>
@@ -23,6 +24,8 @@
 #include "resources.h"
 
 namespace fb200 {
+
+struct SearchParameters;
 
 // ------------------------------------------------------------------------------------------
 // faiss::Index
@@ -49,6 +52,11 @@ struct Index {
     virtual void reconstruct_n(idx_t i0, idx_t ni, float* recons) const;
     virtual void compute_residual(const float* x, float* residual, idx_t key) const;
     virtual void compute_residual_n(idx_t n, const float* xs, float* residuals, const idx_t* keys) const;
+    // faiss::Index::search_and_reconstruct (faiss/Index.h:238-254): search, and recons [n][k][d] = the stored vector of
+    // each result, all 0xFF bytes where the label is -1.  Only GpuIndexFlat and the IVF indexes implement it.
+    virtual void search_and_reconstruct(
+            idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, float* recons,
+            const SearchParameters* params = nullptr) const;
 };
 
 // faiss::SearchParameters / SearchParametersIVF (faiss/Index.h:88-93, faiss/IndexIVF.h:68-90): per-call overrides.
@@ -186,6 +194,10 @@ class GpuIndexFlat : public GpuIndex {
     void compute_residual_n(idx_t n, const float* xs, float* residuals, const idx_t* keys) const override;
     using GpuIndex::search;
     void search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels) const override;
+    // search, then the returned rows (fp16 storage: widened, as reconstruct)
+    void search_and_reconstruct(
+            idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, float* recons,
+            const SearchParameters* params = nullptr) const override;
 
     // device-pointer entry points used by IVF / clustering (role of FlatIndex::query)
     void searchDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
@@ -468,7 +480,45 @@ class GpuIndexIVF : public GpuIndex {
             float* distances,
             idx_t* labels) const;
 
+    // faiss::IndexIVF retrieval (faiss/IndexIVF.cpp:1056-1248), decoded on the device with reconstruct_from_offset's
+    // arithmetic.  No direct map is kept: an id stored more than once resolves to the entry last in (list, offset)
+    // order, as the CPU's reconstruct_n loop; reconstruct / reconstruct_batch throw "key not found" for an id that is
+    // not stored, before writing anything.  Outputs may live on the host or the device.
+    void reconstruct(idx_t key, float* recons) const override;
+    void reconstruct_n(idx_t i0, idx_t ni, float* recons) const override; // rows of ids not stored are left as they are
+    void reconstruct_batch(idx_t n, const idx_t* keys, float* recons) const override;
+    // D and I equal search(..., params); recons decodes the entry each result came from
+    void search_and_reconstruct(
+            idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, float* recons,
+            const SearchParameters* params = nullptr) const override;
+    // codes [n][k][coarse_code_size() (include_listno) + code_size]: the CPU ArrayInvertedLists bytes of each result,
+    // prefixed by its list number in little-endian bytes; all 0xFF where the label is -1
+    void search_and_return_codes(
+            idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, uint8_t* codes, bool include_listno,
+            const SearchParameters* params = nullptr) const;
+    // IndexIVF::coarse_code_size: bytes of a list number (faiss/IndexIVF.cpp encode_listno)
+    int coarse_code_size() const;
+    int code_size() const {
+        return lists_->codeSize();
+    }
+
    protected:
+    // the decoder's view of this index's lists
+    virtual IvfStoredLayout storedLayout_() const = 0;
+    IvfStoredLayout listLayout_() const;
+    idx_t retrievalPageRows_(const float* out, idx_t n) const;
+    // search with the slot of every result: per page of queries, `page(i0, nb, slotsDev)` runs after D / I of the
+    // page are on the device (slotsDev [nb][k], -1 with a missing result); resultBytes (the page's output per result)
+    // bounds the page size
+    void searchWithSlots_(
+            idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, const SearchParameters* params,
+            size_t resultBytes, const std::function<void(idx_t, idx_t, const idx_t*)>& page) const;
+    // set while searchWithSlots_ runs: scanImpl_ hands the scans callSlots_->identity instead of the list ids
+    mutable const IvfSlotOutput* callSlots_ = nullptr;
+    const idx_t* scanIds_() const {
+        return callSlots_ ? callSlots_->identity : lists_->ids();
+    }
+
     bool addImplRequiresIDs_() const override {
         return true;
     }
@@ -523,6 +573,7 @@ class GpuIndexIVFFlat : public GpuIndexIVF {
    protected:
     const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
     void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
+    IvfStoredLayout storedLayout_() const override;
 };
 
 struct GpuIndexIVFPQConfig : GpuIndexIVFConfig { // faiss/gpu/GpuIndexIVFPQ.h:25-49
@@ -593,6 +644,7 @@ class GpuIndexIVFPQ : public GpuIndexIVF {
     void trainEncoder_(idx_t n, const float* xDev) override; // the PQ, on residuals
     const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
     void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
+    IvfStoredLayout storedLayout_() const override;
 
     int M_, nbits_;
     int ksub_() const {
@@ -665,6 +717,7 @@ class GpuIndexIVFScalarQuantizer : public GpuIndexIVF {
     void trainEncoder_(idx_t n, const float* xDev) override; // the RS_minmax ranges
     const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
     void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
+    IvfStoredLayout storedLayout_() const override;
 
     int qtype_;
     std::vector<float> trained_;

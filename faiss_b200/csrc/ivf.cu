@@ -480,7 +480,8 @@ void runIvfScanBatches(
         float* outD,
         idx_t* outI,
         cudaStream_t stream,
-        const std::function<void(const IvfScanBatch&)>& launch) {
+        const std::function<void(const IvfScanBatch&)>& launch,
+        const IvfSlotOutput* slots) {
     if (nq == 0)
         return;
     int probesPerCta = 1;
@@ -498,9 +499,14 @@ void runIvfScanBatches(
         launch(batch);
         KernelTiming::end(timingName, stream);
         CUDA_CHECK_LAST();
-        runMergeTopKKeyspace(
-                partD.as<float>(), partI.as<idx_t>(), nb, ctasPerQuery, k, k, metric, 0, outD + q0 * k, outI + q0 * k,
-                stream);
+        if (slots)
+            runIvfMergeTopKSlots(
+                    partD.as<float>(), partI.as<idx_t>(), slots->arenaIds, nb, ctasPerQuery, k, k, metric, outD + q0 * k,
+                    outI + q0 * k, slots->outSlot + q0 * k, stream);
+        else
+            runMergeTopKKeyspace(
+                    partD.as<float>(), partI.as<idx_t>(), nb, ctasPerQuery, k, k, metric, 0, outD + q0 * k, outI + q0 * k,
+                    stream);
     }
 }
 
@@ -522,7 +528,8 @@ void runIvfFlatScan(
         float* outD,
         idx_t* outI,
         cudaStream_t stream,
-        const uint32_t* slotMask) {
+        const uint32_t* slotMask,
+        const IvfSlotOutput* slots) {
     if (nq == 0)
         return;
     const int LIST = std::max(64, next_pow2(k));
@@ -542,7 +549,7 @@ void runIvfFlatScan(
                 });
             });
         });
-    });
+    }, slots);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -692,7 +699,8 @@ void runIvfPqScan(
         float* outD,
         idx_t* outI,
         cudaStream_t stream,
-        const uint32_t* slotMask) {
+        const uint32_t* slotMask,
+        const IvfSlotOutput* slots) {
     if (nq == 0)
         return;
     FB_THROW_IF_NOT(nbits >= 1 && nbits <= 8);
@@ -716,7 +724,7 @@ void runIvfPqScan(
                 });
             });
         });
-    });
+    }, slots);
 }
 
 } // namespace fb200

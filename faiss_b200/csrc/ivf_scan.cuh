@@ -26,6 +26,8 @@ struct IvfScanBatch {
     idx_t* partI;
 };
 
+// With `slots`, the launch writes arena positions (the scan reads slots->identity as its id table), merged by
+// runIvfMergeTopKSlots into outI and slots->outSlot.
 // Splits nq queries into batches that bound the partial-result scratch, calls `launch` once per batch (the
 // scan kernel launch, bracketed by KernelTiming `timingName`) and merges each batch's partial results into
 // outD / outI [nq][k].  oneProbePerCta: one CTA per (query, probe); else the probes are split by ivfScanChunks.
@@ -41,7 +43,8 @@ void runIvfScanBatches(
         float* outD,
         idx_t* outI,
         cudaStream_t stream,
-        const std::function<void(const IvfScanBatch&)>& launch);
+        const std::function<void(const IvfScanBatch&)>& launch,
+        const IvfSlotOutput* slots = nullptr);
 
 // runtime value -> compile-time constant (see withBool): f(std::integral_constant<int, V>{}) for the V of Vs equal to v
 template <int... Vs, typename F>

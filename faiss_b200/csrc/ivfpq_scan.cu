@@ -14,6 +14,7 @@
 #include <cfloat>
 #include <type_traits>
 
+#include "ivf_layout.cuh"
 #include "ivf_scan.cuh"
 #include "kernels.h"
 #include "select.cuh"
@@ -24,13 +25,6 @@ namespace {
 constexpr int kLutSlots = 64; // 256 B per code value
 constexpr int kIlvScanWarps = 16;  // warps per scan CTA (ivf_scan.cuh's kScanWarps is the 4-warp scans')
 constexpr int kScanMinCtas = 2; // CTAs per SM the scan kernel's register budget is set for (64 registers)
-
-__device__ __forceinline__ int64_t interleaved_pos(int64_t v, int j, int M) {
-    // byte position j of list-relative vector v
-    const int64_t g = v >> 5;
-    const int t = (int)(v & 31);
-    return g * 32 * M + (j >> 4) * 512 + t * 16 + (j & 15);
-}
 
 __global__ void pq_scatter_interleaved_kernel(
         const uint8_t* __restrict__ flat,
@@ -50,9 +44,8 @@ __global__ void pq_scatter_interleaved_kernel(
         return;
     const int64_t ls = listStart[assign[i]];
     uint8_t* base = arenaCodes + ls * M;
-    const int t = off & 31;
-    for (int j = lane_id(); j < M; j += 32)
-        base[interleaved_pos(off, j, M)] = flat[i * M + ((j ^ t) & (M - 1))];
+    for (int b = lane_id(); b < M; b += 32)
+        base[ivfInterleavedByte(off, b, M)] = flat[i * M + b];
     if (lane_id() == 0)
         arenaIds[ls + off] = ids[i];
 }
@@ -62,8 +55,8 @@ __global__ void pq_list_to_interleaved_kernel(const uint8_t* __restrict__ flat, 
     if (e >= len * M)
         return;
     const int64_t v = e / M;
-    const int j = (int)(e - v * M);
-    dst[interleaved_pos(v, j, M)] = flat[v * M + ((j ^ (int)(v & 31)) & (M - 1))];
+    const int b = (int)(e - v * M);
+    dst[ivfInterleavedByte(v, b, M)] = flat[e];
 }
 
 __global__ void pq_list_from_interleaved_kernel(const uint8_t* __restrict__ src, int64_t len, int M, uint8_t* __restrict__ flat) {
@@ -71,8 +64,8 @@ __global__ void pq_list_from_interleaved_kernel(const uint8_t* __restrict__ src,
     if (e >= len * M)
         return;
     const int64_t v = e / M;
-    const int j = (int)(e - v * M);
-    flat[v * M + ((j ^ (int)(v & 31)) & (M - 1))] = src[interleaved_pos(v, j, M)];
+    const int b = (int)(e - v * M);
+    flat[e] = src[ivfInterleavedByte(v, b, M)];
 }
 
 // PRMT with the generic-mode selector (PTX prmt.b32): nibble n picks byte (n & 7) of {a (0-3), b (4-7)};
@@ -566,7 +559,8 @@ void runIvfPqScanInterleaved(
         float* outD,
         idx_t* outI,
         cudaStream_t stream,
-        const uint32_t* slotMask) {
+        const uint32_t* slotMask,
+        const IvfSlotOutput* slots) {
     if (nq == 0)
         return;
     FB_THROW_IF_NOT(ivfPqInterleavedSupported(M));
@@ -606,7 +600,7 @@ void runIvfPqScanInterleaved(
                 });
             });
         });
-    });
+    }, slots);
 }
 
 } // namespace fb200

@@ -9,6 +9,8 @@
 
 namespace fb200 {
 
+struct IvfSlotOutput; // ivf_reconstruct.cu section below
+
 // ---------------------------------------------------------------- flat_exact.cu
 // ||x||^2 per row (role of runL2Norm, faiss/gpu/impl/L2Norm.cu:176)
 void runL2Norms(const float* x, int64_t n, int d, float* norms, cudaStream_t stream);
@@ -142,8 +144,11 @@ void runCalcResidual(
         float* out,
         cudaStream_t stream,
         int yHalf = 0);
-// gather rows by id (reconstruct_batch) / by range
-void runGatherRows(const void* src, const idx_t* ids, int64_t n, int d, float* out, cudaStream_t stream, int yHalf = 0);
+// gather rows by id (reconstruct_batch) / by range; id < 0 gives a NaN row, or all 0xFF bytes with missingAllOnes (a
+// missing search result's reconstruction)
+void runGatherRows(
+        const void* src, const idx_t* ids, int64_t n, int d, float* out, cudaStream_t stream, int yHalf = 0,
+        bool missingAllOnes = false);
 
 // ---------------------------------------------------------------- kmeans.cu
 // centroid update (role of compute_centroids, faiss/impl/ClusteringHelpers.cpp:101-172):
@@ -231,7 +236,8 @@ void runIvfFlatScan(
         float* outD,
         idx_t* outI,
         cudaStream_t stream,
-        const uint32_t* slotMask = nullptr); // SearchParameters::sel over the arena, or null
+        const uint32_t* slotMask = nullptr, // SearchParameters::sel over the arena, or null
+        const IvfSlotOutput* slots = nullptr); // the slot-keeping search, or null
 
 // IVF-PQ list scan (role of runPQScanMultiPassNoPrecomputed + pqCodeDistances,
 // faiss/gpu/impl/PQScanMultiPassNoPrecomputed-inl.cuh:527, PQCodeDistances-inl.cuh:591): the
@@ -263,7 +269,69 @@ void runIvfPqScan(
         float* outD,
         idx_t* outI,
         cudaStream_t stream,
-        const uint32_t* slotMask = nullptr); // SearchParameters::sel over the arena, or null
+        const uint32_t* slotMask = nullptr, // SearchParameters::sel over the arena, or null
+        const IvfSlotOutput* slots = nullptr); // the slot-keeping search, or null
+
+// ---------------------------------------------------------------- ivf_reconstruct.cu
+// What a decoder needs to know about an IVF index's stored lists (all pointers on the device).  Every entry is
+// addressed by its arena slot; lists start in ascending list order, so a slot's list is found by bisection.
+enum IvfStoredKind { IVF_STORED_FLAT = 0, IVF_STORED_SQ = 1, IVF_STORED_PQ = 2 };
+struct IvfStoredLayout {
+    int kind = IVF_STORED_FLAT;
+    int d = 0;
+    int codeSize = 0;         // bytes of one CPU code (fp32 row for IVF-Flat)
+    bool interleaved = false; // codes in the interleaved-by-32 layout (8-bit PQ, M in {16, 32}; 4-bit nibble pairs)
+    const int64_t* listStart = nullptr;
+    const int* listLen = nullptr;
+    int64_t nlist = 0;
+    int64_t arenaElems = 0;
+    const uint8_t* codes = nullptr;
+    const idx_t* ids = nullptr;
+    const float* centroids = nullptr; // coarse centroid added to every decoded entry of its list, or null
+    // SQ: codec of ivf_layout.cuh, decode x = vmin + (c + 0.5) / levels * vdiff per dimension; levels 0: x = c
+    int sqCodec = 0;
+    float levels = 0.f;
+    const float* vmin = nullptr;
+    const float* vdiff = nullptr;
+    // PQ: codebooks [M][2^nbits][d / M], codes LSB-first bitstrings
+    int M = 0, nbits = 8;
+    const float* pq = nullptr;
+};
+
+// out[i] = i: a table of arena slots the list scans read as their id table, so that they return positions
+void runIvfIdentitySlots(idx_t* out, int64_t n, cudaStream_t stream);
+// runMergeTopKKeyspace over partial results holding arena positions: each position becomes its stored id on the way in
+// (same keys, ids and tie order as the plain merge) and is returned in outSlot beside it (-1 with the id -1)
+void runIvfMergeTopKSlots(
+        const float* inD,
+        const idx_t* inPos,
+        const idx_t* arenaIds,
+        int64_t rows,
+        int nlists,
+        int kin,
+        int k,
+        MetricType metric,
+        float* outD,
+        idx_t* outI,
+        idx_t* outSlot,
+        cudaStream_t stream);
+// slots[id - i0] = the largest arena slot storing id, for i0 <= id < i0 + ni; -1 where no entry has that id
+void runIvfSlotsOfRange(const IvfStoredLayout& a, idx_t i0, idx_t ni, idx_t* slots, cudaStream_t stream);
+// slots[i] = the largest arena slot storing keys[i], or -1; returns false when some key is not stored (synchronises)
+bool runIvfSlotsOfKeys(
+        GpuResources* res, int device, const IvfStoredLayout& a, const idx_t* keys, int64_t n, idx_t* slots, cudaStream_t stream);
+// out[i] = the CPU's reconstruct_from_offset of the entry at slots[i]; slot -1: all 0xFF bytes (fillMissing) or untouched
+void runIvfReconstruct(const IvfStoredLayout& a, const idx_t* slots, int64_t n, bool fillMissing, float* out, cudaStream_t stream);
+// out[i] = [listno, listnoBytes little-endian bytes][the CPU code bytes] of the entry at slots[i]; slot -1: all 0xFF
+void runIvfGatherCodes(const IvfStoredLayout& a, const idx_t* slots, int64_t n, int listnoBytes, uint8_t* out, cudaStream_t stream);
+
+// the slot-keeping variant of a list scan: the scan is handed `identity` as its id table, so its partial results hold
+// arena positions, and runIvfScanBatches merges them with runIvfMergeTopKSlots against the real ids
+struct IvfSlotOutput {
+    const idx_t* identity;
+    const idx_t* arenaIds;
+    idx_t* outSlot; // [nq][k], beside outD / outI
+};
 
 // ---------------------------------------------------------------- ivfsq_scan.cu
 // ScalarQuantizer::QuantizerType values (faiss/impl/ScalarQuantizer.h:27-34) the GPU index accepts
@@ -325,7 +393,8 @@ void runIvfSqScan(
         float* outD,
         idx_t* outI,
         cudaStream_t stream,
-        const uint32_t* slotMask = nullptr); // SearchParameters::sel over the arena, or null
+        const uint32_t* slotMask = nullptr, // SearchParameters::sel over the arena, or null
+        const IvfSlotOutput* slots = nullptr); // the slot-keeping search, or null
 
 // ---- "rotated, interleaved-by-32" PQ code layout (native storage for M % 16 == 0, M <= 32) ----
 // List-relative vector v = 32*g + t is stored in group g; byte position j of the vector holds
@@ -386,6 +455,7 @@ void runIvfPqScanInterleaved(
         float* outD,
         idx_t* outI,
         cudaStream_t stream,
-        const uint32_t* slotMask = nullptr); // SearchParameters::sel over the arena, or null
+        const uint32_t* slotMask = nullptr, // SearchParameters::sel over the arena, or null
+        const IvfSlotOutput* slots = nullptr); // the slot-keeping search, or null
 
 } // namespace fb200

@@ -238,6 +238,15 @@ FB200_API int faiss_SearchParametersIVF_new_with_sel(FaissSearchParametersIVF** 
 /* c_api/Index_c.h faiss_Index_search_with_params: per-call nprobe for IVF indexes (max_codes must be 0) and an
    IDSelector for GPU indexes */
 FB200_API int faiss_Index_search_with_params(const FaissIndex* index, idx_t n, const float* x, idx_t k, const FaissSearchParameters* params, float* distances, idx_t* labels);
+/* faiss::Index::search_and_reconstruct (GpuIndexFlat and the IVF indexes; params may be NULL): distances / labels as
+   faiss_Index_search_with_params, recons [n][k][d] the stored vector of each result (all 0xFF bytes for label -1).
+   IVF: the entry the search returned, decoded as IndexIVF::reconstruct_from_offset. */
+FB200_API int faiss_Index_search_and_reconstruct(const FaissIndex* index, idx_t n, const float* x, idx_t k, const FaissSearchParameters* params, float* distances, idx_t* labels, float* recons);
+/* faiss::IndexIVF::search_and_return_codes: codes [n][k][(include_listno ? coarse code size : 0) + code size], the
+   CPU inverted-list bytes of each result, prefixed by its list number (little-endian); all 0xFF for label -1 */
+FB200_API int faiss_GpuIndexIVF_search_and_return_codes(const FaissGpuIndex* index, idx_t n, const float* x, idx_t k, const FaissSearchParameters* params, float* distances, idx_t* labels, uint8_t* codes, int include_listno);
+/* IndexIVF::coarse_code_size and code_size: the byte widths of a search_and_return_codes row */
+FB200_API int faiss_GpuIndexIVF_code_sizes(const FaissGpuIndex* index, int* coarse_code_size, int* code_size);
 /* polled between query pages, add pages and clustering iterations; non-zero return -> the running call fails with
    "computation interrupted" (-2).  NULL clears it. */
 FB200_API void faiss_b200_set_interrupt_callback(int (*want_interrupt)(void* ctx), void* ctx);
