@@ -829,6 +829,229 @@ class GpuIndexIVFScalarQuantizer(GpuIndexIVF):
         check(lib.faiss_GpuIndexIVFScalarQuantizer_set_rangestat(self._h, int(rangestat), ctypes.c_float(rangestat_arg)))
 
 
+# faiss::gpu::graph_build_algo, codebook_gen, search_algo, hash_mode (faiss/gpu/GpuIndexCagra.h:44-204)
+graph_build_algo_IVF_PQ = 0
+graph_build_algo_NN_DESCENT = 1
+graph_build_algo_ITERATIVE_SEARCH = 2
+codebook_gen_PER_SUBSPACE = 0
+codebook_gen_PER_CLUSTER = 1
+search_algo_SINGLE_CTA = 0
+search_algo_MULTI_CTA = 1
+search_algo_MULTI_KERNEL = 2
+search_algo_AUTO = 100
+hash_mode_HASH = 0
+hash_mode_SMALL = 1
+hash_mode_AUTO = 100
+
+
+class _CagraConfigC(ctypes.Structure):
+    """FaissGpuIndexCagraConfig (include/faiss_b200_c.h)"""
+
+    _fields_ = [
+        ("device", ctypes.c_int),
+        ("intermediate_graph_degree", ctypes.c_size_t),
+        ("graph_degree", ctypes.c_size_t),
+        ("build_algo", ctypes.c_int),
+        ("nn_descent_niter", ctypes.c_size_t),
+        ("refine_rate", ctypes.c_float),
+        ("store_dataset", ctypes.c_int),
+        ("guarantee_connectivity", ctypes.c_int),
+        ("n_lists", ctypes.c_uint32),
+        ("kmeans_n_iters", ctypes.c_uint32),
+        ("kmeans_trainset_fraction", ctypes.c_double),
+        ("pq_bits", ctypes.c_uint32),
+        ("pq_dim", ctypes.c_uint32),
+        ("codebook_kind", ctypes.c_int),
+        ("force_random_rotation", ctypes.c_int),
+        ("conservative_memory_allocation", ctypes.c_int),
+        ("n_probes", ctypes.c_uint32),
+        ("max_internal_batch_size", ctypes.c_uint32),
+    ]
+
+
+class _CagraSearchC(ctypes.Structure):
+    """FaissSearchParametersCagraConfig (include/faiss_b200_c.h)"""
+
+    _fields_ = [
+        ("max_queries", ctypes.c_size_t),
+        ("itopk_size", ctypes.c_size_t),
+        ("max_iterations", ctypes.c_size_t),
+        ("algo", ctypes.c_int),
+        ("team_size", ctypes.c_size_t),
+        ("search_width", ctypes.c_size_t),
+        ("min_iterations", ctypes.c_size_t),
+        ("thread_block_size", ctypes.c_size_t),
+        ("hashmap_mode", ctypes.c_int),
+        ("hashmap_min_bitlen", ctypes.c_size_t),
+        ("hashmap_max_fill_rate", ctypes.c_float),
+        ("num_random_samplings", ctypes.c_uint32),
+        ("seed", ctypes.c_uint64),
+    ]
+
+
+def _defaults(struct, init):
+    c = struct()
+    init(ctypes.byref(c))
+    return c
+
+
+class IVFPQBuildCagraConfig:
+    """faiss::gpu::IVFPQBuildCagraConfig (faiss/gpu/GpuIndexCagra.h:59-127)"""
+
+    _names = ("n_lists", "kmeans_n_iters", "kmeans_trainset_fraction", "pq_bits", "pq_dim", "codebook_kind",
+              "force_random_rotation", "conservative_memory_allocation")
+
+    def __init__(self):
+        c = _defaults(_CagraConfigC, lib.faiss_GpuIndexCagraConfig_init)
+        for n in self._names:
+            setattr(self, n, getattr(c, n))
+
+
+class IVFPQSearchCagraConfig:
+    """faiss::gpu::IVFPQSearchCagraConfig (faiss/gpu/GpuIndexCagra.h:129-174); lut_dtype, internal_distance_dtype and
+    preferred_shmem_carveout are accepted and have no effect"""
+
+    def __init__(self):
+        c = _defaults(_CagraConfigC, lib.faiss_GpuIndexCagraConfig_init)
+        self.n_probes = c.n_probes
+        self.max_internal_batch_size = c.max_internal_batch_size
+        self.lut_dtype = None
+        self.internal_distance_dtype = None
+        self.preferred_shmem_carveout = 1.0
+
+
+class GpuIndexCagraConfig:
+    """faiss::gpu::GpuIndexCagraConfig (faiss/gpu/GpuIndexCagra.h:176-193)"""
+
+    _names = ("device", "intermediate_graph_degree", "graph_degree", "build_algo", "nn_descent_niter", "refine_rate",
+              "store_dataset", "guarantee_connectivity")
+
+    def __init__(self):
+        c = _defaults(_CagraConfigC, lib.faiss_GpuIndexCagraConfig_init)
+        for n in self._names:
+            setattr(self, n, getattr(c, n))
+        self.store_dataset = bool(self.store_dataset)
+        self.guarantee_connectivity = bool(self.guarantee_connectivity)
+        self.ivf_pq_params = None  # None: IVFPQBuildCagraConfig()
+        self.ivf_pq_search_params = None  # None: IVFPQSearchCagraConfig()
+
+    def _c(self):
+        c = _defaults(_CagraConfigC, lib.faiss_GpuIndexCagraConfig_init)
+        for n in self._names:
+            setattr(c, n, type(getattr(c, n))(getattr(self, n)))
+        bp = self.ivf_pq_params or IVFPQBuildCagraConfig()
+        for n in IVFPQBuildCagraConfig._names:
+            setattr(c, n, type(getattr(c, n))(getattr(bp, n)))
+        sp = self.ivf_pq_search_params or IVFPQSearchCagraConfig()
+        c.n_probes = int(sp.n_probes)
+        c.max_internal_batch_size = int(sp.max_internal_batch_size)
+        return c
+
+
+class SearchParametersCagra(SearchParameters):
+    """faiss::gpu::SearchParametersCagra (faiss/gpu/GpuIndexCagra.h:206-251).  Fields may be set after construction;
+    a search reads them when it starts."""
+
+    _names = tuple(f[0] for f in _CagraSearchC._fields_)
+
+    def __init__(self, sel=None, **kw):
+        self.sel = sel
+        self._handle = None
+        c = _defaults(_CagraSearchC, lib.faiss_SearchParametersCagraConfig_init)
+        for n in self._names:
+            setattr(self, n, getattr(c, n))
+        for n, v in kw.items():
+            assert n in self._names, "unknown SearchParametersCagra field %s" % n
+            setattr(self, n, v)
+
+    @property
+    def _h(self):
+        c = _defaults(_CagraSearchC, lib.faiss_SearchParametersCagraConfig_init)
+        for n in self._names:
+            setattr(c, n, type(getattr(c, n))(getattr(self, n)))
+        self._free()
+        self._handle = ctypes.c_void_p()
+        check(lib.faiss_SearchParametersCagra_new(
+            ctypes.byref(self._handle), self.sel._h if self.sel is not None else None, ctypes.byref(c)))
+        return self._handle
+
+    def _free(self):
+        if getattr(self, "_handle", None) and lib is not None:
+            lib.faiss_SearchParameters_free(self._handle)
+            self._handle = None
+
+    def __del__(self):
+        self._free()
+
+
+class GpuIndexCagra(Index):
+    """faiss::gpu::GpuIndexCagra (faiss/gpu/GpuIndexCagra.h:253-379): fp32, METRIC_L2 / METRIC_INNER_PRODUCT.
+    train (or add) builds the graph on the device: IVF-PQ candidates, exact refine, optimise (DESIGN "GpuIndexCagra").
+    Search takes SearchParametersCagra through params=."""
+
+    def __init__(self, res, d, metric=METRIC_L2, config=None):
+        super().__init__()
+        self._keep.append(res)
+        c = (config or GpuIndexCagraConfig())._c()
+        check(lib.faiss_GpuIndexCagra_new(ctypes.byref(self._h), res._h, int(d), int(metric), ctypes.byref(c)))
+
+    @property
+    def graph_degree(self):
+        out = ctypes.c_int()
+        check(lib.faiss_GpuIndexCagra_graph_degree(self._h, ctypes.byref(out)))
+        return out.value
+
+    def get_knngraph(self):
+        """[ntotal, graph_degree] int64 (-1: no edge)"""
+        out = np.empty((self.ntotal, self.graph_degree), dtype=np.int64)
+        check(lib.faiss_GpuIndexCagra_get_knngraph(self._h, _ptr(out, _c_i64)))
+        return out
+
+    def copyFrom(self, xb, graph):
+        """the IndexHNSWCagra payload: xb [n, d], graph [n, degree] int64 (its level-0 table; -1 entries are skipped)"""
+        xb = _as_f32(xb)
+        graph = np.ascontiguousarray(graph, dtype=np.int64)
+        assert graph.ndim == 2 and graph.shape[0] == xb.shape[0] and xb.shape[1] == self.d
+        check(lib.faiss_GpuIndexCagra_copyFrom(
+            self._h, ctypes.c_int64(xb.shape[0]), _ptr(xb, _c_f), _ptr(graph, _c_i64), int(graph.shape[1])))
+
+    def copyTo(self):
+        """-> (xb [ntotal, d] float32, graph [ntotal, graph_degree] int64)"""
+        xb = np.empty((self.ntotal, self.d), dtype=np.float32)
+        graph = np.empty((self.ntotal, self.graph_degree), dtype=np.int64)
+        check(lib.faiss_GpuIndexCagra_copyTo(self._h, _ptr(xb, _c_f), _ptr(graph, _c_i64)))
+        return xb, graph
+
+    def lastSearchDistanceCount(self):
+        """distance evaluations of the last search, summed over its queries"""
+        out = ctypes.c_int64()
+        check(lib.faiss_GpuIndexCagra_lastSearchDistanceCount(self._h, ctypes.byref(out)))
+        return out.value
+
+    def lastBuildSeconds(self):
+        """{"ivf_pq", "refine", "optimize"}: seconds of the last build's three stages"""
+        out = (ctypes.c_double * 3)()
+        check(lib.faiss_GpuIndexCagra_lastBuildSeconds(self._h, out))
+        return {"ivf_pq": out[0], "refine": out[1], "optimize": out[2]}
+
+
+def cagra_optimize(res, G0, K, device=0):
+    """The build's graph optimisation on its own (b200_cagra_optimize): G0 [n, K0] -> G [n, K], uint32 ids.  G0 may be a
+    numpy array or a CUDA tensor (int32 / int64 / uint32 values); the result follows its residency as int64."""
+    import torch
+
+    t = G0 if _is_torch(G0) else torch.from_numpy(np.ascontiguousarray(G0).astype(np.int64))
+    g0 = t.to(device="cuda:%d" % device, dtype=torch.int64).to(torch.int32).contiguous()
+    n, K0 = g0.shape
+    G = torch.empty((n, int(K)), dtype=torch.int32, device=g0.device)
+    torch.cuda.synchronize(g0.device)
+    check(lib.b200_cagra_optimize(res._h, int(device), ctypes.c_void_p(g0.data_ptr()), ctypes.c_int64(n), int(K0), int(K),
+                                  ctypes.c_void_p(G.data_ptr())))
+    res.syncDefaultStream(device)
+    out = G.to(torch.int64) & 0xFFFFFFFF
+    return out if _is_torch(G0) else out.cpu().numpy()
+
+
 class IndexShards(Index):
     """faiss::IndexShards (faiss/IndexShards.h:21-106)."""
 

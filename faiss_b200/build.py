@@ -19,6 +19,8 @@ FLAGS = [
     "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "--expt-relaxed-constexpr", "-I" + os.path.join(HERE, "..", "include"), "-I" + SRC,
 ]
+# per-file additions: the CAGRA search kernel reports its registers, shared memory and spills at every build
+FILE_FLAGS = {"cagra_search.cu": ["-Xptxas", "-v"]}
 
 
 def _sources():
@@ -52,7 +54,7 @@ def build(jobs=None, force=False, verbose=True):
 
     def cc(so):
         s, o = so
-        cmd = [NVCC] + FLAGS + ["-x", "cu", "-c", s, "-o", o]
+        cmd = [NVCC] + FLAGS + FILE_FLAGS.get(os.path.basename(s), []) + ["-x", "cu", "-c", s, "-o", o]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("nvcc failed for %s:\n%s\n%s" % (s, r.stdout, r.stderr))

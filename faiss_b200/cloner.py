@@ -11,6 +11,8 @@ a file reader -- can feed them; nothing here depends on the reference's classes.
                "pq" [M, 2^nbits, dsub] f32 (IVFPQ only; nbits != 8 builds the index with interleaved_layout),
                "sq" {"qtype", "by_residual", "trained" f32} (IVF scalar quantiser only: ScalarQuantizer::trained),
                "codes": [nlist] uint8 arrays, "ids": [nlist] int64 arrays}
+
+    cagra payload = {"d", "metric", "xb" [n, d] f32, "graph" [n, degree] int64}   (GpuIndexCagra <-> IndexHNSWCagra)
 """
 import numpy as np
 
@@ -133,3 +135,25 @@ def gpu_ivf_shards_from_payload(resources, payload, shard_type=SHARD_BY_ID_MOD, 
         sub["codes"], sub["ids"] = ci, ii
         shards.add_shard(gpu_ivf_from_payload(r, sub, device=dev))
     return shards
+
+
+# ------------------------------------------------------------------------------------------------
+# GpuIndexCagra <-> IndexHNSWCagra: the "cagra" payload {"d", "metric", "xb" [n, d] f32, "graph" [n, degree] int64}
+# is what GpuIndexCagra::copyFrom(IndexHNSWCagra*) and copyTo move (faiss/gpu/GpuIndexCagra.cu copyFrom_ex / copyTo):
+# the stored vectors and the level-0 neighbour table (-1: no edge).
+# ------------------------------------------------------------------------------------------------
+def cagra_payload(index):
+    """the payload of a built GpuIndexCagra"""
+    xb, graph = index.copyTo()
+    return {"d": int(index.d), "metric": int(index.metric_type), "xb": xb, "graph": graph}
+
+
+def gpu_cagra_from_payload(res, payload, device=0):
+    """a GpuIndexCagra holding exactly the payload's vectors and graph"""
+    import faiss_b200 as fb
+
+    cfg = fb.GpuIndexCagraConfig()
+    cfg.device = int(device)
+    index = fb.GpuIndexCagra(res, int(payload["d"]), int(payload.get("metric", fb.METRIC_L2)), cfg)
+    index.copyFrom(payload["xb"], payload["graph"])
+    return index

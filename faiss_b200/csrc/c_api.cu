@@ -796,6 +796,144 @@ int faiss_SearchParametersIVF_new_with_sel(FaissSearchParametersIVF** out, Faiss
     }
     CATCH_AND_HANDLE
 }
+// ---------------------------------------------------------------- GpuIndexCagra
+void faiss_GpuIndexCagraConfig_init(FaissGpuIndexCagraConfig* c) {
+    const GpuIndexCagraConfig d;
+    c->device = d.device;
+    c->intermediate_graph_degree = d.intermediate_graph_degree;
+    c->graph_degree = d.graph_degree;
+    c->build_algo = (int)d.build_algo;
+    c->nn_descent_niter = d.nn_descent_niter;
+    c->refine_rate = d.refine_rate;
+    c->store_dataset = d.store_dataset;
+    c->guarantee_connectivity = d.guarantee_connectivity;
+    c->n_lists = d.ivf_pq_params.n_lists;
+    c->kmeans_n_iters = d.ivf_pq_params.kmeans_n_iters;
+    c->kmeans_trainset_fraction = d.ivf_pq_params.kmeans_trainset_fraction;
+    c->pq_bits = d.ivf_pq_params.pq_bits;
+    c->pq_dim = d.ivf_pq_params.pq_dim;
+    c->codebook_kind = (int)d.ivf_pq_params.codebook_kind;
+    c->force_random_rotation = d.ivf_pq_params.force_random_rotation;
+    c->conservative_memory_allocation = d.ivf_pq_params.conservative_memory_allocation;
+    c->n_probes = d.ivf_pq_search_params.n_probes;
+    c->max_internal_batch_size = d.ivf_pq_search_params.max_internal_batch_size;
+}
+int faiss_GpuIndexCagra_new(FaissGpuIndex** p, FaissStandardGpuResources* r, int d, FaissMetricType metric, const FaissGpuIndexCagraConfig* cc) {
+    try {
+        FB_THROW_IF_NOT_MSG(p != nullptr && cc != nullptr, "null argument");
+        auto res = RES(r);
+        GpuIndexCagraConfig c;
+        c.device = cc->device;
+        c.intermediate_graph_degree = cc->intermediate_graph_degree;
+        c.graph_degree = cc->graph_degree;
+        c.build_algo = (graph_build_algo)cc->build_algo;
+        c.nn_descent_niter = cc->nn_descent_niter;
+        c.refine_rate = cc->refine_rate;
+        c.store_dataset = cc->store_dataset != 0;
+        c.guarantee_connectivity = cc->guarantee_connectivity != 0;
+        c.ivf_pq_params.n_lists = cc->n_lists;
+        c.ivf_pq_params.kmeans_n_iters = cc->kmeans_n_iters;
+        c.ivf_pq_params.kmeans_trainset_fraction = cc->kmeans_trainset_fraction;
+        c.ivf_pq_params.pq_bits = cc->pq_bits;
+        c.ivf_pq_params.pq_dim = cc->pq_dim;
+        c.ivf_pq_params.codebook_kind = (codebook_gen)cc->codebook_kind;
+        c.ivf_pq_params.force_random_rotation = cc->force_random_rotation != 0;
+        c.ivf_pq_params.conservative_memory_allocation = cc->conservative_memory_allocation != 0;
+        c.ivf_pq_search_params.n_probes = cc->n_probes;
+        c.ivf_pq_search_params.max_internal_batch_size = cc->max_internal_batch_size;
+        std::unique_ptr<Index> ix(new GpuIndexCagra(res, d, MT_L2IP(metric), c));
+        *p = new FaissIndex_H{ix.release(), res};
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexCagra_graph_degree(const FaissGpuIndex* p, int* degree) {
+    try {
+        *degree = AS<GpuIndexCagra>(p, "GpuIndexCagra")->graphDegree();
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexCagra_get_knngraph(const FaissGpuIndex* p, idx_t* graph) {
+    try {
+        auto g = AS<GpuIndexCagra>(p, "GpuIndexCagra")->get_knngraph();
+        std::memcpy(graph, g.data(), g.size() * sizeof(idx_t));
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexCagra_copyFrom(FaissGpuIndex* p, idx_t n, const float* xb, const idx_t* graph, int degree) {
+    try {
+        AS<GpuIndexCagra>(p, "GpuIndexCagra")->copyFrom(n, xb, graph, degree);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexCagra_copyTo(const FaissGpuIndex* p, float* xb, idx_t* graph) {
+    try {
+        AS<GpuIndexCagra>(p, "GpuIndexCagra")->copyTo(xb, graph);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexCagra_lastSearchDistanceCount(const FaissGpuIndex* p, int64_t* count) {
+    try {
+        *count = AS<GpuIndexCagra>(p, "GpuIndexCagra")->lastSearchDistanceCount;
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIndexCagra_lastBuildSeconds(const FaissGpuIndex* p, double* seconds3) {
+    try {
+        const auto* ix = AS<GpuIndexCagra>(p, "GpuIndexCagra");
+        for (int i = 0; i < 3; i++)
+            seconds3[i] = ix->lastBuildSeconds[i];
+    }
+    CATCH_AND_HANDLE
+}
+void faiss_SearchParametersCagraConfig_init(FaissSearchParametersCagraConfig* c) {
+    const SearchParametersCagra d;
+    c->max_queries = d.max_queries;
+    c->itopk_size = d.itopk_size;
+    c->max_iterations = d.max_iterations;
+    c->algo = (int)d.algo;
+    c->team_size = d.team_size;
+    c->search_width = d.search_width;
+    c->min_iterations = d.min_iterations;
+    c->thread_block_size = d.thread_block_size;
+    c->hashmap_mode = (int)d.hashmap_mode;
+    c->hashmap_min_bitlen = d.hashmap_min_bitlen;
+    c->hashmap_max_fill_rate = d.hashmap_max_fill_rate;
+    c->num_random_samplings = d.num_random_samplings;
+    c->seed = d.seed;
+}
+int faiss_SearchParametersCagra_new(FaissSearchParametersCagra** out, FaissIDSelector* sel, const FaissSearchParametersCagraConfig* c) {
+    try {
+        FB_THROW_IF_NOT_MSG(out != nullptr && c != nullptr, "null argument");
+        auto sp = std::make_unique<SearchParametersCagra>();
+        sp->sel = sel ? SEL(sel) : nullptr;
+        sp->max_queries = c->max_queries;
+        sp->itopk_size = c->itopk_size;
+        sp->max_iterations = c->max_iterations;
+        sp->algo = (search_algo)c->algo;
+        sp->team_size = c->team_size;
+        sp->search_width = c->search_width;
+        sp->min_iterations = c->min_iterations;
+        sp->thread_block_size = c->thread_block_size;
+        sp->hashmap_mode = (hash_mode)c->hashmap_mode;
+        sp->hashmap_min_bitlen = c->hashmap_min_bitlen;
+        sp->hashmap_max_fill_rate = c->hashmap_max_fill_rate;
+        sp->num_random_samplings = c->num_random_samplings;
+        sp->seed = c->seed;
+        *out = new FaissSearchParameters_H{sp.release()};
+    }
+    CATCH_AND_HANDLE
+}
+int b200_cagra_optimize(FaissStandardGpuResources* r, int device, const uint32_t* G0, int64_t n, int K0, int K, uint32_t* G) {
+    try {
+        auto res = RES(r);
+        DeviceScope scope(device);
+        res->initializeForDevice(device);
+        auto stream = res->getDefaultStream(device);
+        runCagraOptimize(res.get(), device, G0, n, K0, K, G, stream);
+    }
+    CATCH_AND_HANDLE
+}
+
 void faiss_SearchParameters_free(FaissSearchParameters* p) {
     if (p) {
         delete p->p;

@@ -296,6 +296,7 @@ void GpuIndex::search(idx_t n, const float* x, idx_t k, float* distances, idx_t*
         DeviceView<float> xv(resources_.get(), config_.device, x + (size_t)i0 * d, (size_t)nb * d, stream);
         DeviceOut<float> dv(resources_.get(), config_.device, distances + (size_t)i0 * k, (size_t)nb * k);
         DeviceOut<idx_t> lv(resources_.get(), config_.device, labels + (size_t)i0 * k, (size_t)nb * k);
+        callRow0_ = i0;
         searchImpl_(nb, xv.ptr, (int)k, dv.ptr, lv.ptr);
         dv.finish(stream);
         lv.finish(stream);
@@ -389,6 +390,7 @@ bool GpuIndex::searchFromCpuPaged_(idx_t n, const float* x, idx_t k, float* dist
             CUDA_VERIFY(cudaStreamWaitEvent(stream, ready[b], 0));
             DeviceOut<float> dv(resources_.get(), config_.device, distances + (size_t)i0 * k, (size_t)nb * k);
             DeviceOut<idx_t> lv(resources_.get(), config_.device, labels + (size_t)i0 * k, (size_t)nb * k);
+            callRow0_ = i0;
             searchImpl_(nb, devBuf[b].as<float>(), (int)k, dv.ptr, lv.ptr);
             dv.finish(stream);
             lv.finish(stream);
@@ -2117,6 +2119,201 @@ IvfStoredLayout GpuIndexIVFScalarQuantizer::storedLayout_() const {
     a.vdiff = params_.data() + d;
     a.centroids = by_residual ? quantizer->vectorsDevice() : nullptr;
     return a;
+}
+
+// ------------------------------------------------------------------------------------------
+// GpuIndexCagra
+// ------------------------------------------------------------------------------------------
+GpuIndexCagra::GpuIndexCagra(std::shared_ptr<GpuResources> resources, int dims, MetricType metric, GpuIndexCagraConfig config)
+        : GpuIndex(std::move(resources), dims, metric, 0.f, config),
+          cagraConfig_(config),
+          data_(resources_.get(), config.device, AllocType::FlatData),
+          graph_(resources_.get(), config.device, AllocType::Other) {
+    FB_THROW_IF_NOT_MSG(
+            metric == METRIC_L2 || metric == METRIC_INNER_PRODUCT,
+            "GpuIndexCagra supports METRIC_L2 and METRIC_INNER_PRODUCT only");
+    this->is_trained = false;
+}
+
+void GpuIndexCagra::train(idx_t n, const float* x) {
+    DeviceScope scope(config_.device);
+    if (this->is_trained)
+        return;
+    const GpuIndexCagraConfig& c = cagraConfig_;
+    FB_THROW_IF_NOT_MSG(
+            c.build_algo == graph_build_algo::IVF_PQ,
+            "GpuIndexCagra builds with graph_build_algo IVF_PQ only (NN_DESCENT and ITERATIVE_SEARCH are not implemented)");
+    FB_THROW_IF_NOT_MSG(!c.guarantee_connectivity, "GpuIndexCagra: guarantee_connectivity is not implemented");
+    FB_THROW_IF_NOT_MSG(c.store_dataset, "GpuIndexCagra: store_dataset = false is not implemented (the search reads the stored rows)");
+    FB_THROW_IF_NOT_MSG(
+            c.ivf_pq_params.codebook_kind == codebook_gen::PER_SUBSPACE,
+            "GpuIndexCagra: codebook_kind PER_CLUSTER is not implemented");
+    FB_THROW_IF_NOT_MSG(!c.ivf_pq_params.force_random_rotation, "GpuIndexCagra: force_random_rotation is not implemented");
+    FB_THROW_IF_NOT_MSG(c.refine_rate >= 1.f, "GpuIndexCagra: refine_rate must be >= 1");
+    FB_THROW_IF_NOT_MSG(n >= 2, "GpuIndexCagra needs at least 2 vectors to build a graph");
+    FB_THROW_IF_NOT_MSG(n < (idx_t(1) << 31) - 1, "GpuIndexCagra holds fewer than 2^31 - 1 vectors");
+    FB_THROW_IF_NOT_MSG(c.graph_degree >= 1, "GpuIndexCagra: graph_degree must be >= 1");
+    // K0 <= N - 1 (a row has no more distinct neighbours) and K <= K0 (the prune only drops edges)
+    const int K0 = (int)std::min<idx_t>((idx_t)c.intermediate_graph_degree, n - 1);
+    const int K = (int)std::min<idx_t>((idx_t)c.graph_degree, K0);
+    FB_THROW_IF_NOT_FMT(K0 <= 1024, "GpuIndexCagra: intermediate_graph_degree %d > 1024", K0);
+    auto stream = stream_();
+    try {
+        DeviceView<float> xv(resources_.get(), config_.device, x, (size_t)n * d, stream);
+        data_.clear();
+        data_.reserve((size_t)n * d, stream, true);
+        data_.append(xv.ptr, (size_t)n * d, stream);
+        cagraBuildGraph(resources_, config_.device, data_.data(), n, d, metric_type, c, K0, K, graph_, lastBuildSeconds);
+    } catch (...) {
+        reset();
+        throw;
+    }
+    graphDegree_ = K;
+    this->ntotal = n;
+    this->is_trained = true;
+}
+
+void GpuIndexCagra::add(idx_t n, const float* x) {
+    train(n, x);
+}
+
+void GpuIndexCagra::addImpl_(idx_t, const float*, const idx_t*) {
+    FB_THROW_MSG("adding vectors is not supported by GpuIndexCagra.");
+}
+
+void GpuIndexCagra::reset() {
+    DeviceScope scope(config_.device);
+    data_.clear();
+    graph_.clear();
+    graphDegree_ = 0;
+    this->ntotal = 0;
+    this->is_trained = false;
+}
+
+void GpuIndexCagra::copyFrom(idx_t n, const float* xb, const idx_t* graph, int degree) {
+    DeviceScope scope(config_.device);
+    FB_THROW_IF_NOT_MSG(n >= 1 && n < (idx_t(1) << 31) - 1, "GpuIndexCagra::copyFrom: bad number of vectors");
+    FB_THROW_IF_NOT_MSG(degree >= 1, "GpuIndexCagra::copyFrom: graph degree must be >= 1");
+    auto stream = stream_();
+    std::vector<idx_t> g((size_t)n * degree);
+    CUDA_VERIFY(cudaMemcpy(g.data(), graph, g.size() * sizeof(idx_t), cudaMemcpyDefault));
+    std::vector<uint32_t> g32(g.size());
+    for (size_t i = 0; i < g.size(); i++) {
+        FB_THROW_IF_NOT_FMT(g[i] >= -1 && g[i] < n, "GpuIndexCagra::copyFrom: graph entry %ld out of range", (long)g[i]);
+        g32[i] = g[i] < 0 ? 0xFFFFFFFFu : (uint32_t)g[i];
+    }
+    reset();
+    DeviceView<float> xv(resources_.get(), config_.device, xb, (size_t)n * d, stream);
+    data_.reserve((size_t)n * d, stream, true);
+    data_.append(xv.ptr, (size_t)n * d, stream);
+    graph_.reserve(g32.size(), stream, true);
+    graph_.append(g32.data(), g32.size(), stream);
+    CUDA_VERIFY(cudaStreamSynchronize(stream));
+    graphDegree_ = degree;
+    this->ntotal = n;
+    this->is_trained = true;
+}
+
+std::vector<idx_t> GpuIndexCagra::get_knngraph() const {
+    DeviceScope scope(config_.device);
+    FB_THROW_IF_NOT_MSG(this->is_trained, "GpuIndexCagra: the index is not built");
+    std::vector<uint32_t> g32(graph_.size());
+    CUDA_VERIFY(cudaMemcpy(g32.data(), graph_.data(), g32.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    std::vector<idx_t> g(g32.size());
+    for (size_t i = 0; i < g.size(); i++)
+        g[i] = g32[i] == 0xFFFFFFFFu ? -1 : (idx_t)g32[i];
+    return g;
+}
+
+void GpuIndexCagra::copyTo(float* xb, idx_t* graph) const {
+    auto g = get_knngraph();
+    DeviceScope scope(config_.device);
+    CUDA_VERIFY(cudaMemcpy(xb, data_.data(), sizeof(float) * (size_t)ntotal * d, cudaMemcpyDefault));
+    CUDA_VERIFY(cudaMemcpy(graph, g.data(), sizeof(idx_t) * g.size(), cudaMemcpyDefault));
+}
+
+GpuMemoryReservation GpuIndexCagra::selMask_(const IDSelector&) const {
+    FB_THROW_MSG("GpuIndexCagra does not support SearchParameters::sel");
+}
+
+void GpuIndexCagra::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
+    const SearchParametersCagra defaults;
+    const auto* sp = dynamic_cast<const SearchParametersCagra*>(callParams_);
+    if (!sp)
+        sp = &defaults;
+    FB_THROW_IF_NOT_MSG(
+            sp->algo == search_algo::SINGLE_CTA || sp->algo == search_algo::AUTO,
+            "GpuIndexCagra implements search_algo SINGLE_CTA (and AUTO) only; MULTI_CTA and MULTI_KERNEL are not implemented");
+    FB_THROW_IF_NOT_FMT(sp->itopk_size <= 512, "GpuIndexCagra: itopk_size %zu > 512", sp->itopk_size);
+    FB_THROW_IF_NOT_FMT((size_t)k <= sp->itopk_size, "GpuIndexCagra: k %d > itopk_size %zu", k, sp->itopk_size);
+    FB_THROW_IF_NOT_MSG(sp->search_width >= 1, "GpuIndexCagra: search_width must be >= 1");
+    FB_THROW_IF_NOT_MSG(sp->num_random_samplings >= 1, "GpuIndexCagra: num_random_samplings must be >= 1");
+    FB_THROW_IF_NOT_MSG(
+            sp->team_size == 0 || sp->team_size == 4 || sp->team_size == 8 || sp->team_size == 16 || sp->team_size == 32,
+            "GpuIndexCagra: team_size must be 0, 4, 8, 16 or 32");
+    FB_THROW_IF_NOT_MSG(
+            sp->thread_block_size == 0 || sp->thread_block_size == 64 || sp->thread_block_size == 128 ||
+                    sp->thread_block_size == 256 || sp->thread_block_size == 512 || sp->thread_block_size == 1024,
+            "GpuIndexCagra: thread_block_size must be 0, 64, 128, 256, 512 or 1024");
+    FB_THROW_IF_NOT_MSG(
+            sp->hashmap_max_fill_rate >= 0.1f && sp->hashmap_max_fill_rate <= 0.9f,
+            "GpuIndexCagra: hashmap_max_fill_rate must be in [0.1, 0.9]");
+    FB_THROW_IF_NOT_MSG(sp->hashmap_min_bitlen <= 16, "GpuIndexCagra: hashmap_min_bitlen must be <= 16");
+
+    CagraSearchArgs a{};
+    a.data = data_.data();
+    a.graph = graph_.data();
+    a.n = ntotal;
+    a.d = d;
+    a.graphDegree = graphDegree_;
+    a.metric = metric_type;
+    a.k = k;
+    a.itopk = (int)round_up(std::max<size_t>(sp->itopk_size, 1), 32);
+    a.bufSize = next_pow2(a.itopk);
+    a.searchWidth = (int)sp->search_width;
+    const int64_t gather = (int64_t)a.searchWidth * a.graphDegree;
+    const int64_t numInit = (int64_t)sp->num_random_samplings * gather;
+    FB_THROW_IF_NOT_FMT(gather <= 4096, "GpuIndexCagra: search_width * graph_degree = %ld > 4096", (long)gather);
+    FB_THROW_IF_NOT_FMT(numInit <= 8192, "GpuIndexCagra: num_random_samplings * search_width * graph_degree = %ld > 8192", (long)numInit);
+    a.numInit = (int)numInit;
+    a.candSize = next_pow2((int)std::max(numInit, gather));
+    // automatic cap: twice the iterations that expand every itopk entry once, plus a margin
+    const size_t autoIter = 2 * (size_t)a.itopk / a.searchWidth + 16;
+    a.maxIterations = (int)std::min<size_t>(std::max(sp->max_iterations ? sp->max_iterations : autoIter, sp->min_iterations), 1 << 20);
+    a.teamSize = sp->team_size ? (int)sp->team_size : std::min(32, std::max(4, next_pow2((d + 15) / 16)));
+    a.blockSize = sp->thread_block_size ? (int)sp->thread_block_size : (a.itopk <= 64 ? 64 : a.itopk <= 256 ? 128 : 256);
+    // the visited set holds every id inserted between two refills: at least the initial samples, and itopk plus a few
+    // iterations of gathers
+    const double need = std::max<double>((double)numInit + a.itopk, 4.0 * (a.itopk + gather));
+    int bits = std::max<int>(8, (int)sp->hashmap_min_bitlen);
+    while ((double)(1 << bits) * sp->hashmap_max_fill_rate < need)
+        bits++;
+    FB_THROW_IF_NOT_FMT(bits <= 16, "GpuIndexCagra: the visited set would need 2^%d entries", bits);
+    a.hashBits = bits;
+    a.hashLimit = (int)((double)(1 << bits) * sp->hashmap_max_fill_rate);
+    a.seed = sp->seed;
+    FB_THROW_IF_NOT_MSG(cagraSearchSmemBytes(a) <= 227 * 1024, "GpuIndexCagra: the search does not fit shared memory");
+
+    auto stream = stream_();
+    auto count = resources_->temp(config_.device, sizeof(unsigned long long));
+    CUDA_VERIFY(cudaMemsetAsync(count.data, 0, sizeof(unsigned long long), stream));
+    a.distanceCount = count.as<unsigned long long>();
+    const idx_t batch = sp->max_queries ? (idx_t)sp->max_queries : n;
+    for (idx_t b0 = 0; b0 < n; b0 += batch) {
+        InterruptCallback::check(); // between query batches
+        a.queries = xDev + (size_t)b0 * d;
+        a.nq = std::min(batch, n - b0);
+        a.rowOffset = callRow0_ + b0;
+        a.outD = dDev + (size_t)b0 * k;
+        a.outI = iDev + (size_t)b0 * k;
+        runCagraSearch(a, stream);
+    }
+    unsigned long long hCount = 0;
+    CUDA_VERIFY(cudaMemcpyAsync(&hCount, count.data, sizeof(hCount), cudaMemcpyDeviceToHost, stream));
+    CUDA_VERIFY(cudaStreamSynchronize(stream));
+    if (callRow0_ == 0)
+        lastSearchDistanceCount = 0;
+    lastSearchDistanceCount += (int64_t)hCount;
 }
 
 // ------------------------------------------------------------------------------------------

@@ -123,6 +123,8 @@ class GpuIndex : public Index {
    protected:
     // the per-call parameters of the search in flight (an index instance is not re-entrant, as upstream)
     mutable const SearchParameters* callParams_ = nullptr;
+    // the row, in the whole search call, of the first query handed to searchImpl_ (set by the query paging)
+    mutable idx_t callRow0_ = 0;
     // callParams_->sel evaluated once per call over the index's storage slots (idselector.h), else null
     mutable const uint32_t* callMask_ = nullptr;
     // sel over this index's slots into a device mask of slotMaskWords(slots) words (temporary memory)
@@ -723,6 +725,106 @@ class GpuIndexIVFScalarQuantizer : public GpuIndexIVF {
     std::vector<float> trained_;
     DeviceVector<float> params_; // [4][d]: vmin | vdiff (encode) | m | b (scan decode x = m + b * code)
 };
+
+// ------------------------------------------------------------------------------------------
+// GpuIndexCagra (faiss/gpu/GpuIndexCagra.h:41-380): a graph index built and searched on the device
+// ------------------------------------------------------------------------------------------
+enum class graph_build_algo { IVF_PQ = 0, NN_DESCENT = 1, ITERATIVE_SEARCH = 2 }; // only IVF_PQ is implemented
+enum class codebook_gen { PER_SUBSPACE = 0, PER_CLUSTER = 1 };                   // only PER_SUBSPACE is implemented
+enum class search_algo { SINGLE_CTA = 0, MULTI_CTA = 1, MULTI_KERNEL = 2, AUTO = 100 }; // AUTO runs SINGLE_CTA
+enum class hash_mode { HASH = 0, SMALL = 1, AUTO = 100 }; // accepted; the visited set is always in shared memory
+
+struct IVFPQBuildCagraConfig {
+    uint32_t n_lists = 1024;               // clamped so that k-means gets >= 39 training rows per list
+    uint32_t kmeans_n_iters = 20;
+    double kmeans_trainset_fraction = 0.5; // the k-means and PQ training subsample
+    uint32_t pq_bits = 8;                  // any width GpuIndexIVFPQ takes (4, 5, 6 with its interleaved layout)
+    uint32_t pq_dim = 0;                   // 0: the largest divisor of d that is <= min(32, d / 2)
+    codebook_gen codebook_kind = codebook_gen::PER_SUBSPACE;
+    bool force_random_rotation = false;    // must stay false
+    bool conservative_memory_allocation = false; // accepted, no effect
+};
+
+struct IVFPQSearchCagraConfig {
+    uint32_t n_probes = 20;
+    int lut_dtype = 0;                     // accepted, no effect (the LUT is fp32)
+    int internal_distance_dtype = 0;       // accepted, no effect
+    double preferred_shmem_carveout = 1.0; // accepted, no effect
+    uint32_t max_internal_batch_size = 4096; // rows per candidate self-search page
+};
+
+struct GpuIndexCagraConfig : GpuIndexConfig {
+    size_t intermediate_graph_degree = 128; // K0, clamped to N - 1
+    size_t graph_degree = 64;               // K, clamped to K0
+    graph_build_algo build_algo = graph_build_algo::IVF_PQ;
+    size_t nn_descent_niter = 20;           // NN_DESCENT is not implemented
+    IVFPQBuildCagraConfig ivf_pq_params;
+    IVFPQSearchCagraConfig ivf_pq_search_params;
+    float refine_rate = 2.0f;               // >= 1
+    bool store_dataset = true;              // must stay true: the search reads the stored rows
+    bool guarantee_connectivity = false;    // must stay false
+};
+
+struct SearchParametersCagra : SearchParameters {
+    size_t max_queries = 0;     // queries per launch; 0: the whole page
+    size_t itopk_size = 64;     // rounded up to a multiple of 32; <= 512 and >= k
+    size_t max_iterations = 0;  // 0: 2 * itopk / search_width + 16 (itopk rounded)
+    search_algo algo = search_algo::AUTO;
+    size_t team_size = 0;       // lanes per distance: 4, 8, 16, 32; 0: by d
+    size_t search_width = 1;
+    size_t min_iterations = 0;
+    size_t thread_block_size = 0; // 64 ... 1024; 0: by itopk
+    hash_mode hashmap_mode = hash_mode::AUTO;
+    size_t hashmap_min_bitlen = 0;
+    float hashmap_max_fill_rate = 0.5f;
+    uint32_t num_random_samplings = 1;
+    uint64_t seed = 0x128394;
+};
+
+class GpuIndexCagra : public GpuIndex {
+   public:
+    GpuIndexCagra(
+            std::shared_ptr<GpuResources> resources,
+            int dims,
+            MetricType metric = METRIC_L2,
+            GpuIndexCagraConfig config = GpuIndexCagraConfig());
+
+    // train builds the graph over x (the index stores x as its dataset); add calls train.  Either does nothing on a
+    // built index.
+    void train(idx_t n, const float* x) override;
+    void add(idx_t n, const float* x) override;
+    void reset() override;
+    // IndexHNSWCagra payload: xb [n][d] and the level-0 table [n][degree]; -1 entries are skipped by the search
+    void copyFrom(idx_t n, const float* xb, const idx_t* graph, int degree);
+    void copyTo(float* xb, idx_t* graph) const; // xb [ntotal][d], graph [ntotal][graph degree] (host or device)
+    std::vector<idx_t> get_knngraph() const;
+    int graphDegree() const {
+        return graphDegree_;
+    }
+    // distance evaluations of the last search, summed over all its queries
+    mutable int64_t lastSearchDistanceCount = 0;
+    // seconds spent in the last build: IVF-PQ candidates, refine, optimise
+    double lastBuildSeconds[3] = {0, 0, 0};
+
+   protected:
+    bool addImplRequiresIDs_() const override {
+        return false;
+    }
+    void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) override;
+    void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const override;
+    GpuMemoryReservation selMask_(const IDSelector& sel) const override; // throws: no filtered graph search
+
+    GpuIndexCagraConfig cagraConfig_;
+    int graphDegree_ = 0;
+    DeviceVector<float> data_;     // [ntotal][d]
+    DeviceVector<uint32_t> graph_; // [ntotal][graphDegree_]; 0xFFFFFFFF = no edge
+};
+
+// the GpuIndexCagra build pipeline (cagra_build.cu): IVF-PQ candidates, refine, optimise into graph [n][K];
+// seconds[] = the time of the three stages
+void cagraBuildGraph(
+        std::shared_ptr<GpuResources> res, int device, const float* xDev, idx_t n, int d, MetricType metric,
+        const GpuIndexCagraConfig& cfg, int K0, int K, DeviceVector<uint32_t>& graph, double seconds[3]);
 
 // fvecs_maybe_subsample (faiss/utils/utils.cpp:464-489) on a device matrix: when n > nmax, the rows
 // rand_perm(n, seed)[0:nmax] are gathered into `hold` and n becomes nmax; returns the rows to use

@@ -458,4 +458,47 @@ void runIvfPqScanInterleaved(
         const uint32_t* slotMask = nullptr, // SearchParameters::sel over the arena, or null
         const IvfSlotOutput* slots = nullptr); // the slot-keeping search, or null
 
+// ---------------------------------------------------------------- cagra_build.cu
+// G0[rows[i]] for a batch of rows: the exact fp32 distances of each row's cand [nb][nc] (IVF-PQ ids; -1 skipped), the
+// row itself dropped, the best K0 kept by (distance, id) (IP: larger first).  G0 entries past a row's valid candidates
+// are 0xFFFFFFFF; valid[i] = the number of valid entries written (<= K0).  nc <= 2048.
+void runCagraRefine(
+        const float* data, int64_t n, int d, MetricType metric, int64_t row0, int64_t nb, const idx_t* cand, int nc,
+        int K0, uint32_t* G0, int* valid, cudaStream_t stream);
+
+// the graph optimisation (DESIGN "GpuIndexCagra"): G0 [n][K0] -> G [n][K] (detour-count prune, reverse edges, merge).
+// Every G0 entry must be a row id other than its own row, and no row may hold an id twice.  K <= K0 <= 1024.
+void runCagraOptimize(GpuResources* res, int device, const uint32_t* G0, int64_t n, int K0, int K, uint32_t* G, cudaStream_t stream);
+
+// ---------------------------------------------------------------- cagra_search.cu
+// one single-CTA CAGRA search launch over nq queries (device pointers); see cagra_search.cu for the kernel layout
+struct CagraSearchArgs {
+    const float* queries;  // [nq][d]
+    int64_t nq;
+    int64_t rowOffset;    // the row of queries[0] in the whole search call (the random entry ids depend on it)
+    const float* data;    // [n][d]
+    const uint32_t* graph; // [n][graphDegree]; entries >= n (copyFrom's -1) are skipped
+    int64_t n;
+    int d;
+    int graphDegree;
+    MetricType metric;    // METRIC_L2 or METRIC_INNER_PRODUCT
+    int k;
+    int itopk;            // internal top-k (a multiple of 32, <= 512)
+    int bufSize;          // next power of two >= itopk
+    int searchWidth;
+    int candSize;         // next power of two >= max(numInit, searchWidth * graphDegree)
+    int numInit;          // num_random_samplings * searchWidth * graphDegree
+    int maxIterations;
+    int teamSize;         // 4, 8, 16 or 32 lanes per distance
+    int blockSize;
+    int hashBits;
+    int hashLimit;        // insertions allowed before the visited set is refilled from itopk
+    uint64_t seed;
+    float* outD;          // [nq][k]
+    idx_t* outI;          // [nq][k]
+    unsigned long long* distanceCount; // += distances computed
+};
+size_t cagraSearchSmemBytes(const CagraSearchArgs& a);
+void runCagraSearch(const CagraSearchArgs& a, cudaStream_t stream);
+
 } // namespace fb200

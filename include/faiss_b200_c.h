@@ -235,6 +235,71 @@ FB200_API int faiss_b200_IDSelectorCallback_new(FaissIDSelector** p_sel, int (*i
 FB200_API int faiss_SearchParameters_new(FaissSearchParameters** p_sp, FaissIDSelector* sel);
 FB200_API int faiss_SearchParametersIVF_new_with_sel(FaissSearchParametersIVF** p_sp, FaissIDSelector* sel, size_t nprobe, size_t max_codes);
 
+/* ---- GpuIndexCagra (faiss/gpu/GpuIndexCagra.h:41-380): fp32, METRIC_L2 / METRIC_INNER_PRODUCT, one GPU.
+   The configuration structs flatten GpuIndexCagraConfig with its IVFPQBuildCagraConfig / IVFPQSearchCagraConfig
+   and SearchParametersCagra; enums take the reference's values (graph_build_algo IVF_PQ = 0, NN_DESCENT = 1,
+   ITERATIVE_SEARCH = 2; codebook_gen PER_SUBSPACE = 0, PER_CLUSTER = 1; search_algo SINGLE_CTA = 0, MULTI_CTA = 1,
+   MULTI_KERNEL = 2, AUTO = 100; hash_mode HASH = 0, SMALL = 1, AUTO = 100).  Search goes through
+   faiss_Index_search_with_params with a FaissSearchParametersCagra (or faiss_Index_search: the defaults). ---- */
+typedef struct FaissGpuIndexCagraConfig {
+    int device;
+    size_t intermediate_graph_degree; /* 128 */
+    size_t graph_degree;              /* 64 */
+    int build_algo;                   /* 0 */
+    size_t nn_descent_niter;          /* 20 */
+    float refine_rate;                /* 2.0 */
+    int store_dataset;                /* 1 */
+    int guarantee_connectivity;       /* 0 */
+    /* IVFPQBuildCagraConfig */
+    uint32_t n_lists;                 /* 1024 */
+    uint32_t kmeans_n_iters;          /* 20 */
+    double kmeans_trainset_fraction;  /* 0.5 */
+    uint32_t pq_bits;                 /* 8 */
+    uint32_t pq_dim;                  /* 0 */
+    int codebook_kind;                /* 0 */
+    int force_random_rotation;        /* 0 */
+    int conservative_memory_allocation; /* 0 */
+    /* IVFPQSearchCagraConfig */
+    uint32_t n_probes;                /* 20 */
+    uint32_t max_internal_batch_size; /* 4096 */
+} FaissGpuIndexCagraConfig;
+/* the reference's defaults */
+FB200_API void faiss_GpuIndexCagraConfig_init(FaissGpuIndexCagraConfig* config);
+FB200_API int faiss_GpuIndexCagra_new(FaissGpuIndex** p_index, FaissStandardGpuResources* res, int d, FaissMetricType metric, const FaissGpuIndexCagraConfig* config);
+/* graph [ntotal][degree] as int64 (-1: no edge) */
+FB200_API int faiss_GpuIndexCagra_graph_degree(const FaissGpuIndex* index, int* degree);
+FB200_API int faiss_GpuIndexCagra_get_knngraph(const FaissGpuIndex* index, idx_t* graph);
+/* the IndexHNSWCagra payload: xb [n][d], graph [n][degree] (level 0; -1 entries are skipped by the search) */
+FB200_API int faiss_GpuIndexCagra_copyFrom(FaissGpuIndex* index, idx_t n, const float* xb, const idx_t* graph, int degree);
+FB200_API int faiss_GpuIndexCagra_copyTo(const FaissGpuIndex* index, float* xb, idx_t* graph);
+/* distance evaluations of the last search; seconds of the last build (IVF-PQ candidates, refine, optimise) */
+FB200_API int faiss_GpuIndexCagra_lastSearchDistanceCount(const FaissGpuIndex* index, int64_t* count);
+FB200_API int faiss_GpuIndexCagra_lastBuildSeconds(const FaissGpuIndex* index, double* seconds3);
+
+typedef struct FaissSearchParametersCagraConfig {
+    size_t max_queries;           /* 0 */
+    size_t itopk_size;            /* 64 */
+    size_t max_iterations;        /* 0 */
+    int algo;                     /* 100 */
+    size_t team_size;             /* 0 */
+    size_t search_width;          /* 1 */
+    size_t min_iterations;        /* 0 */
+    size_t thread_block_size;     /* 0 */
+    int hashmap_mode;             /* 100 */
+    size_t hashmap_min_bitlen;    /* 0 */
+    float hashmap_max_fill_rate;  /* 0.5 */
+    uint32_t num_random_samplings; /* 1 */
+    uint64_t seed;                /* 0x128394 */
+} FaissSearchParametersCagraConfig;
+typedef struct FaissSearchParameters_H FaissSearchParametersCagra;
+FB200_API void faiss_SearchParametersCagraConfig_init(FaissSearchParametersCagraConfig* config);
+/* sel may be NULL (GpuIndexCagra rejects a selector at search time) */
+FB200_API int faiss_SearchParametersCagra_new(FaissSearchParametersCagra** p_sp, FaissIDSelector* sel, const FaissSearchParametersCagraConfig* config);
+
+/* the graph optimisation of the GpuIndexCagra build on its own (device pointers, uint32 ids): G0 [n][K0] -> G [n][K].
+   Every G0 row must hold K0 distinct ids other than its own row; 1 <= K <= K0 <= 1024. */
+FB200_API int b200_cagra_optimize(FaissStandardGpuResources* res, int device, const uint32_t* G0, int64_t n, int K0, int K, uint32_t* G);
+
 /* c_api/Index_c.h faiss_Index_search_with_params: per-call nprobe for IVF indexes (max_codes must be 0) and an
    IDSelector for GPU indexes */
 FB200_API int faiss_Index_search_with_params(const FaissIndex* index, idx_t n, const float* x, idx_t k, const FaissSearchParameters* params, float* distances, idx_t* labels);
