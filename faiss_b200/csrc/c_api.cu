@@ -929,6 +929,8 @@ int b200_cagra_optimize(FaissStandardGpuResources* r, int device, const uint32_t
         DeviceScope scope(device);
         res->initializeForDevice(device);
         auto stream = res->getDefaultStream(device);
+        FB_THROW_IF_NOT_FMT(n >= 0 && K0 >= 1, "b200_cagra_optimize: bad shape (%ld, %d)", (long)n, K0);
+        checkCagraG0(res.get(), device, G0, n, K0, stream);
         runCagraOptimize(res.get(), device, G0, n, K0, K, G, stream);
     }
     CATCH_AND_HANDLE

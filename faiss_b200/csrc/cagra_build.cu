@@ -252,6 +252,18 @@ __global__ void cagra_merge_kernel(
         G[u * K + t] = p[t];
 }
 
+// bad[0] = 1 when some G0[u][j] >= n (a -1 read as uint32, or out of range), bad[1] = 1 when some G0[u][j] == u
+__global__ void cagra_check_g0_kernel(const uint32_t* __restrict__ G0, int64_t n, int K0, int* bad) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n * K0)
+        return;
+    const uint32_t v = G0[e];
+    if (v >= (uint64_t)n)
+        bad[0] = 1;
+    else if (v == (uint64_t)(e / K0))
+        bad[1] = 1;
+}
+
 double secondsSince(std::chrono::steady_clock::time_point t0) {
     return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
@@ -271,6 +283,20 @@ void runCagraRefine(
     cagra_refine_kernel<<<(unsigned)nb, 256, smem, stream>>>(
             data, n, d, metric == METRIC_INNER_PRODUCT, row0, cand, nc, ncPow2, K0, G0, valid);
     CUDA_CHECK_LAST();
+}
+
+void checkCagraG0(GpuResources* res, int device, const uint32_t* G0, int64_t n, int K0, cudaStream_t stream) {
+    if (n == 0 || K0 <= 0)
+        return;
+    auto bad = res->device_alloc(device, 2 * sizeof(int), AllocType::Other);
+    CUDA_VERIFY(cudaMemsetAsync(bad.data, 0, 2 * sizeof(int), stream));
+    cagra_check_g0_kernel<<<(unsigned)ceil_div(n * K0, 256), 256, 0, stream>>>(G0, n, K0, bad.as<int>());
+    CUDA_CHECK_LAST();
+    int h[2] = {0, 0};
+    CUDA_VERIFY(cudaMemcpyAsync(h, bad.data, sizeof(h), cudaMemcpyDeviceToHost, stream));
+    CUDA_VERIFY(cudaStreamSynchronize(stream));
+    FB_THROW_IF_NOT_MSG(!h[0], "CAGRA optimize: a G0 entry is >= n (no edge, or out of range)");
+    FB_THROW_IF_NOT_MSG(!h[1], "CAGRA optimize: a G0 row holds its own id");
 }
 
 void runCagraOptimize(GpuResources* res, int device, const uint32_t* G0, int64_t n, int K0, int K, uint32_t* G, cudaStream_t stream) {

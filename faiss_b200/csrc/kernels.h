@@ -469,6 +469,9 @@ void runCagraRefine(
 // the graph optimisation (DESIGN "GpuIndexCagra"): G0 [n][K0] -> G [n][K] (detour-count prune, reverse edges, merge).
 // Every G0 entry must be a row id other than its own row, and no row may hold an id twice.  K <= K0 <= 1024.
 void runCagraOptimize(GpuResources* res, int device, const uint32_t* G0, int64_t n, int K0, int K, uint32_t* G, cudaStream_t stream);
+// throws when a G0 entry is >= n (a -1 read as uint32) or equals its own row: the checks of b200_cagra_optimize,
+// whose caller's G0 comes from outside the build (synchronises the stream; writes nothing of the caller's)
+void checkCagraG0(GpuResources* res, int device, const uint32_t* G0, int64_t n, int K0, cudaStream_t stream);
 
 // ---------------------------------------------------------------- cagra_search.cu
 // one single-CTA CAGRA search launch over nq queries (device pointers); see cagra_search.cu for the kernel layout

@@ -297,7 +297,8 @@ FB200_API void faiss_SearchParametersCagraConfig_init(FaissSearchParametersCagra
 FB200_API int faiss_SearchParametersCagra_new(FaissSearchParametersCagra** p_sp, FaissIDSelector* sel, const FaissSearchParametersCagraConfig* config);
 
 /* the graph optimisation of the GpuIndexCagra build on its own (device pointers, uint32 ids): G0 [n][K0] -> G [n][K].
-   Every G0 row must hold K0 distinct ids other than its own row; 1 <= K <= K0 <= 1024. */
+   Every G0 row must hold K0 distinct ids other than its own row; 1 <= K <= K0 <= 1024.  An entry >= n (such as a -1)
+   or equal to its own row is an error, reported before G is written. */
 FB200_API int b200_cagra_optimize(FaissStandardGpuResources* res, int device, const uint32_t* G0, int64_t n, int K0, int K, uint32_t* G);
 
 /* c_api/Index_c.h faiss_Index_search_with_params: per-call nprobe for IVF indexes (max_codes must be 0) and an
