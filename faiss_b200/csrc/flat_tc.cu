@@ -190,6 +190,7 @@ __global__ void tc_prepare_queries_kernel(
         int d,
         int dpad,
         const float* __restrict__ qScale,
+        float yScale,
         float c1,
         float c2,
         float yMaxNorm,
@@ -213,11 +214,16 @@ __global__ void tc_prepare_queries_kernel(
         acc += __shfl_xor_sync(kFullMask, acc, o);
     if (lane_id() == 0) {
         float qn = sqrtf(acc) * 1.0001f;
-        // |approx score - score implied by the exact kernel's fp32 distance| <= c1*|q||y| + c2*(|q|+|y|)^2
-        // (see DESIGN.md, error model): c1 = fp16 input rounding + fp32 accumulation of q.y, c2 = fp32
-        // rounding of the bias (norms), of the final FMA and of the exact kernel's own sum (d terms)
+        // |approx score - score implied by the exact kernel's fp32 distance| <= eps (DESIGN.md 3.1, error model):
+        //   c1*|q||y|          fp16 input rounding + fp32 accumulation of q.y
+        //   c2*(|q|+|y|)^2     fp32 rounding of the bias (norms), of the final FMA and of the exact kernel's own sum
+        //   1.01*(uq*|y| + uy*|q| + uq*uy)   elements in fp16's subnormal range, off by up to 2^-25 / s absolute
+        //                      rather than 2^-11 relative.  s is the whole batch's scale (yScale the database's), so
+        //                      next to a much larger query this bounds the extra error norm: u = sqrt(dpad) 2^-25 / s
+        const float u0 = sqrtf((float)dpad) * ldexpf(1.f, -25);
+        const float uq = u0 / scale, uy = u0 / yScale;
         const float qy = qn + yMaxNorm;
-        eps[row] = c1 * qn * yMaxNorm + c2 * qy * qy;
+        eps[row] = c1 * qn * yMaxNorm + c2 * qy * qy + 1.01f * (uq * yMaxNorm + uy * qn + uq * uy);
         thr[row] = -CUDART_INF_F;
     }
 }
@@ -1354,7 +1360,8 @@ void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
         tc_query_scale_kernel<<<1, 1, 0, stream>>>(sc + 0, scale_, sc + 1, sc + 2);
         CUDA_CHECK_LAST();
         tc_prepare_queries_kernel<<<(unsigned)ceil_div(nq, 8), 256, 0, stream>>>(
-                b.Q, nq, d_, dpad_, sc + 1, c1, c2, maxNorm_, b.q16.as<__half>(), b.eps.as<float>(), b.thr.as<float>());
+                b.Q, nq, d_, dpad_, sc + 1, scale_, c1, c2, maxNorm_, b.q16.as<__half>(), b.eps.as<float>(),
+                b.thr.as<float>());
         CUDA_CHECK_LAST();
     }
     if (!c.s.streaming) {
