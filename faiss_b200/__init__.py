@@ -1467,3 +1467,71 @@ def flat_tc_scores_debug(res, Q16, Y16, device=0):
         )
     )
     return S
+
+
+_c_i32 = ctypes.POINTER(ctypes.c_int32)
+
+
+def _as_i32(x):
+    if _is_torch(x):
+        import torch
+
+        assert x.dtype == torch.int32
+        return x.contiguous()
+    return np.ascontiguousarray(x, dtype=np.int32)
+
+
+class GpuIcmEncoder:
+    """faiss::gpu::GpuIcmEncoder (faiss/gpu/GpuIcmEncoder.h): LocalSearchQuantizer's ICM encoding
+    (lsq::IcmEncoder::encode, faiss/impl/LocalSearchQuantizer.cpp:539-795) on one or more devices.
+
+    ``res`` is one StandardGpuResources per entry of ``devices``.  The perturbation draws are the caller's, an int32
+    array [ils_iters, n, nperts, 2] of (m, k) in the order of LocalSearchQuantizer::perturb_codes; given the CPU's
+    draws, the codes equal the CPU encoder's where fp32 is exact.  Limits: 1 <= K <= 1024, nperts <= M."""
+
+    def __init__(self, M, K, d, res, devices=(0,)):
+        if isinstance(res, StandardGpuResources):
+            res = [res]
+        devices = [int(v) for v in devices]
+        assert len(res) == len(devices), "one StandardGpuResources per device"
+        self.M, self.K, self.d = int(M), int(K), int(d)
+        self._res = list(res)  # the handle keeps its own references; this keeps the Python objects alive too
+        hs = (ctypes.c_void_p * len(res))(*[r._h.value for r in res])
+        devs = (ctypes.c_int * len(devices))(*devices)
+        self._h = ctypes.c_void_p()
+        check(lib.faiss_GpuIcmEncoder_new(ctypes.byref(self._h), self.M, self.K, self.d, len(devices), hs, devs))
+
+    def __del__(self):
+        if getattr(self, "_h", None) and lib is not None:
+            lib.faiss_GpuIcmEncoder_free(self._h)
+            self._h = None
+
+    def setBinaryTerm(self, codebooks):
+        """codebooks [M, K, d] (or [M * K, d]), numpy or torch"""
+        cb = _as_f32(codebooks)
+        size = cb.numel() if _is_torch(cb) else cb.size
+        assert size == self.M * self.K * self.d, "codebooks must hold M * K * d floats"
+        check(lib.faiss_GpuIcmEncoder_set_binary_term(self._h, _ptr(cb, _c_f)))
+
+    def encode(self, codes, x, perturbations, icm_iters=4, page_bytes=None):
+        """codes [n, M] int32 (start codes), x [n, d], perturbations [ils_iters, n, nperts, 2] int32 -> the best codes
+        [n, M] int32, with the residency of ``codes``.  page_bytes: the page budget (default 256 MiB)."""
+        x = _as_f32(x)
+        codes = _as_i32(codes)
+        pert = _as_i32(perturbations)
+        n = int(x.shape[0])
+        assert tuple(codes.shape) == (n, self.M) and tuple(x.shape) == (n, self.d)
+        assert len(pert.shape) == 4 and int(pert.shape[1]) == n and int(pert.shape[3]) == 2, "perturbations [ils, n, nperts, 2]"
+        ils, nperts = int(pert.shape[0]), int(pert.shape[2])
+        out = codes.clone() if _is_torch(codes) else codes.copy()
+        if _is_torch(out) and out.is_cuda:
+            import torch
+
+            torch.cuda.current_stream(out.device).synchronize()  # the clone is read on the resources' stream
+        args = (self._h, _ptr(out, _c_i32), _ptr(x, _c_f), ctypes.c_int64(n), ctypes.c_size_t(ils), ctypes.c_size_t(nperts),
+                ctypes.c_size_t(int(icm_iters)), _ptr(pert, _c_i32))
+        if page_bytes is None:
+            check(lib.faiss_GpuIcmEncoder_encode(*args))
+        else:
+            check(lib.b200_icm_encode_paged(*args, ctypes.c_size_t(int(page_bytes))))
+        return out

@@ -52,6 +52,8 @@ lib.faiss_GpuIndexIVF_get_list_size.restype = ctypes.c_size_t
 lib.faiss_GpuIndexIVF_get_list_size.argtypes = [ctypes.c_void_p, ctypes.c_size_t]
 lib.faiss_IDSelector_free.argtypes = [ctypes.c_void_p]
 lib.faiss_IDSelector_free.restype = None
+lib.faiss_GpuIcmEncoder_free.argtypes = [ctypes.c_void_p]
+lib.faiss_GpuIcmEncoder_free.restype = None
 lib.faiss_IDSelector_is_member.argtypes = [ctypes.c_void_p, ctypes.c_int64]
 
 

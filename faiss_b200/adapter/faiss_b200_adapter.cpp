@@ -303,6 +303,64 @@ void B200IndexIVFPQ::copyTo(faiss::IndexIVFPQ* index) const { // faiss/gpu/GpuIn
 }
 
 // ---------------------------------------------------------------- cloner
+// ------------------------------------------------------------------------------------------
+// B200IcmEncoder
+// ------------------------------------------------------------------------------------------
+B200IcmEncoder::B200IcmEncoder(
+        const faiss::LocalSearchQuantizer* lsq_in,
+        const std::vector<B200Resources*>& res,
+        const std::vector<int>& devices)
+        : faiss::lsq::IcmEncoder(lsq_in) {
+    FAISS_THROW_IF_NOT_MSG(res.size() == devices.size() && !res.empty(), "one B200Resources per device");
+    std::vector<FaissStandardGpuResources*> hs;
+    for (auto* r : res)
+        hs.push_back(r->handle());
+    ck(faiss_GpuIcmEncoder_new(&h_, (int)lsq->M, (int)lsq->K, (int)lsq->d, (int)devices.size(), hs.data(), devices.data()));
+}
+
+B200IcmEncoder::~B200IcmEncoder() {
+    if (h_)
+        faiss_GpuIcmEncoder_free(h_);
+}
+
+void B200IcmEncoder::set_binary_term() {
+    ck(faiss_GpuIcmEncoder_set_binary_term(h_, lsq->codebooks.data()));
+}
+
+void B200IcmEncoder::encode(int32_t* codes, const float* x, std::mt19937& gen, size_t n, size_t ils_iters) const {
+    const size_t M = lsq->M, K = lsq->K, nperts = lsq->nperts;
+    FAISS_THROW_IF_NOT(nperts <= M); // as icm_encode_impl, before any draw
+    // LocalSearchQuantizer::perturb_codes (faiss/impl/LocalSearchQuantizer.cpp:673-688), once per ILS iteration
+    std::uniform_int_distribution<size_t> m_distrib(0, M - 1);
+    std::uniform_int_distribution<int32_t> k_distrib(0, K - 1);
+    std::vector<int32_t> perts(ils_iters * n * nperts * 2);
+    int32_t* p = perts.data();
+    for (size_t it = 0; it < ils_iters; it++) {
+        for (size_t i = 0; i < n; i++) {
+            for (size_t j = 0; j < nperts; j++) {
+                p[0] = (int32_t)m_distrib(gen);
+                p[1] = k_distrib(gen);
+                p += 2;
+            }
+        }
+    }
+    ck(faiss_GpuIcmEncoder_encode(h_, codes, x, (::idx_t)n, ils_iters, nperts, lsq->icm_iters, perts.data()));
+}
+
+B200IcmEncoderFactory::B200IcmEncoderFactory(int ngpus) {
+    for (int i = 0; i < ngpus; i++) {
+        res.push_back(std::make_unique<B200Resources>());
+        devices.push_back(i);
+    }
+}
+
+faiss::lsq::IcmEncoder* B200IcmEncoderFactory::get(const faiss::LocalSearchQuantizer* lsq) {
+    std::vector<B200Resources*> rs;
+    for (auto& r : res)
+        rs.push_back(r.get());
+    return new B200IcmEncoder(lsq, rs, devices);
+}
+
 faiss::Index* index_cpu_to_b200(B200Resources* res, int device, const faiss::Index* index, const B200ClonerOptions* options) {
     if (auto* f = dynamic_cast<const faiss::IndexFlat*>(index))
         return new B200IndexFlat(res, f, device, options && options->useFloat16);

@@ -17,11 +17,15 @@
 #include <faiss/IndexIVF.h>
 #include <faiss/IndexIVFFlat.h>
 #include <faiss/IndexIVFPQ.h>
+#include <faiss/impl/LocalSearchQuantizer.h>
 
 #include <memory>
+#include <random>
+#include <vector>
 
 struct FaissStandardGpuResources_H;
 struct FaissIndex_H;
+struct FaissGpuIcmEncoder_H;
 
 namespace faiss_b200_adapter {
 
@@ -142,6 +146,31 @@ class B200IndexIVFPQ : public B200IndexIVF { // faiss/gpu/GpuIndexIVFPQ.h:56-181
     void copyFrom(const faiss::IndexIVFPQ* index);
     void copyTo(faiss::IndexIVFPQ* index) const;
     size_t M, nbits;
+};
+
+// faiss::gpu::GpuIcmEncoder (faiss/gpu/GpuIcmEncoder.h): LocalSearchQuantizer's ICM encoding on the devices.  encode()
+// draws the perturbations from `gen` exactly as LocalSearchQuantizer::perturb_codes does and hands them to the device,
+// so `gen` ends in the state the CPU encoder leaves it in and the codes follow the CPU's random trajectory.
+class B200IcmEncoder : public faiss::lsq::IcmEncoder {
+   public:
+    B200IcmEncoder(const faiss::LocalSearchQuantizer* lsq, const std::vector<B200Resources*>& res, const std::vector<int>& devices);
+    ~B200IcmEncoder() override;
+    B200IcmEncoder(const B200IcmEncoder&) = delete;
+    B200IcmEncoder& operator=(const B200IcmEncoder&) = delete;
+    void set_binary_term() override;
+    void encode(int32_t* codes, const float* x, std::mt19937& gen, size_t n, size_t ils_iters) const override;
+
+   private:
+    FaissGpuIcmEncoder_H* h_ = nullptr;
+};
+
+// faiss::gpu::GpuIcmEncoderFactory: one B200Resources per device 0 .. ngpus - 1.  LocalSearchQuantizer deletes its
+// icm_encoder_factory, so give it one made with new:  lsq.icm_encoder_factory = new B200IcmEncoderFactory(1);
+struct B200IcmEncoderFactory : public faiss::lsq::IcmEncoderFactory {
+    explicit B200IcmEncoderFactory(int ngpus = 1);
+    faiss::lsq::IcmEncoder* get(const faiss::LocalSearchQuantizer* lsq) override;
+    std::vector<std::unique_ptr<B200Resources>> res;
+    std::vector<int> devices;
 };
 
 // faiss::gpu::index_cpu_to_gpu / index_gpu_to_cpu (faiss/gpu/GpuCloner.cpp:124-255) for the three index types on the path

@@ -6,6 +6,7 @@
 #include "comm.h"
 #include "distance.h"
 #include "faiss_b200_c.h"
+#include "icm_encode.h"
 #include "index.h"
 
 using namespace fb200;
@@ -1412,6 +1413,55 @@ int faiss_b200_bfKnn_tiling(
     try {
         const GpuDistanceParams a = DP(params);
         bfKnn_tiling(RES(r), a, vectorsMemoryLimit, queriesMemoryLimit);
+    }
+    CATCH_AND_HANDLE
+}
+struct FaissGpuIcmEncoder_H {
+    std::unique_ptr<GpuIcmEncoder> enc;
+};
+static GpuIcmEncoder* ICM(FaissGpuIcmEncoder* p) {
+    if (!p || !p->enc)
+        FB_THROW_MSG("null encoder handle");
+    return p->enc.get();
+}
+int faiss_GpuIcmEncoder_new(FaissGpuIcmEncoder** p, int M, int K, int d, int ndevices, FaissStandardGpuResources** r, const int* devices) {
+    try {
+        FB_THROW_IF_NOT_MSG(p != nullptr && r != nullptr && devices != nullptr, "null argument");
+        FB_THROW_IF_NOT_MSG(ndevices >= 1, "at least one device is needed");
+        std::vector<std::shared_ptr<GpuResources>> res;
+        std::vector<int> devs;
+        for (int i = 0; i < ndevices; i++) {
+            res.push_back(RES(r[i]));
+            devs.push_back(devices[i]);
+        }
+        auto h = std::make_unique<FaissGpuIcmEncoder_H>();
+        h->enc = std::make_unique<GpuIcmEncoder>(M, K, d, std::move(res), std::move(devs));
+        *p = h.release();
+    }
+    CATCH_AND_HANDLE
+}
+void faiss_GpuIcmEncoder_free(FaissGpuIcmEncoder* p) {
+    delete p;
+}
+int faiss_GpuIcmEncoder_set_binary_term(FaissGpuIcmEncoder* p, const float* codebooks) {
+    try {
+        ICM(p)->setBinaryTerm(codebooks);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_GpuIcmEncoder_encode(
+        FaissGpuIcmEncoder* p, int32_t* codes, const float* x, idx_t n, size_t ils_iters, size_t nperts, size_t icm_iters,
+        const int32_t* perturbations) {
+    try {
+        ICM(p)->encode(codes, x, n, ils_iters, nperts, icm_iters, perturbations);
+    }
+    CATCH_AND_HANDLE
+}
+int b200_icm_encode_paged(
+        FaissGpuIcmEncoder* p, int32_t* codes, const float* x, idx_t n, size_t ils_iters, size_t nperts, size_t icm_iters,
+        const int32_t* perturbations, size_t page_bytes) {
+    try {
+        ICM(p)->encode(codes, x, n, ils_iters, nperts, icm_iters, perturbations, page_bytes);
     }
     CATCH_AND_HANDLE
 }

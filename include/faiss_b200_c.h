@@ -349,6 +349,22 @@ FB200_API int faiss_DistributedIndexShards_sync(FaissIndexShards* index); /* col
 FB200_API int faiss_DistributedIndexShards_info(const FaissIndexShards* index, int* rank, int* nranks, idx_t* id_offset);
 FB200_API int b200_shards_search(FaissStandardGpuResources* res, FaissGpuIndex* local_shard, int successive_ids, idx_t n, const float* x, idx_t k, float* distances, idx_t* labels);
 
+/* ---- GpuIcmEncoder (faiss/gpu/GpuIcmEncoder.h; faiss/impl/LocalSearchQuantizer.cpp:539-795) ----
+   LocalSearchQuantizer's ICM encoding (lsq::IcmEncoder::encode) on one or more devices, rows split into contiguous
+   ranges.  The perturbation draws are the caller's: perturbations is [ils_iters][n][nperts] pairs (m, k) as int32,
+   drawn in the order of LocalSearchQuantizer::perturb_codes, so a caller that draws them from its std::mt19937 follows
+   the CPU encoder's random trajectory.  codes [n][M] int32 (in: start codes, out: best codes), x [n][d] and
+   perturbations may each be host or device memory.  Limits: 1 <= K <= 1024, nperts <= M. */
+typedef struct FaissGpuIcmEncoder_H FaissGpuIcmEncoder;
+/* res[i] serves devices[i]; each device needs a resources object of its own */
+FB200_API int faiss_GpuIcmEncoder_new(FaissGpuIcmEncoder** p_enc, int M, int K, int d, int ndevices, FaissStandardGpuResources** res, const int* devices);
+FB200_API void faiss_GpuIcmEncoder_free(FaissGpuIcmEncoder* enc);
+/* codebooks [M][K][d] (host or device): lsq::IcmEncoder::set_binary_term */
+FB200_API int faiss_GpuIcmEncoder_set_binary_term(FaissGpuIcmEncoder* enc, const float* codebooks);
+FB200_API int faiss_GpuIcmEncoder_encode(FaissGpuIcmEncoder* enc, int32_t* codes, const float* x, idx_t n, size_t ils_iters, size_t nperts, size_t icm_iters, const int32_t* perturbations);
+/* faiss_GpuIcmEncoder_encode with a page budget of page_bytes instead of 256 MiB */
+FB200_API int b200_icm_encode_paged(FaissGpuIcmEncoder* enc, int32_t* codes, const float* x, idx_t n, size_t ils_iters, size_t nperts, size_t icm_iters, const int32_t* perturbations, size_t page_bytes);
+
 /* ---- Clustering (c_api/Clustering_c.h faiss_kmeans_clustering; faiss/Clustering.cpp:60-380) ----
    Lloyd k-means with the training set resident on the device; x host or device. */
 FB200_API int faiss_b200_kmeans(FaissStandardGpuResources* res, int device, size_t d, size_t n, size_t k, const float* x, int niter, int seed, int max_points_per_centroid, float* centroids_out /* host [k*d] */, float* obj_out /* host [niter] or NULL */);
