@@ -92,7 +92,7 @@ def _empty_like_residency(x, shape, dtype):
     if _is_torch(x) and x.is_cuda:
         import torch
 
-        tdt = {np.float32: torch.float32, np.int64: torch.int64, np.uint8: torch.uint8}[dtype]
+        tdt = {np.float32: torch.float32, np.int64: torch.int64, np.uint8: torch.uint8, np.int32: torch.int32}[dtype]
         return torch.empty(shape, dtype=tdt, device=x.device)
     return np.empty(shape, dtype=dtype)
 
@@ -1535,3 +1535,105 @@ class GpuIcmEncoder:
         else:
             check(lib.b200_icm_encode_paged(*args, ctypes.c_size_t(int(page_bytes))))
         return out
+
+
+# AdditiveQuantizer::Search_type_t (faiss/impl/AdditiveQuantizer.h:71-86)
+ST_decompress, ST_LUT_nonorm, ST_norm_from_LUT, ST_norm_float, ST_norm_qint8, ST_norm_qint4 = range(6)
+ST_norm_cqint8, ST_norm_cqint4, ST_norm_lsq2x4, ST_norm_rq2x4 = range(6, 10)
+
+
+class GpuRqEncoder:
+    """ResidualQuantizer's beam-search encoding (faiss/impl/ResidualQuantizer.cpp:432-520) on one device.
+
+    ``nbits`` is one entry per codebook (1 <= nbits[m] <= 12); every beam is in [1, 256].  Inputs may be numpy arrays or
+    torch tensors, host or device; outputs have the residency of the first array argument.  On integer-valued data and
+    codebooks the results equal the CPU's bit for bit.  ``page_bytes`` overrides the 256 MiB page budget."""
+
+    def __init__(self, d, nbits, res, device=0):
+        self.d, self.nbits = int(d), [int(b) for b in nbits]
+        self.M = len(self.nbits)
+        self._res = res
+        nb = (ctypes.c_int * self.M)(*self.nbits)
+        self._h = ctypes.c_void_p()
+        check(lib.faiss_b200_RqEncoder_new(ctypes.byref(self._h), res._h, int(device), self.d, self.M, nb))
+
+    def __del__(self):
+        if getattr(self, "_h", None) and lib is not None:
+            lib.faiss_b200_RqEncoder_free(self._h)
+            self._h = None
+
+    def setCodebooks(self, codebooks):
+        """codebooks [total_K, d], numpy or torch, host or device"""
+        cb = _as_f32(codebooks)
+        size = cb.numel() if _is_torch(cb) else cb.size
+        assert size == sum(1 << b for b in self.nbits) * self.d, "codebooks must hold total_K * d floats"
+        check(lib.faiss_b200_RqEncoder_set_codebooks(self._h, _ptr(cb, _c_f)))
+
+    def finalBeam(self, beam_in, out_beam):
+        b = ctypes.c_int()
+        check(lib.faiss_b200_RqEncoder_final_beam(self._h, int(beam_in), int(out_beam), ctypes.byref(b)))
+        return b.value
+
+    def refineBeam(self, residuals, out_beam, page_bytes=None):
+        """ResidualQuantizer::refine_beam: residuals [n, beam_in, d] -> (codes [n, B, M] int32, residuals [n, B, d],
+        distances [n, B])"""
+        r = _as_f32(residuals)
+        n, beam_in = int(r.shape[0]), int(r.shape[1])
+        assert len(r.shape) == 3 and int(r.shape[2]) == self.d, "residuals [n, beam_in, d]"
+        B = self.finalBeam(beam_in, out_beam)
+        codes = _empty_like_residency(r, (n, B, self.M), np.int32)
+        ro = _empty_like_residency(r, (n, B, self.d), np.float32)
+        dis = _empty_like_residency(r, (n, B), np.float32)
+        args = (self._h, ctypes.c_int64(n), int(beam_in), _ptr(r, _c_f), int(out_beam), _ptr(codes, _c_i32), _ptr(ro, _c_f),
+                _ptr(dis, _c_f))
+        if page_bytes is None:
+            check(lib.faiss_b200_RqEncoder_refine_beam(*args))
+        else:
+            check(lib.b200_rq_refine_beam_paged(*args, ctypes.c_size_t(int(page_bytes))))
+        return codes, ro, dis
+
+    def refineBeamLUT(self, x, out_beam, page_bytes=None):
+        """ResidualQuantizer::refine_beam_LUT from x [n, d] (the device makes ‖x‖² and x·Cᵀ) -> (codes [n, B, M] int32,
+        distances [n, B])"""
+        x = _as_f32(x)
+        n = int(x.shape[0])
+        assert tuple(x.shape) == (n, self.d)
+        B = self.finalBeam(1, out_beam)
+        codes = _empty_like_residency(x, (n, B, self.M), np.int32)
+        dis = _empty_like_residency(x, (n, B), np.float32)
+        args = (self._h, ctypes.c_int64(n), _ptr(x, _c_f), int(out_beam), _ptr(codes, _c_i32), _ptr(dis, _c_f))
+        if page_bytes is None:
+            check(lib.faiss_b200_RqEncoder_refine_beam_lut(*args))
+        else:
+            check(lib.b200_rq_refine_beam_lut_paged(*args, ctypes.c_size_t(int(page_bytes))))
+        return codes, dis
+
+    def codeSize(self, search_type=ST_decompress):
+        norm_bits = {ST_norm_float: 32, ST_norm_qint8: 8, ST_norm_qint4: 4, ST_norm_cqint8: 8, ST_norm_cqint4: 4,
+                     ST_norm_lsq2x4: 8, ST_norm_rq2x4: 8}.get(search_type, 0)
+        return (sum(self.nbits) + norm_bits + 7) // 8
+
+    def computeCodes(self, x, use_beam_LUT=0, max_beam_size=5, search_type=ST_decompress, norm_min=0.0, norm_max=0.0,
+                     centroids=None, page_bytes=None):
+        """ResidualQuantizer::compute_codes_add_centroids -> packed codes [n, code_size] uint8"""
+        x = _as_f32(x)
+        n = int(x.shape[0])
+        assert tuple(x.shape) == (n, self.d)
+        cen = None if centroids is None else _as_f32(centroids)
+        out = _empty_like_residency(x, (n, self.codeSize(search_type)), np.uint8)
+        args = (self._h, _ptr(x, _c_f), ctypes.c_int64(n), int(bool(use_beam_LUT)), int(max_beam_size), int(search_type),
+                ctypes.c_float(norm_min), ctypes.c_float(norm_max), _ptr(cen, _c_f), _ptr(out, _c_u8))
+        if page_bytes is None:
+            check(lib.faiss_b200_RqEncoder_compute_codes(*args))
+        else:
+            check(lib.b200_rq_compute_codes_paged(*args, ctypes.c_size_t(int(page_bytes))))
+        return out
+
+    def encodeUnpacked(self, x, use_beam_LUT=0, max_beam_size=5):
+        """the compute_codes search, unpacked -> codes [n, M] int32 (entry 0 of the beam)"""
+        x = _as_f32(x)
+        n = int(x.shape[0])
+        codes = _empty_like_residency(x, (n, self.M), np.int32)
+        check(lib.faiss_b200_RqEncoder_encode_unpacked(self._h, _ptr(x, _c_f), ctypes.c_int64(n), int(bool(use_beam_LUT)),
+                                                       int(max_beam_size), _ptr(codes, _c_i32)))
+        return codes

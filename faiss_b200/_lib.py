@@ -54,6 +54,8 @@ lib.faiss_IDSelector_free.argtypes = [ctypes.c_void_p]
 lib.faiss_IDSelector_free.restype = None
 lib.faiss_GpuIcmEncoder_free.argtypes = [ctypes.c_void_p]
 lib.faiss_GpuIcmEncoder_free.restype = None
+lib.faiss_b200_RqEncoder_free.argtypes = [ctypes.c_void_p]
+lib.faiss_b200_RqEncoder_free.restype = None
 lib.faiss_IDSelector_is_member.argtypes = [ctypes.c_void_p, ctypes.c_int64]
 
 

@@ -361,6 +361,49 @@ faiss::lsq::IcmEncoder* B200IcmEncoderFactory::get(const faiss::LocalSearchQuant
     return new B200IcmEncoder(lsq, rs, devices);
 }
 
+// ------------------------------------------------------------------------------------------
+// B200ResidualQuantizer
+// ------------------------------------------------------------------------------------------
+B200ResidualQuantizer::B200ResidualQuantizer(
+        B200Resources* res,
+        size_t d,
+        const std::vector<size_t>& nbits,
+        Search_type_t search_type,
+        int device)
+        : faiss::ResidualQuantizer(d, nbits, search_type), res_(res), device_(device) {
+    FAISS_THROW_IF_NOT_MSG(res != nullptr, "null B200Resources");
+}
+
+B200ResidualQuantizer::B200ResidualQuantizer(B200Resources* res, size_t d, size_t M, size_t nbits, Search_type_t search_type, int device)
+        : B200ResidualQuantizer(res, d, std::vector<size_t>(M, nbits), search_type, device) {}
+
+void B200ResidualQuantizer::compute_codes_add_centroids(const float* x, uint8_t* codes_out, size_t n, const float* centroids) const {
+    FAISS_THROW_IF_NOT_MSG(is_trained, "RQ is not trained yet.");
+    FAISS_THROW_IF_NOT_MSG(
+            approx_topk_mode == ::EXACT_TOPK,
+            "B200ResidualQuantizer: the device beam search takes approx_topk_mode = EXACT_TOPK only");
+    FAISS_THROW_IF_NOT_MSG(use_beam_LUT == 0 || use_beam_LUT == 1, "use_beam_LUT must be 0 or 1");
+    std::vector<int> nb(nbits.begin(), nbits.end());
+    FaissGpuRqEncoder* h = nullptr;
+    ck(faiss_b200_RqEncoder_new(&h, res_->handle(), device_, (int)d, (int)M, nb.data()));
+    std::unique_ptr<FaissGpuRqEncoder, void (*)(FaissGpuRqEncoder*)> guard(h, faiss_b200_RqEncoder_free);
+    ck(faiss_b200_RqEncoder_set_codebooks(h, codebooks.data()));
+    if (search_type <= ST_norm_qint4) { // packed on the device
+        ck(faiss_b200_RqEncoder_compute_codes(
+                h, x, (::idx_t)n, use_beam_LUT, max_beam_size, (int)search_type, norm_min, norm_max, centroids, codes_out));
+        return;
+    }
+    // ST_norm_cqint*, ST_norm_*2x4: the CPU packs these from the decoded codes too (norms = nullptr)
+    std::vector<int32_t> codes(n * M);
+    ck(faiss_b200_RqEncoder_encode_unpacked(h, x, (::idx_t)n, use_beam_LUT, max_beam_size, codes.data()));
+    pack_codes(n, codes.data(), codes_out, M, nullptr, centroids);
+}
+
+faiss::Index* B200ProgressiveDimIndexFactory::operator()(int dim) {
+    ncall++;
+    return new B200IndexFlat(&res, dim, faiss::METRIC_L2, device);
+}
+
 faiss::Index* index_cpu_to_b200(B200Resources* res, int device, const faiss::Index* index, const B200ClonerOptions* options) {
     if (auto* f = dynamic_cast<const faiss::IndexFlat*>(index))
         return new B200IndexFlat(res, f, device, options && options->useFloat16);

@@ -18,6 +18,7 @@
 #include <faiss/IndexIVFFlat.h>
 #include <faiss/IndexIVFPQ.h>
 #include <faiss/impl/LocalSearchQuantizer.h>
+#include <faiss/impl/ResidualQuantizer.h>
 
 #include <memory>
 #include <random>
@@ -171,6 +172,39 @@ struct B200IcmEncoderFactory : public faiss::lsq::IcmEncoderFactory {
     faiss::lsq::IcmEncoder* get(const faiss::LocalSearchQuantizer* lsq) override;
     std::vector<std::unique_ptr<B200Resources>> res;
     std::vector<int> devices;
+};
+
+// faiss::ResidualQuantizer whose compute_codes (and so retrain_AQ_codebook under Train_refine_codebook) runs the beam
+// search on the device, in the mode use_beam_LUT selects, with the codebooks of the moment uploaded on each call.  The
+// search is the one compute_codes runs without an assign_index_factory; approx_topk_mode must be EXACT_TOPK.  The
+// device packs ST_decompress .. ST_norm_qint4; for the other search types it returns the codes and the inherited
+// pack_codes packs them on the host.  train() is the CPU's; give it a B200ProgressiveDimIndexFactory to put its
+// k-means and beam assignment on the device.
+class B200ResidualQuantizer : public faiss::ResidualQuantizer {
+   public:
+    B200ResidualQuantizer(
+            B200Resources* res,
+            size_t d,
+            const std::vector<size_t>& nbits,
+            Search_type_t search_type = ST_decompress,
+            int device = 0);
+    B200ResidualQuantizer(B200Resources* res, size_t d, size_t M, size_t nbits, Search_type_t search_type = ST_decompress, int device = 0);
+    void compute_codes_add_centroids(const float* x, uint8_t* codes, size_t n, const float* centroids = nullptr) const override;
+
+   private:
+    B200Resources* res_;
+    int device_;
+};
+
+// faiss::gpu::GpuProgressiveDimIndexFactory (faiss/gpu/GpuCloner.h:85-100) on one device: every index it makes is a
+// B200IndexFlat (L2), so ProgressiveDimClustering's k-means and ResidualQuantizer's beam assignment run on the Flat
+// kernels.  ncall counts the indexes made.
+struct B200ProgressiveDimIndexFactory : public faiss::ProgressiveDimIndexFactory {
+    explicit B200ProgressiveDimIndexFactory(int device = 0) : device(device) {}
+    faiss::Index* operator()(int dim) override;
+    B200Resources res;
+    int device;
+    int ncall = 0;
 };
 
 // faiss::gpu::index_cpu_to_gpu / index_gpu_to_cpu (faiss/gpu/GpuCloner.cpp:124-255) for the three index types on the path

@@ -19,9 +19,9 @@ FLAGS = [
     "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "--expt-relaxed-constexpr", "-I" + os.path.join(HERE, "..", "include"), "-I" + SRC,
 ]
-# per-file additions: the CAGRA search kernel and the ICM encode kernel report their registers, shared memory and
-# spills at every build
-FILE_FLAGS = {"cagra_search.cu": ["-Xptxas", "-v"], "icm_encode.cu": ["-Xptxas", "-v"]}
+# per-file additions: the CAGRA search kernel, the ICM encode kernel and the RQ beam-search kernels report their
+# registers, shared memory and spills at every build
+FILE_FLAGS = {"cagra_search.cu": ["-Xptxas", "-v"], "icm_encode.cu": ["-Xptxas", "-v"], "rq_encode.cu": ["-Xptxas", "-v"]}
 
 
 def _sources():

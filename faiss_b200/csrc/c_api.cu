@@ -8,6 +8,7 @@
 #include "faiss_b200_c.h"
 #include "icm_encode.h"
 #include "index.h"
+#include "rq_encode.h"
 
 using namespace fb200;
 
@@ -1462,6 +1463,84 @@ int b200_icm_encode_paged(
         const int32_t* perturbations, size_t page_bytes) {
     try {
         ICM(p)->encode(codes, x, n, ils_iters, nperts, icm_iters, perturbations, page_bytes);
+    }
+    CATCH_AND_HANDLE
+}
+struct FaissGpuRqEncoder_H {
+    std::unique_ptr<GpuRqEncoder> enc;
+};
+static GpuRqEncoder* RQ(const FaissGpuRqEncoder* p) {
+    if (!p || !p->enc)
+        FB_THROW_MSG("null encoder handle");
+    return p->enc.get();
+}
+int faiss_b200_RqEncoder_new(FaissGpuRqEncoder** p, FaissStandardGpuResources* r, int device, int d, int M, const int* nbits) {
+    try {
+        FB_THROW_IF_NOT_MSG(p != nullptr && nbits != nullptr, "null argument");
+        FB_THROW_IF_NOT_FMT(M >= 1, "M = %d: at least one codebook is needed", M);
+        auto h = std::make_unique<FaissGpuRqEncoder_H>();
+        h->enc = std::make_unique<GpuRqEncoder>(d, std::vector<int>(nbits, nbits + M), RES(r), device);
+        *p = h.release();
+    }
+    CATCH_AND_HANDLE
+}
+void faiss_b200_RqEncoder_free(FaissGpuRqEncoder* p) {
+    delete p;
+}
+int faiss_b200_RqEncoder_set_codebooks(FaissGpuRqEncoder* p, const float* codebooks) {
+    try {
+        RQ(p)->setCodebooks(codebooks);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_b200_RqEncoder_final_beam(const FaissGpuRqEncoder* p, int beam_in, int out_beam, int* beam) {
+    try {
+        FB_THROW_IF_NOT_MSG(beam != nullptr, "null argument");
+        *beam = RQ(p)->finalBeam(beam_in, out_beam);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_b200_RqEncoder_refine_beam(
+        FaissGpuRqEncoder* p, idx_t n, int beam_in, const float* residuals, int out_beam, int32_t* codes, float* residuals_out,
+        float* distances) {
+    return b200_rq_refine_beam_paged(p, n, beam_in, residuals, out_beam, codes, residuals_out, distances, kRqPageBytes);
+}
+int b200_rq_refine_beam_paged(
+        FaissGpuRqEncoder* p, idx_t n, int beam_in, const float* residuals, int out_beam, int32_t* codes, float* residuals_out,
+        float* distances, size_t page_bytes) {
+    try {
+        RQ(p)->refineBeam(n, beam_in, residuals, out_beam, codes, residuals_out, distances, page_bytes);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_b200_RqEncoder_refine_beam_lut(FaissGpuRqEncoder* p, idx_t n, const float* x, int out_beam, int32_t* codes, float* distances) {
+    return b200_rq_refine_beam_lut_paged(p, n, x, out_beam, codes, distances, kRqPageBytes);
+}
+int b200_rq_refine_beam_lut_paged(
+        FaissGpuRqEncoder* p, idx_t n, const float* x, int out_beam, int32_t* codes, float* distances, size_t page_bytes) {
+    try {
+        RQ(p)->refineBeamLUT(n, x, out_beam, codes, distances, page_bytes);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_b200_RqEncoder_compute_codes(
+        FaissGpuRqEncoder* p, const float* x, idx_t n, int use_beam_lut, int max_beam, int search_type, float norm_min,
+        float norm_max, const float* centroids, uint8_t* packed) {
+    return b200_rq_compute_codes_paged(
+            p, x, n, use_beam_lut, max_beam, search_type, norm_min, norm_max, centroids, packed, kRqPageBytes);
+}
+int b200_rq_compute_codes_paged(
+        FaissGpuRqEncoder* p, const float* x, idx_t n, int use_beam_lut, int max_beam, int search_type, float norm_min,
+        float norm_max, const float* centroids, uint8_t* packed, size_t page_bytes) {
+    try {
+        RQ(p)->computeCodes(x, n, use_beam_lut != 0, max_beam, search_type, norm_min, norm_max, centroids, packed, page_bytes);
+    }
+    CATCH_AND_HANDLE
+}
+int faiss_b200_RqEncoder_encode_unpacked(
+        FaissGpuRqEncoder* p, const float* x, idx_t n, int use_beam_lut, int max_beam, int32_t* codes) {
+    try {
+        RQ(p)->encodeUnpacked(x, n, use_beam_lut != 0, max_beam, codes);
     }
     CATCH_AND_HANDLE
 }

@@ -365,6 +365,34 @@ FB200_API int faiss_GpuIcmEncoder_encode(FaissGpuIcmEncoder* enc, int32_t* codes
 /* faiss_GpuIcmEncoder_encode with a page budget of page_bytes instead of 256 MiB */
 FB200_API int b200_icm_encode_paged(FaissGpuIcmEncoder* enc, int32_t* codes, const float* x, idx_t n, size_t ils_iters, size_t nperts, size_t icm_iters, const int32_t* perturbations, size_t page_bytes);
 
+/* ---- GpuRqEncoder (faiss/impl/ResidualQuantizer.cpp:432-520; faiss/impl/residual_quantizer_encode_steps.cpp) ----
+   ResidualQuantizer's beam-search encoding on one device, in both distance modes.  nbits[m] in [1, 12]; every beam in
+   [1, 256].  Every pointer may be host or device memory.  B below is the beam after the M steps,
+   min(beam_in * prod 2^nbits, out_beam) (faiss_b200_RqEncoder_final_beam). */
+typedef struct FaissGpuRqEncoder_H FaissGpuRqEncoder;
+FB200_API int faiss_b200_RqEncoder_new(FaissGpuRqEncoder** p_enc, FaissStandardGpuResources* res, int device, int d, int M, const int* nbits);
+FB200_API void faiss_b200_RqEncoder_free(FaissGpuRqEncoder* enc);
+/* codebooks [total_K][d]: the device copy, the centroid norms and the per-step cross-product blocks */
+FB200_API int faiss_b200_RqEncoder_set_codebooks(FaissGpuRqEncoder* enc, const float* codebooks);
+FB200_API int faiss_b200_RqEncoder_final_beam(const FaissGpuRqEncoder* enc, int beam_in, int out_beam, int* beam);
+/* ResidualQuantizer::refine_beam (use_beam_LUT = 0): residuals [n][beam_in][d] -> codes [n][B][M], residuals_out
+   [n][B][d], distances [n][B]; each output may be NULL */
+FB200_API int faiss_b200_RqEncoder_refine_beam(FaissGpuRqEncoder* enc, idx_t n, int beam_in, const float* residuals, int out_beam, int32_t* codes, float* residuals_out, float* distances);
+/* ResidualQuantizer::refine_beam_LUT (use_beam_LUT = 1), given x [n][d] instead of (query_norms, query_cp): the device
+   computes both.  codes [n][B][M], distances [n][B]; each may be NULL */
+FB200_API int faiss_b200_RqEncoder_refine_beam_lut(FaissGpuRqEncoder* enc, idx_t n, const float* x, int out_beam, int32_t* codes, float* distances);
+/* ResidualQuantizer::compute_codes_add_centroids with out_beam_size max_beam: packed [n][code_size] for search_type
+   ST_decompress, ST_LUT_nonorm, ST_norm_from_LUT, ST_norm_float, ST_norm_qint8 or ST_norm_qint4 (0 .. 5); the other
+   search types return an error.  centroids [n][d] or NULL. */
+FB200_API int faiss_b200_RqEncoder_compute_codes(FaissGpuRqEncoder* enc, const float* x, idx_t n, int use_beam_lut, int max_beam, int search_type, float norm_min, float norm_max, const float* centroids, uint8_t* packed);
+/* the same search, unpacked: codes [n][M] (entry 0 of the beam), for a caller that packs with a search type the
+   device does not */
+FB200_API int faiss_b200_RqEncoder_encode_unpacked(FaissGpuRqEncoder* enc, const float* x, idx_t n, int use_beam_lut, int max_beam, int32_t* codes);
+/* refine_beam, refine_beam_lut and compute_codes with a page budget of page_bytes instead of 256 MiB */
+FB200_API int b200_rq_refine_beam_paged(FaissGpuRqEncoder* enc, idx_t n, int beam_in, const float* residuals, int out_beam, int32_t* codes, float* residuals_out, float* distances, size_t page_bytes);
+FB200_API int b200_rq_refine_beam_lut_paged(FaissGpuRqEncoder* enc, idx_t n, const float* x, int out_beam, int32_t* codes, float* distances, size_t page_bytes);
+FB200_API int b200_rq_compute_codes_paged(FaissGpuRqEncoder* enc, const float* x, idx_t n, int use_beam_lut, int max_beam, int search_type, float norm_min, float norm_max, const float* centroids, uint8_t* packed, size_t page_bytes);
+
 /* ---- Clustering (c_api/Clustering_c.h faiss_kmeans_clustering; faiss/Clustering.cpp:60-380) ----
    Lloyd k-means with the training set resident on the device; x host or device. */
 FB200_API int faiss_b200_kmeans(FaissStandardGpuResources* res, int device, size_t d, size_t n, size_t k, const float* x, int niter, int seed, int max_points_per_centroid, float* centroids_out /* host [k*d] */, float* obj_out /* host [niter] or NULL */);
