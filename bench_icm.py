@@ -22,7 +22,7 @@ import torch
 import faiss_b200 as fb
 from bench import synthetic_dataset
 from oracle import oracle_lsq_np as lo
-from oracle import ref_lsq
+from oracle import ref, ref_lsq
 
 M, K, D, ILS, ICM, NPERTS, SEED = 8, 256, 128, 16, 4, 4, 0x12345
 
@@ -113,7 +113,7 @@ def main():
         q = ref_lsq.LSQ(cb, nperts=NPERTS, icm_iters=ICM)
         cpu_rows = []
         for th in sorted({1, 8, os.cpu_count() or 1}):
-            ref_lsq.set_threads(th)
+            ref.set_omp_threads(th)
             t0 = time.perf_counter()
             cpu, _ = q.icm_encode(cs, xs, ILS, SEED)
             dt = time.perf_counter() - t0

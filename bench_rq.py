@@ -27,7 +27,7 @@ import torch
 
 import faiss_b200 as fb
 from bench import synthetic_dataset
-from oracle import ref_rq
+from oracle import ref, ref_rq
 
 D, M, NBITS, K = 128, 8, 8, 256
 
@@ -116,7 +116,7 @@ def main():
             for beam in (5, 32):
                 q = ref_rq.RQ(D, [NBITS] * M, cb, max_beam_size=beam, use_beam_LUT=lut)
                 for th in sorted({1, 8, os.cpu_count() or 1}):
-                    ref_rq.set_threads(th)
+                    ref.set_omp_threads(th)
                     t0 = time.perf_counter()
                     cpu = q.compute_codes(xs)
                     dt = time.perf_counter() - t0

@@ -1,15 +1,19 @@
 """TEST INFRASTRUCTURE ONLY -- ctypes wrapper over oracle/_ref/libfaiss_ref.so, the UNMODIFIED
-reference CPU library compiled from /root/reference by oracle/Makefile (+ oracle/ref_shim.cpp).
+reference CPU library compiled from the reference tree (REF) by oracle/Makefile (+ oracle/ref_shim.cpp),
+and the loader (Shim) of the shim libraries oracle/_ref/libfaiss_ref_<name>.so that the ref_<name>.py
+modules wrap.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import
 this module.  Nothing under faiss_b200/ does.
 """
 import ctypes
 import os
+import re
 import subprocess
 
 import numpy as np
 
+REF = "/root/reference"  # the reference source tree; oracle/_ref is (re)built only where it is present
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_ref", "libfaiss_ref.so")
 
@@ -19,14 +23,23 @@ _u8 = ctypes.POINTER(ctypes.c_uint8)
 _i32 = ctypes.POINTER(ctypes.c_int)
 
 
-def build(verbose=False):
-    """Compile oracle/_ref from /root/reference (only possible where the reference is mounted)."""
-    if not os.path.isdir("/root/reference/faiss"):
-        return os.path.exists(LIB_PATH)
-    r = subprocess.run(["make", "-C", _HERE, "-j", str(os.cpu_count() or 4)], capture_output=not verbose, text=True)
+def _make(target, verbose):
+    """make -k one oracle/Makefile target; on failure, raise naming every file that did not build"""
+    if not os.path.isdir(os.path.join(REF, "faiss")):
+        return False
+    r = subprocess.run(["make", "-k", "-C", _HERE, "-j", str(os.cpu_count() or 4), target], capture_output=True, text=True)
+    if verbose:
+        print(r.stdout + r.stderr, end="")
     if r.returncode != 0:
-        raise RuntimeError("oracle/_ref build failed:\n" + (r.stdout or "")[-3000:] + (r.stderr or "")[-3000:])
+        failed = sorted(set(re.findall(r"\*\*\* \[(?:\S+: )?(\S+)\] Error", r.stderr)))
+        raise RuntimeError("oracle/_ref: %s failed to build:\n%s" % (", ".join(failed) or target, r.stderr[-3000:]))
     return True
+
+
+def build(verbose=False):
+    """Compile the reference library and every shim library of oracle/Makefile (only where REF is present);
+    returns whether the reference library is there."""
+    return _make("all", verbose) or available()
 
 
 def available():
@@ -40,7 +53,7 @@ def lib():
     global _lib
     if _lib is None:
         if not available():
-            raise RuntimeError("oracle/_ref/libfaiss_ref.so missing: run `make -C oracle` where /root/reference exists")
+            raise RuntimeError("oracle/_ref/libfaiss_ref.so missing: run `make -k -C oracle` where the reference tree is present")
         L = ctypes.CDLL(LIB_PATH)
         L.ref_last_error.restype = ctypes.c_char_p
         L.ref_compile_options.restype = ctypes.c_char_p
@@ -55,8 +68,54 @@ def lib():
 
 
 def _ck(rc):
+    """raise the reference's own message when a call of this library or of any shim library returned non-zero
+    (the shims report through libfaiss_ref.so's one error slot, oracle/ref_shim.h)"""
     if rc != 0:
         raise RuntimeError("reference error: " + lib().ref_last_error().decode(errors="replace"))
+
+
+class Shim:
+    """the shim library oracle/_ref/libfaiss_ref_<name>.so (oracle/ref_<name>_shim.cpp) over this library;
+    declare(L) sets the restype / argtypes of its entry points once it is loaded"""
+
+    def __init__(self, name, declare=None):
+        self.name = name
+        self._target = "_ref/libfaiss_ref_%s.so" % name  # relative to oracle/, as oracle/Makefile names it
+        self.path = os.path.join(_HERE, self._target)
+        self._declare = declare
+        self._lib = None
+        self._own_error = None
+
+    def build(self, verbose=False):
+        """Compile this shim library (and the reference library under it) where REF is present; returns
+        whether it is there."""
+        return _make(self._target, verbose) or self.available()
+
+    def available(self):
+        return available() and os.path.exists(self.path)
+
+    def lib(self):
+        if self._lib is None:
+            lib()  # the reference library itself, with the generic entry points and the error slot
+            if not self.available():
+                raise RuntimeError("oracle/%s missing: run `make -k -C oracle` where the reference tree is present" % self._target)
+            L = ctypes.CDLL(self.path)
+            if self._declare:
+                self._declare(L)
+            # A shim library built before the shims shared libfaiss_ref.so's error slot keeps its message in its own
+            # ref_<name>_last_error.  Such a prebuilt copy is not rebuilt where the reference tree is absent, nor by
+            # make when it is newer than the sources, and it computes the same results, so it is read, not refused.
+            self._own_error = getattr(L, "ref_%s_last_error" % self.name, None)
+            if self._own_error:
+                self._own_error.restype = ctypes.c_char_p
+            self._lib = L
+        return self._lib
+
+    def ck(self, rc):
+        """_ck for a call into this library"""
+        if rc != 0 and self._own_error:
+            raise RuntimeError("reference error: " + self._own_error().decode(errors="replace"))
+        _ck(rc)
 
 
 def _p(a, t):

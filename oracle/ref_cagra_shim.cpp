@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY.
 //
-// extern "C" entry points around the reference's IndexHNSWCagra, compiled by oracle/cagra.mk into
+// extern "C" entry points around the reference's IndexHNSWCagra, compiled by oracle/Makefile into
 // oracle/_ref/libfaiss_ref_cagra.so against the UNMODIFIED reference CPU library (oracle/_ref/libfaiss_ref.so).  The
 // product (faiss_b200/) never loads this file.
 //   ref_cagra_search_graph  an IndexHNSWCagra made from (xb, graph) as GpuIndexCagra::copyTo makes it
@@ -11,30 +11,16 @@
 #include <faiss/IndexHNSW.h>
 
 #include <cmath>
-#include <string>
 
-static thread_local std::string g_cagra_err;
-
-#define CG_TRY try {
-#define CG_CATCH                      \
-    }                                 \
-    catch (const std::exception& e) { \
-        g_cagra_err = e.what();       \
-        return -1;                    \
-    }                                 \
-    return 0;
+#include "ref_shim.h"
 
 extern "C" {
-
-const char* ref_cagra_last_error() {
-    return g_cagra_err.c_str();
-}
 
 // metric: 0 inner product, 1 L2 (faiss::MetricType); graph [n][degree] int64, degree even
 int ref_cagra_search_graph(
         int d, int metric, int64_t n, const float* xb, const int64_t* graph, int degree, int base_level_only,
         int64_t nq, const float* xq, int64_t k, int efSearch, float* D, int64_t* I) {
-    CG_TRY const int M = degree / 2;
+    REF_TRY const int M = degree / 2;
     faiss::IndexHNSWCagra index(d, M, (faiss::MetricType)metric);
     index.base_level_only = base_level_only != 0;
     index.is_trained = true;
@@ -62,12 +48,12 @@ int ref_cagra_search_graph(
     faiss::SearchParametersHNSW p;
     p.efSearch = efSearch;
     index.search(nq, xq, k, D, I, &p);
-    CG_CATCH
+    REF_CATCH
 }
 
 // graph [n][2 * M] int64 (-1 where a row has fewer neighbours)
 int ref_cagra_build_cpu(int d, int metric, int M, int64_t n, const float* xb, int64_t* graph) {
-    CG_TRY faiss::IndexHNSWCagra index(d, M, (faiss::MetricType)metric);
+    REF_TRY faiss::IndexHNSWCagra index(d, M, (faiss::MetricType)metric);
     index.add(n, xb);
     const int degree = index.hnsw.nb_neighbors(0);
     for (int64_t i = 0; i < n; i++) {
@@ -76,7 +62,7 @@ int ref_cagra_build_cpu(int d, int metric, int M, int64_t n, const float* xb, in
         for (size_t j = begin; j < end; j++)
             graph[i * degree + (j - begin)] = index.hnsw.neighbors[j];
     }
-    CG_CATCH
+    REF_CATCH
 }
 
 } // extern "C"

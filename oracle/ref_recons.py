@@ -1,60 +1,28 @@
 """TEST INFRASTRUCTURE ONLY -- ctypes wrapper of the reference's IndexIVF retrieval calls (search_and_reconstruct,
 search_and_return_codes, a direct map + reconstruct): oracle/_ref/libfaiss_ref_recons.so (oracle/ref_recons_shim.cpp,
-built by oracle/recons.mk) over the UNMODIFIED reference CPU library of oracle/ref.py.  The functions take the IVF
+built by oracle/Makefile) over the UNMODIFIED reference CPU library of oracle/ref.py.  The functions take the IVF
 handles of oracle.ref / oracle.ref_sq.
 
 Only tests/, tests/golden/ and bench_reconstruct.py import this module.  Nothing under faiss_b200/ does.
 """
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
 from oracle import ref
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "_ref", "libfaiss_ref_recons.so")
 
 _f = ctypes.POINTER(ctypes.c_float)
 _i64 = ctypes.POINTER(ctypes.c_int64)
 _u8 = ctypes.POINTER(ctypes.c_uint8)
 
 
-def build(verbose=False):
-    """Compile oracle/_ref/libfaiss_ref_recons.so (only where the reference sources are mounted)."""
-    if not os.path.isdir("/root/reference/faiss") or not ref.available():
-        return available()
-    r = subprocess.run(["make", "-C", _HERE, "-f", "recons.mk"], capture_output=not verbose, text=True)
-    if r.returncode != 0:
-        raise RuntimeError("oracle/_ref retrieval shim build failed:\n" + (r.stdout or "")[-3000:] + (r.stderr or "")[-3000:])
-    return True
+def _declare(L):
+    L.ref_ivf_coarse_code_size.restype = ctypes.c_int64
+    L.ref_ivf_coarse_code_size.argtypes = [ctypes.c_void_p]
 
 
-def available():
-    return ref.available() and os.path.exists(LIB_PATH)
-
-
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        ref.lib()
-        if not available():
-            raise RuntimeError("oracle/_ref/libfaiss_ref_recons.so missing: run `make -C oracle -f recons.mk`")
-        L = ctypes.CDLL(LIB_PATH)
-        L.ref_recons_last_error.restype = ctypes.c_char_p
-        L.ref_ivf_coarse_code_size.restype = ctypes.c_int64
-        L.ref_ivf_coarse_code_size.argtypes = [ctypes.c_void_p]
-        _lib = L
-    return _lib
-
-
-def _ck(rc):
-    if rc != 0:
-        raise RuntimeError("reference error: " + lib().ref_recons_last_error().decode(errors="replace"))
+_shim = ref.Shim("recons", _declare)
+LIB_PATH, build, available, lib, _ck = _shim.path, _shim.build, _shim.available, _shim.lib, _shim.ck
 
 
 def _x(x):

@@ -1,19 +1,14 @@
 """TEST INFRASTRUCTURE ONLY -- ctypes wrapper of the reference's ResidualQuantizer encoding:
-oracle/_ref/libfaiss_ref_rq.so (oracle/ref_rq_shim.cpp, built by oracle/rq.mk) over the UNMODIFIED reference CPU
+oracle/_ref/libfaiss_ref_rq.so (oracle/ref_rq_shim.cpp, built by oracle/Makefile) over the UNMODIFIED reference CPU
 library of oracle/ref.py.
 
 Only tests/, tests/golden/ and bench_rq.py import this module.  Nothing under faiss_b200/ does.
 """
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
 from oracle import ref
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "_ref", "libfaiss_ref_rq.so")
 
 _f = ctypes.POINTER(ctypes.c_float)
 _i32 = ctypes.POINTER(ctypes.c_int32)
@@ -25,55 +20,26 @@ ST_norm_cqint8, ST_norm_cqint4, ST_norm_lsq2x4, ST_norm_rq2x4 = range(6, 10)
 Train_default, Train_progressive_dim, Train_refine_codebook = 0, 1, 2
 
 
-def build(verbose=False):
-    """Compile oracle/_ref/libfaiss_ref_rq.so (only where the reference sources are mounted)."""
-    if not os.path.isdir("/root/reference/faiss") or not ref.available():
-        return available()
-    r = subprocess.run(["make", "-C", _HERE, "-f", "rq.mk"], capture_output=not verbose, text=True)
-    if r.returncode != 0:
-        raise RuntimeError("oracle/_ref RQ shim build failed:\n" + (r.stdout or "")[-3000:] + (r.stderr or "")[-3000:])
-    return True
+def _declare(L):
+    L.ref_rq_new.restype = ctypes.c_void_p
+    L.ref_rq_new.argtypes = [ctypes.c_int, ctypes.c_int, _i32, ctypes.c_int, _f]
+    L.ref_rq_free.argtypes = [ctypes.c_void_p]
+    L.ref_rq_free.restype = None
+    L.ref_rq_set_params.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float]
+    L.ref_rq_code_size.argtypes = [ctypes.c_void_p]
+    L.ref_rq_code_size.restype = ctypes.c_int64
+    L.ref_rq_cross_size.argtypes = [ctypes.c_void_p]
+    L.ref_rq_cross_size.restype = ctypes.c_int64
+    L.ref_rq_train.argtypes = [ctypes.c_void_p, ctypes.c_int64, _f, ctypes.c_int, ctypes.c_int, ctypes.c_int]
+    L.ref_rq_tables.argtypes = [ctypes.c_void_p, _f, _f, _f]
+    L.ref_rq_refine_beam.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, _f, ctypes.c_int, _i32, _f, _f]
+    L.ref_rq_refine_beam_lut.argtypes = [ctypes.c_void_p, ctypes.c_int64, _f, ctypes.c_int, _i32, _f]
+    L.ref_rq_compute_codes.argtypes = [ctypes.c_void_p, _f, ctypes.c_int64, _f, _u8]
+    L.ref_rq_decode.argtypes = [ctypes.c_void_p, _u8, ctypes.c_int64, _f]
 
 
-def available():
-    return ref.available() and os.path.exists(LIB_PATH)
-
-
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        ref.lib()
-        if not available():
-            raise RuntimeError("oracle/_ref/libfaiss_ref_rq.so missing: run `make -C oracle -f rq.mk`")
-        L = ctypes.CDLL(LIB_PATH)
-        L.ref_rq_last_error.restype = ctypes.c_char_p
-        L.ref_rq_new.restype = ctypes.c_void_p
-        L.ref_rq_new.argtypes = [ctypes.c_int, ctypes.c_int, _i32, ctypes.c_int, _f]
-        L.ref_rq_free.argtypes = [ctypes.c_void_p]
-        L.ref_rq_free.restype = None
-        L.ref_rq_set_threads.argtypes = [ctypes.c_int]
-        L.ref_rq_set_threads.restype = None
-        L.ref_rq_set_params.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float]
-        L.ref_rq_code_size.argtypes = [ctypes.c_void_p]
-        L.ref_rq_code_size.restype = ctypes.c_int64
-        L.ref_rq_cross_size.argtypes = [ctypes.c_void_p]
-        L.ref_rq_cross_size.restype = ctypes.c_int64
-        L.ref_rq_train.argtypes = [ctypes.c_void_p, ctypes.c_int64, _f, ctypes.c_int, ctypes.c_int, ctypes.c_int]
-        L.ref_rq_tables.argtypes = [ctypes.c_void_p, _f, _f, _f]
-        L.ref_rq_refine_beam.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, _f, ctypes.c_int, _i32, _f, _f]
-        L.ref_rq_refine_beam_lut.argtypes = [ctypes.c_void_p, ctypes.c_int64, _f, ctypes.c_int, _i32, _f]
-        L.ref_rq_compute_codes.argtypes = [ctypes.c_void_p, _f, ctypes.c_int64, _f, _u8]
-        L.ref_rq_decode.argtypes = [ctypes.c_void_p, _u8, ctypes.c_int64, _f]
-        _lib = L
-    return _lib
-
-
-def _ck(rc):
-    if rc != 0:
-        raise RuntimeError("reference error: " + lib().ref_rq_last_error().decode(errors="replace"))
+_shim = ref.Shim("rq", _declare)
+LIB_PATH, build, available, lib, _ck = _shim.path, _shim.build, _shim.available, _shim.lib, _shim.ck
 
 
 def _p(a, t):
@@ -102,8 +68,8 @@ class RQ:
         self.set_params(max_beam_size, use_beam_LUT, norm_min, norm_max)
 
     def __del__(self):
-        if getattr(self, "h", None) and _lib is not None:
-            _lib.ref_rq_free(self.h)
+        if getattr(self, "h", None):
+            lib().ref_rq_free(self.h)
             self.h = None
 
     def set_params(self, max_beam_size, use_beam_LUT, norm_min=0.0, norm_max=0.0):
@@ -164,7 +130,3 @@ class RQ:
         _ck(lib().ref_rq_decode(self.h, _p(packed, _u8), packed.shape[0], _p(out, _f)))
         return out
 
-
-def set_threads(n):
-    """the OpenMP thread count of the reference encoder"""
-    lib().ref_rq_set_threads(int(n))

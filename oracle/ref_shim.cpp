@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY.
 //
-// A thin extern "C" shim over the UNMODIFIED reference CPU library (compiled from
-// /root/reference by oracle/Makefile into oracle/_ref/libfaiss_ref.so).  It exposes the
+// A thin extern "C" shim over the UNMODIFIED reference CPU library (compiled from the
+// reference tree by oracle/Makefile into oracle/_ref/libfaiss_ref.so).  It exposes the
 // reference's own IndexFlat / IndexIVFFlat / IndexIVFPQ / Clustering / IndexShards objects
 // to the Python test-suite and to bench.py's cpu_baseline / --impl reference legs through
 // ctypes.  It contains no algorithm of its own: every function forwards to a reference
@@ -24,21 +24,18 @@
 #include <cstring>
 #include <string>
 
+#include "ref_shim.h"
+
 using faiss::idx_t;
 
+// the error slot of this library and of every shim library linked against it (ref_shim.h)
 static thread_local std::string g_err;
-
-#define REF_TRY try {
-#define REF_CATCH                     \
-    }                                 \
-    catch (const std::exception& e) { \
-        g_err = e.what();             \
-        return -1;                    \
-    }                                 \
-    return 0;
 
 extern "C" {
 
+void ref_set_last_error(const char* msg) {
+    g_err = msg;
+}
 const char* ref_last_error() {
     return g_err.c_str();
 }

@@ -1,20 +1,15 @@
 """TEST INFRASTRUCTURE ONLY -- ctypes wrapper of the reference's IndexIVFScalarQuantizer:
-oracle/_ref/libfaiss_ref_sq.so (oracle/ref_sq_shim.cpp, built by oracle/sq.mk) over the UNMODIFIED
+oracle/_ref/libfaiss_ref_sq.so (oracle/ref_sq_shim.cpp, built by oracle/Makefile) over the UNMODIFIED
 reference CPU library of oracle/ref.py.  The handles are reference IndexIVF objects, so every generic
 Index / IVF call of oracle.ref applies to them.
 
 Only tests/ and tests/golden/ import this module.  Nothing under faiss_b200/ does.
 """
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
 from oracle import ref
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "_ref", "libfaiss_ref_sq.so")
 
 _f = ctypes.POINTER(ctypes.c_float)
 _i64 = ctypes.POINTER(ctypes.c_int64)
@@ -25,41 +20,14 @@ QT_8bit, QT_4bit, QT_8bit_uniform, QT_4bit_uniform, QT_fp16, QT_8bit_direct, QT_
 QT_NAMES = ["8bit", "4bit", "8bit_uniform", "4bit_uniform", "fp16", "8bit_direct", "6bit"]
 
 
-def build(verbose=False):
-    """Compile oracle/_ref/libfaiss_ref_sq.so (only where the reference sources are mounted)."""
-    if not os.path.isdir("/root/reference/faiss") or not ref.available():
-        return available()
-    r = subprocess.run(["make", "-C", _HERE, "-f", "sq.mk"], capture_output=not verbose, text=True)
-    if r.returncode != 0:
-        raise RuntimeError("oracle/_ref SQ shim build failed:\n" + (r.stdout or "")[-3000:] + (r.stderr or "")[-3000:])
-    return True
+def _declare(L):
+    L.ref_ivfsq_new.restype = ctypes.c_void_p
+    L.ref_ivfsq_trained_size.restype = ctypes.c_int64
+    L.ref_ivfsq_code_size.restype = ctypes.c_int64
 
 
-def available():
-    return ref.available() and os.path.exists(LIB_PATH)
-
-
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        ref.lib()  # the reference library itself, with the generic entry points
-        if not available():
-            raise RuntimeError("oracle/_ref/libfaiss_ref_sq.so missing: run `make -C oracle -f sq.mk`")
-        L = ctypes.CDLL(LIB_PATH)
-        L.ref_sq_last_error.restype = ctypes.c_char_p
-        L.ref_ivfsq_new.restype = ctypes.c_void_p
-        L.ref_ivfsq_trained_size.restype = ctypes.c_int64
-        L.ref_ivfsq_code_size.restype = ctypes.c_int64
-        _lib = L
-    return _lib
-
-
-def _ck(rc):
-    if rc != 0:
-        raise RuntimeError("reference error: " + lib().ref_sq_last_error().decode(errors="replace"))
+_shim = ref.Shim("sq", _declare)
+LIB_PATH, build, available, lib, _ck = _shim.path, _shim.build, _shim.available, _shim.lib, _shim.ck
 
 
 class IndexIVFScalarQuantizer(ref._IVF):
@@ -68,7 +36,7 @@ class IndexIVFScalarQuantizer(ref._IVF):
     def __init__(self, d, nlist, qtype, metric=1, by_residual=True):
         h = lib().ref_ivfsq_new(int(d), ctypes.c_int64(nlist), int(qtype), int(metric), int(bool(by_residual)))
         if not h:
-            raise RuntimeError("reference error: " + lib().ref_sq_last_error().decode(errors="replace"))
+            _ck(-1)
         super().__init__(h)
         self.d, self.qtype, self.by_residual = d, int(qtype), bool(by_residual)
 

@@ -1,6 +1,6 @@
 // TEST DRIVER: the reference's LocalSearchQuantizer with B200IcmEncoderFactory as its icm_encoder_factory, against the
 // same quantizer with the CPU encoder (faiss/impl/LocalSearchQuantizer.cpp).  Built by
-// tests/adapter/build_adapter_lsq.py, run by tests/test_adapter_lsq_gpu.py; prints ADAPTER_LSQ_OK on success.
+// tests/adapter/build_adapter.py, run by tests/test_adapter_gpu.py; prints ADAPTER_LSQ_OK on success.
 //   1. integer codebooks and vectors (every fp32 sum exact): compute_codes gives the CPU's codes byte for byte, over
 //      several chunks, and icm_encode leaves the caller's std::mt19937 where the CPU leaves it (its next output);
 //   2. LocalSearchQuantizer::train through the factory reaches an encode error within 1.05x of the CPU-trained one.

@@ -1,6 +1,6 @@
 // search_and_reconstruct / reconstruct_batch through the faiss_b200 adapter (needs a GPU; built by
-// tests/adapter/build_adapter_recons.py where the reference's headers are available, executed by
-// tests/test_adapter_recons_gpu.py).  faiss::Index::search_and_reconstruct on adapter clones of IndexFlatL2,
+// tests/adapter/build_adapter.py where the reference's headers are available, executed by
+// tests/test_adapter_gpu.py).  faiss::Index::search_and_reconstruct on adapter clones of IndexFlatL2,
 // IndexIVFFlat and IndexIVFPQ whose ids are stored twice with different vectors, against the CPU indexes:
 //   * D and I equal the adapter's search;
 //   * R is the entry the search scored: one of the CPU's entries under that id, and (exact integer data) its

@@ -1,5 +1,5 @@
 // TEST DRIVER: the reference's ResidualQuantizer through the adapter, against the same quantizer on the CPU
-// (faiss/impl/ResidualQuantizer.cpp).  Built by tests/adapter/build_adapter_rq.py, run by tests/test_adapter_rq_gpu.py;
+// (faiss/impl/ResidualQuantizer.cpp).  Built by tests/adapter/build_adapter.py, run by tests/test_adapter_gpu.py;
 // prints ADAPTER_RQ_OK on success.
 //   1. integer codebooks and vectors (every fp32 sum exact): B200ResidualQuantizer::compute_codes gives the CPU's bytes
 //      in both modes, for the search types the device packs and for two the adapter packs on the host, with and

@@ -1,5 +1,5 @@
-// Filtered search through the faiss_b200 adapter (needs a GPU; built by tests/adapter/build_adapter_sel.py where the
-// reference's headers are available, executed by tests/test_adapter_sel_gpu.py).  faiss::Index::search(..., params)
+// Filtered search through the faiss_b200 adapter (needs a GPU; built by tests/adapter/build_adapter.py where the
+// reference's headers are available, executed by tests/test_adapter_gpu.py).  faiss::Index::search(..., params)
 // with the reference's own IDSelectorRange / IDSelectorBatch / IDSelectorNot / IDSelectorAnd, a user IDSelector
 // subclass (the callback path), on an adapter
 // clone of IndexFlatL2 and of IndexIVFFlat (add_with_ids ids with negative and >= 2^40 values), compared with the
