@@ -248,33 +248,33 @@ void InterruptCallback::check() {
         FB_THROW_MSG("computation interrupted");
 }
 
-void GpuIndex::search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, const SearchParameters* params) const {
-    struct Guard {
-        const SearchParameters*& slot;
-        const uint32_t*& mask;
-        ~Guard() {
-            slot = nullptr;
-            mask = nullptr;
-        }
-    } guard{callParams_, callMask_};
-    callParams_ = params;
-    // the selector is evaluated once per call, before the query pages (temporary memory, released last)
-    GpuMemoryReservation mask;
-    if (params && params->sel && n > 0 && this->ntotal > 0) {
-        DeviceScope scope(config_.device);
-        mask = selMask_(*params->sel);
-        callMask_ = mask.as<uint32_t>();
-    }
-    search(n, x, k, distances, labels);
+void GpuIndex::search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels) const {
+    search(n, x, k, distances, labels, nullptr);
 }
 
-void GpuIndex::search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels) const {
+void GpuIndex::search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, const SearchParameters* params) const {
+    searchPaged_(n, x, k, distances, labels, params, 0, [&](idx_t nb, const float* xDev, float* dDev, idx_t* iDev, const SearchCall& call) {
+        searchImpl_(nb, xDev, (int)k, dDev, iDev, call);
+    });
+}
+
+void GpuIndex::searchPaged_(
+        idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, const SearchParameters* params,
+        size_t resultBytes, const SearchPage& page) const {
     DeviceScope scope(config_.device);
     FB_THROW_IF_NOT_MSG(this->is_trained, "Index not trained");
     validateKSelect(k);
     if (n == 0)
         return;
     FB_THROW_IF_NOT_MSG(x && distances && labels, "null pointer passed to search");
+    SearchCall call;
+    call.params = params;
+    // the selector is evaluated once per call, before the query pages (temporary memory, released last)
+    GpuMemoryReservation mask;
+    if (params && params->sel && this->ntotal > 0) {
+        mask = selMask_(*params->sel, call.selected);
+        call.mask = mask.as<uint32_t>();
+    }
     auto stream = stream_();
     // Query paging (role of searchFromCpuPaged_ / searchNonPaged_, faiss/gpu/GpuIndex.cu:554-788).
     // minPagedSize_ is only the THRESHOLD above which host-resident queries are paged (as upstream:
@@ -282,13 +282,15 @@ void GpuIndex::search(idx_t n, const float* x, idx_t k, float* distances, idx_t*
     // byte budget (kSearchPageBytes) and is further bounded by k so that a page's result staging
     // (k * 12 B per query, a few partial copies inside the kernels) stays within the temp arena.
     constexpr size_t kSearchPageBytes = size_t(256) << 20;
-    const bool hostQueries = getDeviceForAddress(x) != config_.device;
+    const bool hostPaged = getDeviceForAddress(x) != config_.device && (size_t)n * d * sizeof(float) >= minPagedSize_;
     idx_t maxQ = idx_t(1) << 18;
-    if (hostQueries && (size_t)n * d * sizeof(float) >= minPagedSize_)
+    if (hostPaged)
         maxQ = std::min<idx_t>(maxQ, (idx_t)(kSearchPageBytes / (sizeof(float) * d)));
     maxQ = std::min<idx_t>(maxQ, (idx_t)((size_t(1) << 30) / ((size_t)k * 12 * 8)));
+    if (resultBytes > 0)
+        maxQ = std::min<idx_t>(maxQ, (idx_t)(kRetrievalPageBytes / ((size_t)k * resultBytes)));
     maxQ = std::max<idx_t>(maxQ, 1);
-    if (hostQueries && (size_t)n * d * sizeof(float) >= minPagedSize_ && searchFromCpuPaged_(n, x, k, distances, labels, maxQ))
+    if (hostPaged && searchFromCpuPaged_(n, x, k, distances, labels, maxQ, call, page))
         return;
     for (idx_t i0 = 0; i0 < n; i0 += maxQ) {
         InterruptCallback::check(); // between query pages
@@ -296,8 +298,8 @@ void GpuIndex::search(idx_t n, const float* x, idx_t k, float* distances, idx_t*
         DeviceView<float> xv(resources_.get(), config_.device, x + (size_t)i0 * d, (size_t)nb * d, stream);
         DeviceOut<float> dv(resources_.get(), config_.device, distances + (size_t)i0 * k, (size_t)nb * k);
         DeviceOut<idx_t> lv(resources_.get(), config_.device, labels + (size_t)i0 * k, (size_t)nb * k);
-        callRow0_ = i0;
-        searchImpl_(nb, xv.ptr, (int)k, dv.ptr, lv.ptr);
+        call.row0 = i0;
+        page(nb, xv.ptr, dv.ptr, lv.ptr, call);
         dv.finish(stream);
         lv.finish(stream);
         if (dv.staged || lv.staged || xv.hold.data)
@@ -311,7 +313,9 @@ void GpuIndex::search(idx_t n, const float* x, idx_t k, float* distances, idx_t*
 // default stream.  (searchImpl_ synchronises with the host -- certificate flags, list offsets -- so the overlap needs
 // a second host thread rather than the reference's single-thread event chain.)  Returns false when there is no
 // pinned memory to page through; the caller then takes the plain loop.
-bool GpuIndex::searchFromCpuPaged_(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, idx_t maxQ) const {
+bool GpuIndex::searchFromCpuPaged_(
+        idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, idx_t maxQ, SearchCall call,
+        const SearchPage& page) const {
     auto pinned = resources_->getPinnedMemory();
     const size_t half = pinned.second / 2;
     const idx_t pageQ = std::min<idx_t>(maxQ, (idx_t)(half / (sizeof(float) * d)));
@@ -390,8 +394,8 @@ bool GpuIndex::searchFromCpuPaged_(idx_t n, const float* x, idx_t k, float* dist
             CUDA_VERIFY(cudaStreamWaitEvent(stream, ready[b], 0));
             DeviceOut<float> dv(resources_.get(), config_.device, distances + (size_t)i0 * k, (size_t)nb * k);
             DeviceOut<idx_t> lv(resources_.get(), config_.device, labels + (size_t)i0 * k, (size_t)nb * k);
-            callRow0_ = i0;
-            searchImpl_(nb, devBuf[b].as<float>(), (int)k, dv.ptr, lv.ptr);
+            call.row0 = i0;
+            page(nb, devBuf[b].as<float>(), dv.ptr, lv.ptr, call);
             dv.finish(stream);
             lv.finish(stream);
             CUDA_VERIFY(cudaStreamSynchronize(stream));
@@ -531,10 +535,10 @@ void GpuIndexFlat::fillEmpty_(idx_t n, int k, float* dDev, idx_t* iDev) const {
     CUDA_VERIFY(cudaStreamSynchronize(stream));
 }
 
-GpuMemoryReservation GpuIndexFlat::selMask_(const IDSelector& sel) const {
+GpuMemoryReservation GpuIndexFlat::selMask_(const IDSelector& sel, idx_t& selected) const {
     auto mask = resources_->temp(config_.device, sizeof(uint32_t) * slotMaskWords(this->ntotal));
     buildSlotMask(resources_.get(), config_.device, sel, this->ntotal, nullptr, nullptr, mask.as<uint32_t>(), stream_());
-    callSelected_ = runCountMask(resources_.get(), config_.device, mask.as<uint32_t>(), this->ntotal, stream_());
+    selected = runCountMask(resources_.get(), config_.device, mask.as<uint32_t>(), this->ntotal, stream_());
     return mask;
 }
 
@@ -545,10 +549,11 @@ GpuMemoryReservation GpuIndexFlat::selMask_(const IDSelector& sel) const {
 // 10 %); the two meet near 250k rows, 1 in 40.  Both costs scale with nq and d alike.
 constexpr idx_t kCompactRatio = 40;
 
-void GpuIndexFlat::searchCompacted_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, idx_t selected) const {
+void GpuIndexFlat::searchCompacted_(
+        idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const uint32_t* mask, idx_t selected) const {
     auto stream = stream_();
     auto rows = resources_->temp(config_.device, sizeof(idx_t) * this->ntotal);
-    runCompactMask(resources_.get(), config_.device, callMask_, this->ntotal, rows.as<idx_t>(), stream);
+    runCompactMask(resources_.get(), config_.device, mask, this->ntotal, rows.as<idx_t>(), stream);
     auto sub = resources_->temp(config_.device, sizeof(float) * selected * d);
     runGatherRows(rows_(), rows.as<idx_t>(), selected, d, sub.as<float>(), stream, yHalf_()); // fp16 widens exactly
     runFlatExact(
@@ -557,13 +562,10 @@ void GpuIndexFlat::searchCompacted_(idx_t n, const float* xDev, int k, float* dD
     runRemapLabels(iDev, n * k, rows.as<idx_t>(), stream);
 }
 
-void GpuIndexFlat::search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels) const {
-    lastSearchFallbackQueries = 0; // summed over the query pages
-    GpuIndex::search(n, x, k, distances, labels);
-}
-
-void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
+void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const SearchCall& call) const {
     auto stream = stream_();
+    if (call.row0 == 0)
+        lastSearchFallbackQueries = 0;
     lastSearchUsedTensorCores = 0;
     lastSearchOperandBits = 0;
     if (this->ntotal == 0) {
@@ -574,15 +576,14 @@ void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, i
     const bool tc = useTensorCores_(k, n);
     GpuMemoryReservation qHold;
     xDev = roundedQueries_(n, xDev, qHold);
-    const uint32_t* mask = callMask_;
+    const uint32_t* mask = call.mask;
     if (mask) {
-        const idx_t selected = callSelected_;
-        if (selected == 0) {
+        if (call.selected == 0) {
             fillEmpty_(n, k, dDev, iDev);
             return;
         }
-        if (selected * kCompactRatio <= this->ntotal) {
-            searchCompacted_(n, xDev, k, dDev, iDev, selected);
+        if (call.selected * kCompactRatio <= this->ntotal) {
+            searchCompacted_(n, xDev, k, dDev, iDev, mask, call.selected);
             return;
         }
     }
@@ -603,10 +604,10 @@ bool GpuIndexFlat::shardPoolingEligible(int k, idx_t n) const {
     return useTensorCores_(k, n);
 }
 
-void GpuIndexFlat::searchShardDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* flatShard) const {
-    lastSearchFallbackQueries = 0;
+void GpuIndexFlat::searchShardDevice(
+        idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* flatShard, const SearchCall& call) const {
     if (!flatShard) {
-        searchImpl_(n, xDev, k, dDev, iDev);
+        searchImpl_(n, xDev, k, dDev, iDev, call);
         return;
     }
     FB_THROW_IF_NOT_MSG(shardPoolingEligible(k, n), "pooled sharded search requested on a shard that cannot take the tensor-core path");
@@ -614,7 +615,9 @@ void GpuIndexFlat::searchShardDevice(idx_t n, const float* xDev, int k, float* d
     tc_.prepare(rows_(), this->ntotal, searchMetric_(), yHalf_(), stream);
     GpuMemoryReservation qHold;
     xDev = roundedQueries_(n, xDev, qHold);
-    lastSearchFallbackQueries = (int)tc_.search(xDev, n, k, dDev, iDev, stream, flatShard);
+    if (call.row0 == 0)
+        lastSearchFallbackQueries = 0;
+    lastSearchFallbackQueries += (int)tc_.search(xDev, n, k, dDev, iDev, stream, flatShard);
     lastSearchUsedTensorCores = 1;
     lastSearchOperandBits = tc_.lastOperandBits();
 }
@@ -1401,11 +1404,11 @@ GpuMemoryReservation GpuIndexIVF::coarseResiduals_(idx_t n, const float* xDev, c
     return resid;
 }
 
-void GpuIndexIVF::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
+void GpuIndexIVF::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const SearchCall& call) const {
     // per-call SearchParametersIVF override the index fields (faiss/gpu/GpuIndexIVF.cu:383-406)
     size_t use_nprobe = nprobe, use_max_codes = max_codes;
-    if (callParams_) {
-        auto* ivfParams = dynamic_cast<const SearchParametersIVF*>(callParams_);
+    if (call.params) {
+        auto* ivfParams = dynamic_cast<const SearchParametersIVF*>(call.params);
         FB_THROW_IF_NOT_MSG(ivfParams != nullptr, "IVF search: search parameters must be SearchParametersIVF");
         use_nprobe = ivfParams->nprobe;
         use_max_codes = ivfParams->max_codes;
@@ -1421,10 +1424,10 @@ void GpuIndexIVF::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, id
     auto cI = resources_->temp(config_.device, sizeof(idx_t) * n * np);
     // coarse quantisation = a Flat search with k = nprobe over the centroids (IVFBase.cu:509-545)
     quantizer->searchDevice(n, xDev, np, cD.as<float>(), cI.as<idx_t>());
-    scanImpl_(n, xDev, cI.as<idx_t>(), cD.as<float>(), np, k, dDev, iDev);
+    scanImpl_(n, xDev, cI.as<idx_t>(), cD.as<float>(), np, k, dDev, iDev, call);
 }
 
-GpuMemoryReservation GpuIndexIVF::selMask_(const IDSelector& sel) const {
+GpuMemoryReservation GpuIndexIVF::selMask_(const IDSelector& sel, idx_t&) const {
     const int64_t slots = lists_->arenaElems();
     auto mask = resources_->temp(config_.device, sizeof(uint32_t) * slotMaskWords(slots));
     std::vector<uint8_t> valid; // a callback is only called for the occupied slots
@@ -1460,7 +1463,7 @@ void GpuIndexIVF::search_preassigned(
     DeviceView<float> cv(resources_.get(), config_.device, centroid_dis, (size_t)n * np, stream);
     DeviceOut<float> dv(resources_.get(), config_.device, distances, (size_t)n * k);
     DeviceOut<idx_t> lv(resources_.get(), config_.device, labels, (size_t)n * k);
-    scanImpl_(n, xv.ptr, av.ptr, cv.ptr, np, (int)k, dv.ptr, lv.ptr);
+    scanImpl_(n, xv.ptr, av.ptr, cv.ptr, np, (int)k, dv.ptr, lv.ptr, SearchCall());
     dv.finish(stream);
     lv.finish(stream);
     CUDA_VERIFY(cudaStreamSynchronize(stream));
@@ -1545,51 +1548,17 @@ void GpuIndexIVF::searchWithSlots_(
         idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, const SearchParameters* params,
         size_t resultBytes, const std::function<void(idx_t, idx_t, const idx_t*)>& page) const {
     DeviceScope scope(config_.device);
-    FB_THROW_IF_NOT_MSG(this->is_trained, "Index not trained");
-    validateKSelect(k);
-    if (n == 0)
-        return;
-    FB_THROW_IF_NOT_MSG(x && distances && labels, "null pointer passed to search");
-    struct Guard {
-        const SearchParameters*& params;
-        const uint32_t*& mask;
-        const IvfSlotOutput*& slots;
-        ~Guard() {
-            params = nullptr;
-            mask = nullptr;
-            slots = nullptr;
-        }
-    } guard{callParams_, callMask_, callSlots_};
-    callParams_ = params;
-    GpuMemoryReservation mask;
-    if (params && params->sel && this->ntotal > 0) {
-        mask = selMask_(*params->sel);
-        callMask_ = mask.as<uint32_t>();
-    }
-    auto stream = stream_();
     const int64_t slotsTotal = lists_->arenaElems();
     auto identity = resources_->device_alloc(config_.device, sizeof(idx_t) * std::max<int64_t>(1, slotsTotal), AllocType::Other);
-    runIvfIdentitySlots(identity.as<idx_t>(), slotsTotal, stream);
-    // query pages: search()'s bound on the result staging, and a bound on the page's decoded output
-    idx_t maxQ = std::min<idx_t>(idx_t(1) << 18, (idx_t)((size_t(1) << 30) / ((size_t)k * 12 * 8)));
-    maxQ = std::min<idx_t>(maxQ, (idx_t)(kRetrievalPageBytes / ((size_t)k * resultBytes)));
-    maxQ = std::max<idx_t>(maxQ, 1);
-    for (idx_t i0 = 0; i0 < n; i0 += maxQ) {
-        InterruptCallback::check(); // between query pages
-        const idx_t nb = std::min(maxQ, n - i0);
-        DeviceView<float> xv(resources_.get(), config_.device, x + (size_t)i0 * d, (size_t)nb * d, stream);
-        DeviceOut<float> dv(resources_.get(), config_.device, distances + (size_t)i0 * k, (size_t)nb * k);
-        DeviceOut<idx_t> lv(resources_.get(), config_.device, labels + (size_t)i0 * k, (size_t)nb * k);
+    runIvfIdentitySlots(identity.as<idx_t>(), slotsTotal, stream_());
+    searchPaged_(n, x, k, distances, labels, params, resultBytes, [&](idx_t nb, const float* xDev, float* dDev, idx_t* iDev, const SearchCall& call) {
         auto slots = resources_->temp(config_.device, sizeof(idx_t) * nb * k);
         const IvfSlotOutput so{identity.as<idx_t>(), lists_->ids(), slots.as<idx_t>()};
-        callSlots_ = &so;
-        searchImpl_(nb, xv.ptr, (int)k, dv.ptr, lv.ptr);
-        callSlots_ = nullptr;
-        page(i0, nb, slots.as<idx_t>());
-        dv.finish(stream);
-        lv.finish(stream);
-        CUDA_VERIFY(cudaStreamSynchronize(stream));
-    }
+        SearchCall withSlots = call;
+        withSlots.slots = &so;
+        searchImpl_(nb, xDev, (int)k, dDev, iDev, withSlots);
+        page(call.row0, nb, slots.as<idx_t>());
+    });
 }
 
 void GpuIndexIVF::search_and_reconstruct(
@@ -1655,11 +1624,12 @@ void GpuIndexIVFFlat::scanImpl_(
         int np,
         int k,
         float* dDev,
-        idx_t* iDev) const {
+        idx_t* iDev,
+        const SearchCall& call) const {
     runIvfFlatScan(
             resources_.get(), config_.device, xDev, n, d, probes, np, lists_->dStart(), lists_->dLen(),
-            reinterpret_cast<const float*>(lists_->codes()), scanIds_(), lists_->arenaElems(), k, metric_type, dDev,
-            iDev, stream_(), callMask_, callSlots_);
+            reinterpret_cast<const float*>(lists_->codes()), scanIds_(call), lists_->arenaElems(), k, metric_type, dDev,
+            iDev, stream_(), call.mask, call.slots);
 }
 
 IvfStoredLayout GpuIndexIVFFlat::storedLayout_() const {
@@ -1884,20 +1854,21 @@ void GpuIndexIVFPQ::scanImpl_(
         int np,
         int k,
         float* dDev,
-        idx_t* iDev) const {
+        idx_t* iDev,
+        const SearchCall& call) const {
     FB_THROW_IF_NOT_MSG(pqCentroids_.size() > 0, "PQ not trained");
     if (lists_->interleaved()) {
         runIvfPqScanInterleaved(
                 resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np, quantizer->vectorsDevice(),
                 pqCentroidsT_.data(), precomputedActive_() ? (ensureTerm2_(), term2_.data()) : nullptr,
-                lists_->codeSize(), nibbleLayout_(), lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(),
-                lists_->arenaElems(), k, metric_type, dDev, iDev, stream_(), callMask_, callSlots_);
+                lists_->codeSize(), nibbleLayout_(), lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(call),
+                lists_->arenaElems(), k, metric_type, dDev, iDev, stream_(), call.mask, call.slots);
         return;
     }
     runIvfPqScan(
             resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np, quantizer->vectorsDevice(),
-            pqCentroids_.data(), M_, nbits_, lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(), k,
-            metric_type, dDev, iDev, stream_(), callMask_, callSlots_);
+            pqCentroids_.data(), M_, nbits_, lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(call), k,
+            metric_type, dDev, iDev, stream_(), call.mask, call.slots);
 }
 
 // IndexIVFPQ::reconstruct_from_offset (faiss/IndexIVFPQ.cpp:358-372): pq.decode, then + the list's centroid
@@ -2096,14 +2067,15 @@ void GpuIndexIVFScalarQuantizer::scanImpl_(
         int np,
         int k,
         float* dDev,
-        idx_t* iDev) const {
+        idx_t* iDev,
+        const SearchCall& call) const {
     FB_THROW_IF_NOT_MSG(params_.size() == (size_t)4 * d, "scalar quantizer not trained");
     const bool needCentroids = by_residual && metric_type == METRIC_L2;
     runIvfSqScan(
             resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np,
             needCentroids ? quantizer->vectorsDevice() : nullptr, by_residual, qtype_, params_.data() + 2 * d,
-            lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(), lists_->arenaElems(), lists_->codeSize(), k,
-            metric_type, dDev, iDev, stream_(), callMask_, callSlots_);
+            lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(call), lists_->arenaElems(), lists_->codeSize(), k,
+            metric_type, dDev, iDev, stream_(), call.mask, call.slots);
 }
 
 // IndexIVFScalarQuantizer::reconstruct_from_offset (faiss/IndexScalarQuantizer.cpp:400-425): sq.decode, then + the
@@ -2232,13 +2204,13 @@ void GpuIndexCagra::copyTo(float* xb, idx_t* graph) const {
     CUDA_VERIFY(cudaMemcpy(graph, g.data(), sizeof(idx_t) * g.size(), cudaMemcpyDefault));
 }
 
-GpuMemoryReservation GpuIndexCagra::selMask_(const IDSelector&) const {
+GpuMemoryReservation GpuIndexCagra::selMask_(const IDSelector&, idx_t&) const {
     FB_THROW_MSG("GpuIndexCagra does not support SearchParameters::sel");
 }
 
-void GpuIndexCagra::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
+void GpuIndexCagra::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const SearchCall& call) const {
     const SearchParametersCagra defaults;
-    const auto* sp = dynamic_cast<const SearchParametersCagra*>(callParams_);
+    const auto* sp = dynamic_cast<const SearchParametersCagra*>(call.params);
     if (!sp)
         sp = &defaults;
     FB_THROW_IF_NOT_MSG(
@@ -2303,7 +2275,7 @@ void GpuIndexCagra::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, 
         InterruptCallback::check(); // between query batches
         a.queries = xDev + (size_t)b0 * d;
         a.nq = std::min(batch, n - b0);
-        a.rowOffset = callRow0_ + b0;
+        a.rowOffset = call.row0 + b0;
         a.outD = dDev + (size_t)b0 * k;
         a.outI = iDev + (size_t)b0 * k;
         runCagraSearch(a, stream);
@@ -2311,7 +2283,7 @@ void GpuIndexCagra::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, 
     unsigned long long hCount = 0;
     CUDA_VERIFY(cudaMemcpyAsync(&hCount, count.data, sizeof(hCount), cudaMemcpyDeviceToHost, stream));
     CUDA_VERIFY(cudaStreamSynchronize(stream));
-    if (callRow0_ == 0)
+    if (call.row0 == 0)
         lastSearchDistanceCount = 0;
     lastSearchDistanceCount += (int64_t)hCount;
 }
@@ -2688,7 +2660,9 @@ void DistributedIndexShards::searchCollective(idx_t n, const float* x, idx_t k, 
         DeviceView<float> xv(res, device, x + (size_t)i0 * d, (size_t)nb * d, stream);
         auto locD = res->temp(device, sizeof(float) * nb * k);
         auto locI = res->temp(device, sizeof(idx_t) * nb * k);
-        local_->searchShardDevice(nb, xv.ptr, (int)k, locD.as<float>(), locI.as<idx_t>(), pooled ? &ctx : nullptr);
+        SearchCall call;
+        call.row0 = i0;
+        local_->searchShardDevice(nb, xv.ptr, (int)k, locD.as<float>(), locI.as<idx_t>(), pooled ? &ctx : nullptr, call);
         auto allD = res->temp(device, sizeof(float) * (size_t)S * nb * k);
         auto allI = res->temp(device, sizeof(idx_t) * (size_t)S * nb * k);
         // ONE exchange: the per-shard [nb,k] distance and label blocks, fused into a single NCCL launch

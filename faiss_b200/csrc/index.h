@@ -73,6 +73,16 @@ struct SearchParametersIVF : SearchParameters {
     SearchParameters* quantizer_params = nullptr;
 };
 
+// What one page of a search call needs to know about the call; passed down with the page, never kept by the index.
+// A default SearchCall is a whole, unfiltered call (the device entry points: IVF coarse search, k-means).
+struct SearchCall {
+    const SearchParameters* params = nullptr; // the caller's, or null
+    const uint32_t* mask = nullptr;           // params->sel over this index's slots (idselector.h), or null
+    idx_t selected = 0;                       // slots set in mask (GpuIndexFlat's compaction choice)
+    idx_t row0 = 0;                           // row, within the whole call, of this page's first query
+    const IvfSlotOutput* slots = nullptr;     // the IVF retrieval searches: scans report the slot of every result
+};
+
 // faiss::InterruptCallback (faiss/impl/AuxIndexStructures.h): a process-wide hook polled between query pages,
 // add pages, search rounds and clustering iterations (the reference polls between tiles,
 // faiss/gpu/impl/Distance.cu:245,266,403-405); when it returns true the running call throws
@@ -121,28 +131,32 @@ class GpuIndex : public Index {
     void compute_residual_n(idx_t n, const float* xs, float* residuals, const idx_t* keys) const override;
 
    protected:
-    // the per-call parameters of the search in flight (an index instance is not re-entrant, as upstream)
-    mutable const SearchParameters* callParams_ = nullptr;
-    // the row, in the whole search call, of the first query handed to searchImpl_ (set by the query paging)
-    mutable idx_t callRow0_ = 0;
-    // callParams_->sel evaluated once per call over the index's storage slots (idselector.h), else null
-    mutable const uint32_t* callMask_ = nullptr;
-    // sel over this index's slots into a device mask of slotMaskWords(slots) words (temporary memory)
-    virtual GpuMemoryReservation selMask_(const IDSelector& sel) const = 0;
+    // sel over this index's slots into a device mask of slotMaskWords(slots) words (temporary memory); GpuIndexFlat
+    // also counts the selected slots into `selected`
+    virtual GpuMemoryReservation selMask_(const IDSelector& sel, idx_t& selected) const = 0;
     virtual bool addImplRequiresIDs_() const = 0;
     virtual void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) = 0;
-    virtual void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const = 0;
+    virtual void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const SearchCall& call) const = 0;
+    // one page of a search call: nb queries and their [nb][k] results, on the device
+    using SearchPage = std::function<void(idx_t nb, const float* xDev, float* dDev, idx_t* iDev, const SearchCall& call)>;
+    // The query paging of every search entry point: the argument checks, params->sel's mask (built once, before the
+    // first page), then `page` on each page of queries.  resultBytes > 0 also bounds a page's output, k * resultBytes
+    // bytes per query, to kRetrievalPageBytes.
+    void searchPaged_(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, const SearchParameters* params,
+                      size_t resultBytes, const SearchPage& page) const;
     // host queries above the paging threshold: pinned double buffers + async-copy stream (GpuIndex.cu:620-788)
-    bool searchFromCpuPaged_(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, idx_t maxQ) const;
+    bool searchFromCpuPaged_(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, idx_t maxQ,
+                             SearchCall call, const SearchPage& page) const;
 
    public:
     // Shard-local half of a sharded search (device pointers, ids local to this shard).  `flatShard` is
     // non-null only when EVERY rank of the communicator runs the tensor-core Flat path: the ranks then pool
     // their thresholds after every round, and a shard may return fewer than k entries (-1 padded) -- those it
     // can prove are not in the global top-k.  All ranks must make the call with identical queries and k.
-    virtual void searchShardDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* flatShard) const {
+    virtual void searchShardDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* flatShard,
+                                   const SearchCall& call) const {
         (void)flatShard;
-        searchImpl_(n, xDev, k, dDev, iDev);
+        searchImpl_(n, xDev, k, dDev, iDev, call);
     }
     // would this index take the tensor-core Flat path for (its current size, k)?  (sharded search: the
     // pooled-threshold protocol is used only if this holds on every rank)
@@ -194,8 +208,6 @@ class GpuIndexFlat : public GpuIndex {
     void reconstruct_batch(idx_t n, const idx_t* keys, float* out) const override;
     void compute_residual(const float* x, float* residual, idx_t key) const override;
     void compute_residual_n(idx_t n, const float* xs, float* residuals, const idx_t* keys) const override;
-    using GpuIndex::search;
-    void search(idx_t n, const float* x, idx_t k, float* distances, idx_t* labels) const override;
     // search, then the returned rows (fp16 storage: widened, as reconstruct)
     void search_and_reconstruct(
             idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, float* recons,
@@ -203,10 +215,10 @@ class GpuIndexFlat : public GpuIndex {
 
     // device-pointer entry points used by IVF / clustering (role of FlatIndex::query)
     void searchDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const {
-        lastSearchFallbackQueries = 0;
-        searchImpl_(n, xDev, k, dDev, iDev);
+        searchImpl_(n, xDev, k, dDev, iDev, SearchCall());
     }
-    void searchShardDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* flatShard) const override;
+    void searchShardDevice(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* flatShard,
+                           const SearchCall& call) const override;
     bool shardPoolingEligible(int k, idx_t n) const override;
     const float* vectorsDevice() const { // fp32 rows (IVF coarse centroids); not available under useFloat16
         FB_THROW_IF_NOT_MSG(!flatConfig_.useFloat16, "fp32 row access on a float16 GpuIndexFlat");
@@ -234,10 +246,11 @@ class GpuIndexFlat : public GpuIndex {
         return false;
     }
     void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) override;
-    void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const override;
-    GpuMemoryReservation selMask_(const IDSelector& sel) const override; // slot = row, id = row
-    // the selected rows only: gathered (fp32) and searched with the exact kernel, labels mapped back
-    void searchCompacted_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, idx_t selected) const;
+    // a call's first page (call.row0 == 0) resets lastSearchFallbackQueries; later pages add to it
+    void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const SearchCall& call) const override;
+    GpuMemoryReservation selMask_(const IDSelector& sel, idx_t& selected) const override; // slot = row, id = row
+    // the `selected` rows of mask only: gathered (fp32) and searched with the exact kernel, labels mapped back
+    void searchCompacted_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const uint32_t* mask, idx_t selected) const;
     void fillEmpty_(idx_t n, int k, float* dDev, idx_t* iDev) const;
     // the metric the kernels run, read at search time: METRIC_Lp with metric_arg 1 is L1 and with 2 is L2
     // (faiss/gpu/impl/Distance.cuh:223-239); only L2 and inner product can take the tensor-core path
@@ -262,7 +275,6 @@ class GpuIndexFlat : public GpuIndex {
     const float* roundedQueries_(idx_t n, const float* xDev, GpuMemoryReservation& hold) const;
 
     GpuIndexFlatConfig flatConfig_;
-    mutable idx_t callSelected_ = 0; // rows selected by callMask_ (counted once per call, in selMask_)
     DeviceVector<float> vecs_;    // fp32 storage (default)
     DeviceVector<__half> vecs16_; // fp16 storage (useFloat16): the only copy of the vectors besides the scoring tiles
     mutable FlatTcDatabase tc_; // rebuilt lazily after the rows change
@@ -515,10 +527,9 @@ class GpuIndexIVF : public GpuIndex {
     void searchWithSlots_(
             idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, const SearchParameters* params,
             size_t resultBytes, const std::function<void(idx_t, idx_t, const idx_t*)>& page) const;
-    // set while searchWithSlots_ runs: scanImpl_ hands the scans callSlots_->identity instead of the list ids
-    mutable const IvfSlotOutput* callSlots_ = nullptr;
-    const idx_t* scanIds_() const {
-        return callSlots_ ? callSlots_->identity : lists_->ids();
+    // the id table the scans read: the slot search's identity table, else the list ids
+    const idx_t* scanIds_(const SearchCall& call) const {
+        return call.slots ? call.slots->identity : lists_->ids();
     }
 
     bool addImplRequiresIDs_() const override {
@@ -539,8 +550,8 @@ class GpuIndexIVF : public GpuIndex {
     // x - (its coarse centroid).  In add, assignDev is the rows' assignment and the buffer comes from the temp stack;
     // in training assignDev is null, the k = 1 assignment runs here, and the buffers are device allocations.
     GpuMemoryReservation coarseResiduals_(idx_t n, const float* xDev, const idx_t* assignDev) const;
-    void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const override;
-    GpuMemoryReservation selMask_(const IDSelector& sel) const override; // slot = arena position, id = stored id
+    void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const SearchCall& call) const override;
+    GpuMemoryReservation selMask_(const IDSelector& sel, idx_t& selected) const override; // slot = arena position, id = stored id
     virtual void scanImpl_(
             idx_t n,
             const float* xDev,
@@ -549,7 +560,8 @@ class GpuIndexIVF : public GpuIndex {
             int nprobe,
             int k,
             float* dDev,
-            idx_t* iDev) const = 0;
+            idx_t* iDev,
+            const SearchCall& call) const = 0;
 
     GpuIndexIVFConfig ivfConfig_;
     std::unique_ptr<IvfLists> lists_;
@@ -574,7 +586,7 @@ class GpuIndexIVFFlat : public GpuIndexIVF {
 
    protected:
     const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
-    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
+    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*, const SearchCall&) const override;
     IvfStoredLayout storedLayout_() const override;
 };
 
@@ -645,7 +657,7 @@ class GpuIndexIVFPQ : public GpuIndexIVF {
     }
     void trainEncoder_(idx_t n, const float* xDev) override; // the PQ, on residuals
     const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
-    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
+    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*, const SearchCall&) const override;
     IvfStoredLayout storedLayout_() const override;
 
     int M_, nbits_;
@@ -718,7 +730,7 @@ class GpuIndexIVFScalarQuantizer : public GpuIndexIVF {
     }
     void trainEncoder_(idx_t n, const float* xDev) override; // the RS_minmax ranges
     const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
-    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*) const override;
+    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*, const SearchCall&) const override;
     IvfStoredLayout storedLayout_() const override;
 
     int qtype_;
@@ -811,8 +823,9 @@ class GpuIndexCagra : public GpuIndex {
         return false;
     }
     void addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) override;
-    void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev) const override;
-    GpuMemoryReservation selMask_(const IDSelector& sel) const override; // throws: no filtered graph search
+    // a call's first page (call.row0 == 0) resets lastSearchDistanceCount; later pages add to it
+    void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const SearchCall& call) const override;
+    GpuMemoryReservation selMask_(const IDSelector& sel, idx_t& selected) const override; // throws: no filtered graph search
 
     GpuIndexCagraConfig cagraConfig_;
     int graphDegree_ = 0;

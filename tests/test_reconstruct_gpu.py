@@ -223,6 +223,19 @@ def test_torch_and_paged_host_queries(res):
     idx.setMinPagingSize(0)
     D, I, R = idx.search_and_reconstruct(xq, K)
     assert np.array_equal(D, D0) and np.array_equal(I, I0) and np.array_equal(R, R0)
+    # a pinned buffer of two 64-query halves: five pages through the pinned pipeline, with a selector
+    r2 = fb.StandardGpuResources()
+    r2.setPinnedMemory(2 * 64 * d * 4)
+    idx2 = _build(r2, rn.PQ, {"M": 16, "nbits": 8}, n=4000)[0]
+    params = fb.SearchParametersIVF(nprobe=4, sel=fb.IDSelectorRange(1000, 3000))
+    D0, I0, R0 = idx2.search_and_reconstruct(xq, K, params=params)
+    _, _, C0 = idx2.search_and_return_codes(xq, K, include_listnos=True, params=params)
+    assert np.all((I0 >= 1000) & (I0 < 3000))
+    idx2.setMinPagingSize(0)
+    D, I, R = idx2.search_and_reconstruct(xq, K, params=params)
+    assert np.array_equal(_bits(D), _bits(D0)) and np.array_equal(I, I0) and np.array_equal(_bits(R), _bits(R0))
+    D, I, C = idx2.search_and_return_codes(xq, K, include_listnos=True, params=params)
+    assert np.array_equal(_bits(D), _bits(D0)) and np.array_equal(I, I0) and np.array_equal(C, C0)
 
 
 @pytest.mark.parametrize("use_float16", [False, True])
