@@ -305,18 +305,28 @@ int64_t runCountMask(GpuResources* res, int device, const uint32_t* maskDev, int
     return h;
 }
 
+// DeviceSelect counts items in int: rows are compacted a page of at most 2^30 at a time, each page's selected
+// rows written after the previous page's
 int64_t runCompactMask(GpuResources* res, int device, const uint32_t* maskDev, int64_t n, idx_t* rowsOut, cudaStream_t stream) {
-    FB_THROW_IF_NOT(n < (int64_t(1) << 31));
+    constexpr int64_t kPage = int64_t(1) << 30;
     auto count = res->temp(device, sizeof(int));
     size_t tmpBytes = 0;
-    cub::CountingInputIterator<idx_t> rows(0);
-    CUDA_VERIFY(cub::DeviceSelect::If(nullptr, tmpBytes, rows, rowsOut, count.as<int>(), (int)n, MaskBit{maskDev}, stream));
+    CUDA_VERIFY(cub::DeviceSelect::If(
+            nullptr, tmpBytes, cub::CountingInputIterator<idx_t>(0), rowsOut, count.as<int>(), (int)std::min(n, kPage),
+            MaskBit{maskDev}, stream));
     auto tmp = res->temp(device, tmpBytes);
-    CUDA_VERIFY(cub::DeviceSelect::If(tmp.data, tmpBytes, rows, rowsOut, count.as<int>(), (int)n, MaskBit{maskDev}, stream));
-    int h = 0;
-    CUDA_VERIFY(cudaMemcpyAsync(&h, count.data, sizeof(int), cudaMemcpyDeviceToHost, stream));
-    CUDA_VERIFY(cudaStreamSynchronize(stream));
-    return h;
+    int64_t total = 0;
+    for (int64_t r0 = 0; r0 < n; r0 += kPage) {
+        const int np = (int)std::min(kPage, n - r0);
+        CUDA_VERIFY(cub::DeviceSelect::If(
+                tmp.data, tmpBytes, cub::CountingInputIterator<idx_t>(r0), rowsOut + total, count.as<int>(), np,
+                MaskBit{maskDev}, stream));
+        int h = 0;
+        CUDA_VERIFY(cudaMemcpyAsync(&h, count.data, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        CUDA_VERIFY(cudaStreamSynchronize(stream));
+        total += h;
+    }
+    return total;
 }
 
 void runRemapLabels(idx_t* labels, int64_t count, const idx_t* ids, cudaStream_t stream) {

@@ -69,7 +69,8 @@ void buildSlotMask(
 // number of set bits among the first n of a mask (synchronises with the host)
 int64_t runCountMask(GpuResources* res, int device, const uint32_t* maskDev, int64_t n, cudaStream_t stream);
 
-// row mask -> ascending list of the selected rows (device), returns their count.  rowsOut [n] (device).
+// row mask -> ascending list of the selected rows (device), returns their count.  rowsOut (device) holds at
+// least as many entries as the mask has set bits among its first n.
 int64_t runCompactMask(GpuResources* res, int device, const uint32_t* maskDev, int64_t n, idx_t* rowsOut, cudaStream_t stream);
 
 // labels of a search over the compacted rows -> row ids (ids[label], -1 stays -1), in place

@@ -552,7 +552,7 @@ constexpr idx_t kCompactRatio = 40;
 void GpuIndexFlat::searchCompacted_(
         idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const uint32_t* mask, idx_t selected) const {
     auto stream = stream_();
-    auto rows = resources_->temp(config_.device, sizeof(idx_t) * this->ntotal);
+    auto rows = resources_->temp(config_.device, sizeof(idx_t) * selected); // selected: the mask's count of its rows
     runCompactMask(resources_.get(), config_.device, mask, this->ntotal, rows.as<idx_t>(), stream);
     auto sub = resources_->temp(config_.device, sizeof(float) * selected * d);
     runGatherRows(rows_(), rows.as<idx_t>(), selected, d, sub.as<float>(), stream, yHalf_()); // fp16 widens exactly

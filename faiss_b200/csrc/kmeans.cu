@@ -12,69 +12,6 @@
 
 namespace fb200 {
 
-__global__ void kmeans_accum_smem_kernel(
-        const float* __restrict__ x,
-        const idx_t* __restrict__ assign,
-        int64_t n,
-        int d,
-        int k,
-        int64_t pointsPerBlock,
-        float* __restrict__ sums,
-        float* __restrict__ counts) {
-    extern __shared__ float sm[]; // [k*d] sums + [k] counts
-    float* ssum = sm;
-    float* scnt = sm + (size_t)k * d;
-    for (int i = threadIdx.x; i < k * d + k; i += blockDim.x)
-        sm[i] = 0.f;
-    __syncthreads();
-    const int64_t p0 = (int64_t)blockIdx.x * pointsPerBlock;
-    const int64_t p1 = min(n, p0 + pointsPerBlock);
-    // flat element loop: element e of the slice = (point, dim)
-    for (int64_t e = p0 * d + threadIdx.x; e < p1 * d; e += blockDim.x) {
-        int64_t pt = e / d;
-        int j = (int)(e - pt * d);
-        idx_t c = assign[pt];
-        if (c >= 0 && c < k) {
-            atomicAdd(&ssum[c * d + j], x[e]);
-            if (j == 0)
-                atomicAdd(&scnt[c], 1.f);
-        }
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < k * d; i += blockDim.x) {
-        float v = ssum[i];
-        if (v != 0.f)
-            atomicAdd(&sums[i], v);
-    }
-    for (int i = threadIdx.x; i < k; i += blockDim.x) {
-        float v = scnt[i];
-        if (v != 0.f)
-            atomicAdd(&counts[i], v);
-    }
-}
-
-__global__ void kmeans_accum_global_kernel(
-        const float* __restrict__ x,
-        const idx_t* __restrict__ assign,
-        int64_t n,
-        int d,
-        int64_t k,
-        float* __restrict__ sums,
-        float* __restrict__ counts) {
-    const int64_t pt = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (pt >= n)
-        return;
-    const idx_t c = assign[pt];
-    if (c < 0 || c >= k)
-        return;
-    const float* xp = x + pt * d;
-    float* sp = sums + c * d;
-    for (int j = lane_id(); j < d; j += 32)
-        atomicAdd(&sp[j], xp[j]);
-    if (lane_id() == 0)
-        atomicAdd(&counts[c], 1.f);
-}
-
 // ---- deterministic update: sort the points by assignment, then one warp per centroid adds its points in
 // index order (no atomics: the sums are bit-reproducible run to run, like the reference's CPU
 // compute_centroids, faiss/impl/ClusteringHelpers.cpp:101-172; SURVEY 7 step 5)
@@ -169,9 +106,12 @@ __global__ void kmeans_segment_sum_kernel(
         counts[c] += (float)(e - lo);
 }
 
-static void runKmeansAccumulateSorted(
+void runKmeansAccumulate(
         const float* x, const idx_t* assign, int64_t n, int d, int64_t k, float* sums, float* counts, cudaStream_t stream) {
-    FB_THROW_IF_NOT_MSG(n < (int64_t(1) << 32) - 1 && k < (int64_t(1) << 32) - 1, "k-means update: too many points / centroids");
+    if (n == 0)
+        return;
+    // the radix sort counts items in int; the keys and row numbers are 32-bit
+    FB_THROW_IF_NOT_MSG(n < (int64_t(1) << 31) && k < (int64_t(1) << 32) - 1, "k-means update: too many points / centroids");
     unsigned *keysIn = nullptr, *keysOut = nullptr, *valsIn = nullptr, *valsOut = nullptr;
     void* tmp = nullptr;
     CUDA_VERIFY(cudaMallocAsync(&keysIn, sizeof(unsigned) * n * 4, stream));
@@ -192,39 +132,6 @@ static void runKmeansAccumulateSorted(
     CUDA_CHECK_LAST();
     CUDA_VERIFY(cudaFreeAsync(tmp, stream));
     CUDA_VERIFY(cudaFreeAsync(keysIn, stream));
-}
-
-void runKmeansAccumulate(
-        const float* x,
-        const idx_t* assign,
-        int64_t n,
-        int d,
-        int64_t k,
-        float* sums,
-        float* counts,
-        cudaStream_t stream) {
-    if (n == 0)
-        return;
-    if (n < (int64_t(1) << 31)) {
-        runKmeansAccumulateSorted(x, assign, n, d, k, sums, counts, stream);
-        return;
-    }
-    // n >= 2^31 exceeds the radix sort's int item count: atomic accumulation, not order-deterministic.
-    // Codebooks whose k*d floats fit in shared memory (e.g. the 256 x dsub PQ codebooks) are accumulated
-    // per block with shared atomics and flushed once; larger ones take one warp per point with global RED.
-    size_t smem = sizeof(float) * ((size_t)k * d + k);
-    if (smem <= 64 * 1024) {
-        int64_t ppb = std::max<int64_t>(256, ceil_div(n, 132 * 4));
-        CUDA_VERIFY(cudaFuncSetAttribute(
-                kmeans_accum_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kmeans_accum_smem_kernel<<<(unsigned)ceil_div(n, ppb), 256, smem, stream>>>(
-                x, assign, n, d, (int)k, ppb, sums, counts);
-    } else {
-        int warps = 8;
-        kmeans_accum_global_kernel<<<(unsigned)ceil_div(n, warps), warps * 32, 0, stream>>>(
-                x, assign, n, d, k, sums, counts);
-    }
-    CUDA_CHECK_LAST();
 }
 
 __global__ void kmeans_finalize_kernel(
