@@ -78,9 +78,8 @@ struct ExactCfg {
 //                packed atomicMin keep "smaller key is better"
 //   kPadNeutral  a zero-filled component (q = y = 0) leaves the state unchanged; the others stop the last
 //                16-component chunk at d instead
-//   kSentinel    a distance that is NaN or not strictly better than the missing-result sentinel (FLT_MAX,
-//                -FLT_MAX for a similarity) is never kept: the CPU heap inserts only when C::cmp(top, d)
-//                holds against its neutral element.  L2 / IP keep their original filter (NaN only).
+// Every op's keys go through isResult (select.cuh): a distance that is NaN or not strictly better than the
+// missing-result sentinel (FLT_MAX, -FLT_MAX for a similarity) is never kept.
 // ------------------------------------------------------------------------------------------
 struct Acc1 {
     float s;
@@ -90,7 +89,7 @@ struct Acc2 {
 };
 
 struct OpL2 {
-    static constexpr bool kSimilarity = false, kPadNeutral = true, kSentinel = false;
+    static constexpr bool kSimilarity = false, kPadNeutral = true;
     using Acc = Acc1;
     __device__ static void init(Acc& a) { a.s = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float) {
@@ -100,21 +99,21 @@ struct OpL2 {
     __device__ static float finish(const Acc& a, float) { return a.s; }
 };
 struct OpIP {
-    static constexpr bool kSimilarity = true, kPadNeutral = true, kSentinel = false;
+    static constexpr bool kSimilarity = true, kPadNeutral = true;
     using Acc = Acc1;
     __device__ static void init(Acc& a) { a.s = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float) { a.s = fmaf(q, y, a.s); }
     __device__ static float finish(const Acc& a, float) { return a.s; }
 };
 struct OpL1 {
-    static constexpr bool kSimilarity = false, kPadNeutral = true, kSentinel = true;
+    static constexpr bool kSimilarity = false, kPadNeutral = true;
     using Acc = Acc1;
     __device__ static void init(Acc& a) { a.s = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float) { a.s = a.s + fabsf(q - y); }
     __device__ static float finish(const Acc& a, float) { return a.s; }
 };
 struct OpLinf {
-    static constexpr bool kSimilarity = false, kPadNeutral = true, kSentinel = true;
+    static constexpr bool kSimilarity = false, kPadNeutral = true;
     using Acc = Acc1;
     __device__ static void init(Acc& a) { a.s = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float) { a.s = fmaxf(a.s, fabsf(q - y)); }
@@ -122,7 +121,7 @@ struct OpLinf {
 };
 // powf(0, p) is 0 only for p > 0: padding is bounded for every p
 struct OpLp {
-    static constexpr bool kSimilarity = false, kPadNeutral = false, kSentinel = true;
+    static constexpr bool kSimilarity = false, kPadNeutral = false;
     using Acc = Acc1;
     __device__ static void init(Acc& a) { a.s = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float p) { a.s = __fadd_rn(a.s, powf(fabsf(q - y), p)); }
@@ -130,7 +129,7 @@ struct OpLp {
 };
 // a = b = 0 is 0/0 = NaN, as on the CPU: such rows are excluded, and padding must not produce it
 struct OpCanberra {
-    static constexpr bool kSimilarity = false, kPadNeutral = false, kSentinel = true;
+    static constexpr bool kSimilarity = false, kPadNeutral = false;
     using Acc = Acc1;
     __device__ static void init(Acc& a) { a.s = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float) {
@@ -139,7 +138,7 @@ struct OpCanberra {
     __device__ static float finish(const Acc& a, float) { return a.s; }
 };
 struct OpBrayCurtis {
-    static constexpr bool kSimilarity = false, kPadNeutral = true, kSentinel = true;
+    static constexpr bool kSimilarity = false, kPadNeutral = true;
     using Acc = Acc2;
     __device__ static void init(Acc& a) { a.a = a.b = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float) {
@@ -150,7 +149,7 @@ struct OpBrayCurtis {
 };
 // 0.5 * sum(-a log(m/a) - b log(m/b)), m = (a+b)/2; a zero component gives NaN, as on the CPU
 struct OpJensenShannon {
-    static constexpr bool kSimilarity = false, kPadNeutral = false, kSentinel = true;
+    static constexpr bool kSimilarity = false, kPadNeutral = false;
     using Acc = Acc1;
     __device__ static void init(Acc& a) { a.s = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float) {
@@ -162,7 +161,7 @@ struct OpJensenShannon {
     __device__ static float finish(const Acc& a, float) { return __fmul_rn(0.5f, a.s); }
 };
 struct OpJaccard {
-    static constexpr bool kSimilarity = true, kPadNeutral = true, kSentinel = true;
+    static constexpr bool kSimilarity = true, kPadNeutral = true;
     using Acc = Acc2;
     __device__ static void init(Acc& a) { a.a = a.b = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float) {
@@ -175,7 +174,7 @@ struct OpJaccard {
 // numeric value against a categorical one) and survives every later add.  Padding would count as a valid
 // numeric dimension.
 struct OpGower {
-    static constexpr bool kSimilarity = false, kPadNeutral = false, kSentinel = true;
+    static constexpr bool kSimilarity = false, kPadNeutral = false;
     using Acc = Acc2;
     __device__ static void init(Acc& a) { a.a = a.b = 0.f; }
     __device__ static void update(Acc& a, float q, float y, float) {
@@ -398,7 +397,7 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
                         if (row < r1 && (!MASK || ((rowMask[row >> 5] >> (row & 31)) & 1u))) {
                             const float dist = Op::finish(acc[r][c], arg);
                             float key = Op::kSimilarity ? -dist : dist;
-                            if (key == key && (!Op::kSentinel || key < FLT_MAX)) { // NaN never wins
+                            if (isResult(key)) {
                                 unsigned long long p =
                                         ((unsigned long long)float_to_ordered(key) << 32) | (unsigned)(row - r0);
                                 mine = min(mine, p);
@@ -415,7 +414,7 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
                         int64_t row = nb + tx * 4 + c;
                         const float dist = Op::finish(acc[r][c], arg);
                         float key = Op::kSimilarity ? -dist : dist;
-                        if (row < r1 && key <= thr && (!Op::kSentinel || key < FLT_MAX) &&
+                        if (row < r1 && key <= thr && isResult(key) &&
                             (!MASK || ((rowMask[row >> 5] >> (row & 31)) & 1u))) {
                             int pos = atomicAdd(&cntS[q], 1);
                             s.keys[LIST + pos] = key;
@@ -468,7 +467,7 @@ __global__ void __launch_bounds__(256) flat_exact_kernel(
             int64_t o = ((int64_t)(q0 + q) * nsplit + split) * k;
             for (int j = lane_id(); j < k; j += 32) {
                 int id = s.ids[j];
-                bool ok = id != IdLimits<int>::max();
+                bool ok = isResult(s.keys[j]);
                 partD[o + j] = s.keys[j];
                 partI[o + j] = ok ? r0 + id : -1;
             }
@@ -509,6 +508,7 @@ __global__ void merge_topk_kernel(
     const int64_t total = (int64_t)nlists * kin;
     const float* D = inD + row * rowStride;
     const idx_t* I = inI + row * rowStride;
+    int64_t entered = 0; // entries offered to the list: the first min(entered, k) slots hold results
     for (int64_t e0 = 0; e0 < total; e0 += 32) {
         int64_t e = e0 + lane;
         bool valid = e < total;
@@ -519,25 +519,45 @@ __global__ void merge_topk_kernel(
             const int64_t at = l * listStride + (e - l * kin);
             id = I[at];
             key = D[at];
-            if (id == -1) { // the "no result" marker; any other id is a stored one (IVF ids may be negative)
-                valid = false;
+            if (IN_KEYSPACE) {
+                // partial results of one search: the result rule decides, so any stored id (-1, INT64_MAX) passes
+                valid = isResult(key);
             } else {
-                if (idOffsets)
-                    id += idOffsets[l];
-                if (!IN_KEYSPACE && !lowerIsBetter)
+                // per-shard results: -1 is the "no result" marker; any other id is a stored one (IVF ids may be
+                // negative).  The distances are the shards' own and are not filtered again.
+                valid = id != -1;
+                if (!lowerIsBetter)
                     key = -key;
+                valid = valid && key == key;
             }
+            if (valid && idOffsets)
+                id += idOffsets[l];
         }
+        entered += __popc(__ballot_sync(kFullMask, valid));
         w.add(valid, key, id);
     }
     w.finish();
-    for (int j = lane; j < k; j += 32) {
-        long long id = w.q.ids[j];
-        bool ok = id != IdLimits<long long>::max();
-        float key = w.q.keys[j];
-        float dis = lowerIsBetter ? key : -key;
-        outD[row * k + j] = ok ? dis : (lowerIsBetter ? FLT_MAX : -FLT_MAX); // faiss/gpu/impl/Distance.cu:152-164
-        outI[row * k + j] = ok ? (idx_t)id + idBase : -1;
+    // Partial results of one search: a stored id of -1 takes its rank in the selection and is then dropped, the
+    // results behind it moving up, as the CPU heap_reorder treats id -1 as an empty slot (faiss/utils/Heap.h:427-456).
+    // Any other id is returned.  Per-shard inputs never enter a -1, so every entry in the list is kept.
+    int kept = 0;
+    for (int j0 = 0; j0 < k; j0 += 32) {
+        const int j = j0 + lane;
+        const bool inList = j < k && j < entered;
+        const long long id = inList ? w.q.ids[j] + idBase : -1;
+        const bool keep = inList && (!IN_KEYSPACE || id != -1);
+        const unsigned m = __ballot_sync(kFullMask, keep);
+        if (keep) {
+            const int o = kept + __popc(m & ((1u << lane) - 1u));
+            const float key = w.q.keys[j];
+            outD[row * k + o] = lowerIsBetter ? key : -key;
+            outI[row * k + o] = (idx_t)id;
+        }
+        kept += __popc(m);
+    }
+    for (int j = kept + lane; j < k; j += 32) {
+        outD[row * k + j] = lowerIsBetter ? FLT_MAX : -FLT_MAX; // faiss/gpu/impl/Distance.cu:152-164
+        outI[row * k + j] = -1;
     }
 }
 

@@ -791,13 +791,13 @@ __global__ void tc_rerank_kernel(
         // sentinels ends the walk.
         if (!__any_sync(kFullMask, present))
             break;
-        w.add(valid, acc, id);
+        w.add(valid && isResult(acc), acc, id);
     }
     w.finish();
     for (int j = lane; j < k; j += 32) {
         int id = w.q.ids[j];
-        bool ok = id != IdLimits<int>::max();
         float key = w.q.keys[j];
+        bool ok = isResult(key);
         outD[(int64_t)q * k + j] = ok ? (IS_L2 ? key : -key) : (IS_L2 ? FLT_MAX : -FLT_MAX);
         outI[(int64_t)q * k + j] = ok ? (idx_t)id : -1;
     }
@@ -888,7 +888,7 @@ __global__ void tc_argmin_finish_kernel(
                 }
                 if (!IS_L2)
                     acc = -acc;
-                if (acc < bestD || (acc == bestD && id < bestI)) {
+                if (isResult(acc) && (acc < bestD || (acc == bestD && id < bestI))) {
                     bestD = acc;
                     bestI = id;
                 }
@@ -905,7 +905,7 @@ __global__ void tc_argmin_finish_kernel(
         }
     }
     if (lane == 0) {
-        const bool ok = bestI != IdLimits<int>::max();
+        const bool ok = isResult(bestD);
         outD[q] = ok ? (IS_L2 ? bestD : -bestD) : (IS_L2 ? FLT_MAX : -FLT_MAX);
         outI[q] = ok ? (idx_t)bestI : -1;
         if (overflow || !ok)

@@ -1381,7 +1381,8 @@ void GpuIndexIVF::addImpl_(idx_t n, const float* xDev, const idx_t* idsDev) {
     GpuMemoryReservation hold;
     const uint8_t* rows = encode_(n, xDev, assign.as<idx_t>(), hold);
     lists_->append(n, rows, idsDev, assign.as<idx_t>(), stream);
-    // vectors that could not be assigned (NaN) are still counted, as upstream (IVFBase.cu addVectors)
+    // vectors the coarse search could not assign (no centroid distance is a result: NaN, inf or overflow) are not
+    // stored but still counted, as upstream (IVFBase.cu addVectors)
     this->ntotal += n;
 }
 

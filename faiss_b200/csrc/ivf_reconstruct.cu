@@ -24,9 +24,6 @@ struct IdSlot {
 __device__ __forceinline__ bool operator<(const IdSlot& a, const IdSlot& b) {
     return a.id < b.id || (a.id == b.id && a.slot < b.slot);
 }
-__device__ __forceinline__ bool operator!=(const IdSlot& a, const IdSlot& b) {
-    return a.id != b.id || a.slot != b.slot;
-}
 template <>
 struct IdLimits<IdSlot> {
     static __host__ __device__ constexpr IdSlot max() {
@@ -228,19 +225,32 @@ __global__ void merge_topk_slots_kernel(
         if (valid) {
             is.slot = P[e];
             key = D[e];
-            is.id = is.slot == -1 ? -1 : arenaIds[is.slot];
-            valid = is.id != -1; // the plain merge's "no result" marker
+            valid = isResult(key); // the plain merge's rule: any stored id passes
+            is.id = valid ? arenaIds[is.slot] : -1;
         }
         w.add(valid, key, is);
     }
     w.finish();
-    for (int j = lane; j < k; j += 32) {
-        const IdSlot is = w.q.ids[j];
-        const bool ok = is != IdLimits<IdSlot>::max();
-        const float key = w.q.keys[j];
-        outD[row * k + j] = ok ? (lowerIsBetter ? key : -key) : (lowerIsBetter ? FLT_MAX : -FLT_MAX);
-        outI[row * k + j] = ok ? (idx_t)is.id : -1;
-        outSlot[row * k + j] = ok ? (idx_t)is.slot : -1;
+    // as the plain merge: a stored id of -1 keeps its rank in the selection and is then dropped (CPU heap_reorder)
+    int kept = 0;
+    for (int j0 = 0; j0 < k; j0 += 32) {
+        const int j = j0 + lane;
+        const IdSlot is = j < k ? w.q.ids[j] : IdSlot{-1, -1};
+        const float key = j < k ? w.q.keys[j] : CUDART_INF_F;
+        const bool keep = isResult(key) && is.id != -1;
+        const unsigned m = __ballot_sync(kFullMask, keep);
+        if (keep) {
+            const int o = kept + __popc(m & ((1u << lane) - 1u));
+            outD[row * k + o] = lowerIsBetter ? key : -key;
+            outI[row * k + o] = (idx_t)is.id;
+            outSlot[row * k + o] = (idx_t)is.slot;
+        }
+        kept += __popc(m);
+    }
+    for (int j = kept + lane; j < k; j += 32) {
+        outD[row * k + j] = lowerIsBetter ? FLT_MAX : -FLT_MAX;
+        outI[row * k + j] = -1;
+        outSlot[row * k + j] = -1;
     }
 }
 

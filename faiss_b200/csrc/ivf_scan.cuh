@@ -102,10 +102,13 @@ __device__ void block_merge_and_write(
             }
         }
         w.finish();
+        // list ids are arena positions, so the sentinel id marks an empty slot; the result rule applies to the final
+        // key (a constant shift per CTA keeps every entry it drops behind the ones it keeps)
         for (int j = lane_id(); j < k; j += 32) {
             IdT id = w.q.ids[j];
-            bool ok2 = id != IdLimits<IdT>::max();
-            outD[j] = ok2 ? w.q.keys[j] + addToKey : CUDART_INF_F;
+            const float key = w.q.keys[j] + addToKey;
+            bool ok2 = id != IdLimits<IdT>::max() && isResult(key);
+            outD[j] = ok2 ? key : CUDART_INF_F;
             outI[j] = ok2 ? (ids ? ids[id] : (idx_t)id) : -1;
         }
     }

@@ -431,7 +431,7 @@ __global__ void __launch_bounds__(kIlvScanWarps * 32, kScanMinCtas) ivfpq_scan_i
     // the CTA's list -> partial result; list ids are arena positions, user labels only for the k survivors
     for (int j = threadIdx.x; j < k; j += kThreads) {
         const IdT id = top.q.ids[j];
-        const bool ok = id != IdLimits<IdT>::max();
+        const bool ok = id != IdLimits<IdT>::max() && isResult(top.q.keys[j]);
         oD[j] = ok ? top.q.keys[j] : CUDART_INF_F;
         oI[j] = ok ? arenaIds[id] : -1;
     }

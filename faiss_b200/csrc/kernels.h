@@ -88,7 +88,8 @@ inline MetricType flatKernelMetric(MetricType metric, float metricArg) {
 
 // Row-wise top-k over candidate lists (role of runBlockSelectPair / merge_knn_results,
 // faiss/gpu/utils/BlockSelectFloat.cu:98, faiss/utils/Heap.cpp:166-238).
-//   inD/inI: [rows, nlists, kin]; ids == -1 are skipped; idOffsets (optional, [nlists]) is added to
+//   inD/inI: [rows, nlists, kin]; ids == -1 are skipped (any other id, negative ones included, is a stored one);
+//   idOffsets (optional, [nlists]) is added to
 //   ids of list l (IndexShards successive_ids translation, faiss/IndexShards.cpp:214-220).
 //   Keys are user-facing distances (larger is better for is_similarity_metric: IP, Jaccard).
 void runMergeTopK(
@@ -120,7 +121,8 @@ void runMergeTopKListMajor(
         cudaStream_t stream);
 
 // runMergeTopK over inputs already in key space (smaller is better: IP distances negated), without id offsets;
-// idBase is added to every id.  Merges the per-CTA partial results of the Flat and IVF scans.
+// idBase is added to every id.  Merges the per-CTA partial results of the Flat and IVF scans: an entry is kept by the
+// result rule on its key (isResult, select.cuh), whatever its id, so stored ids of -1 or INT64_MAX survive.
 void runMergeTopKKeyspace(
         const float* inD,
         const idx_t* inI,

@@ -17,6 +17,7 @@
 #include <cuda_runtime.h>
 #include <math_constants.h>
 
+#include <cfloat>
 #include <cstdint>
 
 namespace fb200 {
@@ -37,6 +38,15 @@ struct IdLimits<long long> {
         return 0x7fffffffffffffffLL;
     }
 };
+
+// The reference's result rule, in key space: an entry is a result only if its key is strictly better than the
+// missing-result sentinel FLT_MAX (faiss/impl/ResultHandler.h:275-282 against the heap's neutral element,
+// faiss/utils/ordered_key_value.h).  That is dis < FLT_MAX for L2 and the other distances, dis > -FLT_MAX for a
+// similarity; NaN never qualifies.  Every list and merge also recognises an empty slot by its key (they start at
+// +inf), never by the id it holds, so any stored id survives.
+__device__ __forceinline__ bool isResult(float key) {
+    return key < FLT_MAX;
+}
 
 template <typename IdT>
 __device__ __forceinline__ bool kv_less(float ka, IdT ia, float kb, IdT ib) {
