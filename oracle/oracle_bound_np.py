@@ -40,6 +40,19 @@ bounds below depend on how many roundings a term meets, never on the order of th
              vmin_i + vdiff_i (c_i + 1/2) / s that moves the component by at most
              u|r_i| + u(|vmin_i| + |vdiff_i|) + (c_i + 1/2) u |vdiff_i| / s + u |a_i| (first order), which
              e_i = 4 u (|r_i| + |vmin_i| + |vdiff_i|) covers with room for the second-order terms.
+  IVF-SQ IP  with the same m_i, b_i the kernel forms w_i = fl(q_i b_i), K = sum_i q_i m_i (an fma chain per
+             thread over d / 128 components, a 32-lane butterfly, then a sequential sum over 4 warps),
+             acc = fma chain sum_i w_i c_i (or per-lane chains and a transposing butterfly) and the value
+             acc + (K + cd), cd the coarse distance <q|c_list> handed in rounded to fp32 (0 without a
+             residual).  Truth: t = <q|c_list> + sum_i q_i X_i with X the exact decode.  The decode moves
+             component i by |m_i + b_i c_i - X_i| <= u (|X_i - vmin_i| + |vmin_i| + |vdiff_i| / 2s) to first
+             order (taken twice, for the second-order terms).  The terms q_i b_i c_i meet at most d + 2
+             roundings (w, the chain, the last add), the terms q_i m_i at most ceil(d / 128) + 10 (chain,
+             butterfly, warps, two adds) and cd 3, so with |b_i c_i| <= |X_i - vmin_i| (1 + u) and
+             |m_i| <= (|vmin_i| + |vdiff_i| / 2s)(1 + u)^2, absorbed into two more roundings each,
+               |err| <= sum_i |q_i| e_i + gamma(d + 4) sum_i |q_i (X_i - vmin_i)|
+                        + gamma(ceil(d / 128) + 12) (sum_i |q_i| (|vmin_i| + |vdiff_i| / 2s) + |<q|c_list>|).
+             fp16 / 8bit_direct: vmin = vdiff = 0, m = 0, b = 1: only the chain's terms remain.
 
 The float64 truth itself carries a rounding error; callers add slack() of the magnitudes involved, far
 below every fp32 bound (d 2^-53 against d 2^-24).
@@ -155,6 +168,25 @@ def sq_l2_truth(r, X, vmin, vdiff):
     return t, perturbed_l2_bound(tc, e, r.shape[0] + 3) + slack(t, r.shape[0])
 
 
+def sq_ip_truth(q, X, vmin, vdiff, s, qc=0.0):
+    """IVF-SQ inner product.  q: [d] query, X: [n, d] the float64 EXACT decode vmin + vdiff (c + 1/2) / s of the
+    stored codes (fp16 / 8bit_direct: the stored value, vmin = vdiff = 0, s = 1), qc: the float64 coarse term
+    <q|c_list> when the index stores residuals, else 0.  Returns (t, beta) with t = qc + <q|X_i>."""
+    q = np.asarray(q, dtype=np.float64)
+    X = np.asarray(X, dtype=np.float64)
+    vmin = np.asarray(vmin, dtype=np.float64)
+    vdiff = np.asarray(vdiff, dtype=np.float64)
+    d = q.shape[0]
+    aq = np.abs(q)
+    t = float(qc) + X @ q
+    rel = np.abs(X - vmin[None, :])  # |vdiff (c + 1/2) / s|
+    mabs = np.abs(vmin) + np.abs(vdiff) / (2.0 * s)
+    dec = 2.0 * U * ((rel + mabs[None, :]) @ aq)
+    chain = gamma(d + 4) * (rel @ aq)
+    head = gamma(-(-d // 128) + 12) * (float(mabs @ aq) + abs(float(qc)))
+    return t, dec + chain + head + slack(np.abs(X) @ aq + abs(float(qc)), d)
+
+
 # ------------------------------------------------------------------ the checker
 class CertificateError(AssertionError):
     pass
@@ -196,7 +228,7 @@ def check_topk(D, I, cand_ids, t, beta, k, metric, what=""):
     sc = cand_ids[order]
     pos = np.searchsorted(sc, Iv)
     pos = np.minimum(pos, n - 1) if n else pos
-    if n == 0 or np.any(sc[pos] != Iv):
+    if nv and (n == 0 or np.any(sc[pos] != Iv)):  # an empty candidate set returns nothing but padding
         bad = Iv if n == 0 else Iv[sc[pos] != Iv]
         _fail(what, "ids not in the candidate set: %s" % bad[:5])
     pos = order[pos]

@@ -299,3 +299,13 @@ def test_rejects_padding_before_a_valid_entry():
     D[7] = f32(0)
     with pytest.raises(ob.CertificateError, match="padding"):
         ob.check_topk(D, I, ids[:4], t[:4], beta[:4], 10, L2)
+
+
+@pytest.mark.parametrize("metric", [L2, IP])
+def test_empty_candidate_set(metric):
+    """a probe set with no vectors (empty lists, -1 probes): only padding is valid"""
+    sentinel = ob.FLT_MAX if metric == L2 else -ob.FLT_MAX
+    none = np.zeros(0)
+    ob.check_topk(np.full(4, sentinel, f32), np.full(4, -1), np.zeros(0, np.int64), none, none, 4, metric)
+    with pytest.raises(ob.CertificateError):
+        ob.check_topk(np.array([1, sentinel], f32), np.array([5, -1]), np.zeros(0, np.int64), none, none, 2, metric)

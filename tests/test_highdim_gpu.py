@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from oracle import oracle_bound_np as ob
+from oracle import oracle_ivf_check_np as oc
 from oracle import oracle_sq_np as osq
 
 pytestmark = pytest.mark.gpu
@@ -98,29 +99,6 @@ def test_flat_highdim_certified(res, d, k, N, nq, metric, fp16, kind, api):
     ob.check_knn(D, I, ids, T, B, k, metric, what="flat d=%d k=%d" % (d, k))
 
 
-# ------------------------------------------------------------------ IVF helpers
-def _probes(xq, cent, nprobe, metric):
-    """probes and coarse distances in float64 from the index's own centroids"""
-    q, c = xq.astype(np.float64), cent.astype(np.float64)
-    if metric == L2:
-        dis = (q * q).sum(1)[:, None] + (c * c).sum(1)[None, :] - 2 * q @ c.T
-        order = np.argsort(dis, 1, kind="stable")[:, :nprobe]
-    else:
-        dis = q @ c.T
-        order = np.argsort(-dis, 1, kind="stable")[:, :nprobe]
-    return order.astype(np.int64), np.take_along_axis(dis, order, 1).astype(f32)
-
-
-def _search_preassigned(idx, xq, k, probes, cdis):
-    """IndexIVF::search_preassigned reads nprobe entries of every assign row, nprobe being the index's"""
-    idx.nprobe = probes.shape[1]
-    return idx.search_preassigned(xq, k, probes, cdis)
-
-
-def _lists(idx, probes_row):
-    return [(int(l), idx.getListIndices(int(l)), idx.getListVectorData(int(l))) for l in probes_row]
-
-
 # ------------------------------------------------------------------ IVF-Flat
 # d 384 / 512: the fast path with nch = 3 / 4 float4 chunks per lane; 640: a multiple of 128 past the fast path;
 # 300 / 1000: the generic path.  (512, 2048, nprobe 1) probes the smallest list, fewer than k vectors: -1 padding.
@@ -147,13 +125,13 @@ def test_ivfflat_highdim_certified(res, d, k, metric, nprobe):
     idx.setClustering(niter=4, seed=7)
     idx.train(xb)
     idx.add(xb)
-    probes, cdis = _probes(xq, idx.getCoarseCentroids(), nprobe, metric)
+    probes, cdis = oc.probes(xq, idx.getCoarseCentroids(), nprobe, metric)
     if nprobe == 1:  # probe the smallest list: fewer than k candidates
         sizes = np.array([idx.getListLength(l) for l in range(nlist)])
         probes[:] = int(np.argmin(np.where(sizes > 0, sizes, N)))
-    D, I = _search_preassigned(idx, xq, k, probes, cdis)
+    D, I = oc.search_preassigned(idx, xq, k, probes, cdis)
     for qi in range(nq):
-        ls = _lists(idx, probes[qi])
+        ls = oc.probed_lists(idx, probes[qi])
         ids = np.concatenate([i for _, i, _ in ls])
         Y = np.concatenate([v.view(f32).reshape(-1, d) for _, _, v in ls])
         for l, li, v in ls:
@@ -165,54 +143,20 @@ def test_ivfflat_highdim_certified(res, d, k, metric, nprobe):
 
 
 # ------------------------------------------------------------------ IVF-PQ
-def _unpack(codes, M, nbits):
-    """ProductQuantizer codes [n, code_size] (LSB-first bitstring) -> [n, M] ints"""
-    if nbits == 8:
-        return codes.astype(np.int64)
-    bits = np.unpackbits(codes, axis=1, bitorder="little")
-    w = 1 << np.arange(nbits)
-    return (bits[:, : M * nbits].reshape(-1, M, nbits) * w).sum(2).astype(np.int64)
-
-
-def _pq_check_codes(x, cent_l, pq, codes, M, exact):
-    """codes against the float64 argmin of the residual sub-vectors; a different pick is allowed only where
-    the two sub-distances lie within their bounds (exact: never -- the first minimum wins)"""
-    dsub = pq.shape[2]
-    r = x.astype(np.float64) - cent_l.astype(np.float64)[None, :]
-    for m in range(M):
-        rm = r[:, m * dsub : (m + 1) * dsub]
-        y = pq[m].astype(np.float64)
-        dist = (rm * rm).sum(1)[:, None] + (y * y).sum(1)[None, :] - 2 * rm @ y.T  # exact on integers
-        best = np.argmin(dist, 1)
-        got = codes[:, m]
-        bad = np.nonzero(got != best)[0]
-        if bad.size == 0:
-            continue
-        assert not exact, "sub-quantiser %d: codes %s, first minimum %s" % (m, got[bad][:5], best[bad][:5])
-        for i in bad:
-            pair = np.array([got[i], best[i]])
-            diff = rm[i][None, :] - y[pair]
-            t = (diff * diff).sum(1)
-            e = np.broadcast_to(2 * ob.U * np.abs(rm[i])[None, :], diff.shape)
-            beta = ob.perturbed_l2_bound(diff, e, dsub + 3) + ob.slack((rm[i] ** 2).sum() + (y[pair] ** 2).sum(1), 4 * dsub)
-            assert t[0] - t[1] <= beta.sum(), "sub-quantiser %d, vector %d: code %d is %.3e worse than %d (bound %.3e)" % (
-                m, i, got[i], t[0] - t[1], best[i], beta.sum())
-
-
 def _pq_search_and_check(idx, xb, xq, k, metric, M, nbits, nprobe, precomp, exact=False):
     d = xb.shape[1]
     dsub = d // M
     cent = idx.getCoarseCentroids()
     pq = idx.getPQCentroids()
-    probes, cdis = _probes(xq, cent, nprobe, metric)
-    D, I = _search_preassigned(idx, xq, k, probes, cdis)
+    probes, cdis = oc.probes(xq, cent, nprobe, metric)
+    D, I = oc.search_preassigned(idx, xq, k, probes, cdis)
     checked = set()
     for qi in range(xq.shape[0]):
         ids_all, t_all, b_all = [], [], []
-        for l, li, raw in _lists(idx, probes[qi]):
-            codes = _unpack(raw.reshape(li.size, -1), M, nbits)
+        for l, li, raw in oc.probed_lists(idx, probes[qi]):
+            codes = oc.unpack(raw.reshape(li.size, -1), M, nbits)
             if l not in checked:
-                _pq_check_codes(xb[li], cent[l], pq, codes, M, exact)
+                oc.pq_check_codes(xb[li], cent[l], pq, codes, M, exact)
                 checked.add(l)
             Yd = pq[np.arange(M)[None, :], codes].reshape(li.size, d)
             if metric == L2 and precomp:
@@ -288,20 +232,6 @@ def test_ivfpq_integer_codebooks_bit_exact(res, M, precomp, metric):
 
 
 # ------------------------------------------------------------------ IVF-SQ
-def _sq_exact_decode(codes, qtype, trained, d):
-    """float64 decode vmin + vdiff (c + 1/2) / s of the index's codes (the kernel's reference value)"""
-    x32 = osq.sq_decode(codes, qtype, trained, d)
-    if qtype in (osq.QT_fp16, osq.QT_8bit_direct):
-        return x32.astype(np.float64), np.zeros(d), np.zeros(d)
-    s = osq._levels(qtype)
-    unit = osq.sq_decode(codes, qtype, np.concatenate([np.zeros(d), np.ones(d)]).astype(f32)
-                         if qtype in osq.NON_UNIFORM else np.array([0, 1], f32), d)
-    lev = np.rint(unit.astype(np.float64) * s - 0.5)  # (c + 1/2) / s rounded to fp32 still names c
-    vmin, vdiff = osq._ranges(qtype, trained, d)
-    vmin, vdiff = vmin.astype(np.float64), vdiff.astype(np.float64)
-    return vmin[None, :] + vdiff[None, :] * (lev + 0.5) / s, vmin, vdiff
-
-
 # (qtype, d, encodeResidual): 8bit d 384 and 6bit d 1000 take the generic scan, fp16 d 512 the fast path's 4 chunks,
 # fp16 d 640 and 4bit d 768 the generic path past it; 8bit_direct on integers 0..15 without a residual is exact
 IVFSQ_CASES = [
@@ -334,12 +264,12 @@ def test_ivfsq_highdim_certified(res, qtype, d, residual):
     idx.add(xb)
     trained = idx.getTrained()
     cent = idx.getCoarseCentroids()
-    probes, cdis = _probes(xq, cent, nprobe, L2)
-    D, I = _search_preassigned(idx, xq, k, probes, cdis)
+    probes, cdis = oc.probes(xq, cent, nprobe, L2)
+    D, I = oc.search_preassigned(idx, xq, k, probes, cdis)
     for qi in range(nq):
         ids_all, t_all, b_all = [], [], []
-        for l, li, raw in _lists(idx, probes[qi]):
-            X, vmin, vdiff = _sq_exact_decode(raw, qtype, trained, d)
+        for l, li, raw in oc.probed_lists(idx, probes[qi]):
+            X, vmin, vdiff = oc.sq_exact_decode(raw, qtype, trained, d)
             r = xq[qi].astype(np.float64) - (cent[l].astype(np.float64) if residual else 0.0)
             t, b = ob.sq_l2_truth(r, X, vmin, vdiff)
             ids_all.append(li)

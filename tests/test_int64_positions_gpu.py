@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 
 from oracle import oracle_bound_np as ob
+from oracle import oracle_ivf_check_np as oc
 
 L2, IP = ob.METRIC_L2, ob.METRIC_INNER_PRODUCT
 METRIC_L1 = 2
@@ -305,24 +306,22 @@ def _arena_bytes(layout, code_size, lens):
 
 def _ivf_truth_check(idx, kind, d, metric, opt, xq, D, I, probes):
     """each query against float64 truth over its probed lists (bound 0 where the data are integers)"""
-    from tests.test_highdim_gpu import _lists, _sq_exact_decode, _unpack
-
     cent = idx.getCoarseCentroids()
     exact = kind == "flat" or (kind == "sq" and opt == 5)
     for qi in range(xq.shape[0]):
         ids_all, t_all, b_all = [], [], []
-        for l, li, raw in _lists(idx, probes[qi]):
+        for l, li, raw in oc.probed_lists(idx, probes[qi]):
             if kind == "flat":
                 Y = raw.view(f32).reshape(-1, d)
                 t, b = ob.l2_truth(xq[qi], Y) if metric == L2 else ob.ip_truth(xq[qi], Y)
             elif kind == "sq":
-                X, vmin, vdiff = _sq_exact_decode(raw, opt, idx.getTrained(), d)
+                X, vmin, vdiff = oc.sq_exact_decode(raw, opt, idx.getTrained(), d)
                 r = xq[qi].astype(np.float64) - (0.0 if opt == 5 else cent[l].astype(np.float64))
                 t, b = ob.sq_l2_truth(r, X, vmin, vdiff)
             else:
                 M, nbits = opt
                 pq = idx.getPQCentroids()
-                codes = _unpack(raw.reshape(li.size, -1), M, nbits)
+                codes = oc.unpack(raw.reshape(li.size, -1), M, nbits)
                 Yd = pq[np.arange(M)[None, :], codes].reshape(li.size, d)
                 t, b = ob.pq_l2_truth(xq[qi].astype(np.float64) - cent[l], Yd, d // M, M)
             ids_all.append(li)
@@ -352,7 +351,6 @@ def _ivf_same(wide, twin, kind, d, metric, opt, xq, what):
     import torch
 
     import faiss_b200 as fb
-    from tests.test_highdim_gpu import _probes
 
     k, n = IVF_K, twin.ntotal
     assert wide.ntotal == n
@@ -368,7 +366,7 @@ def _ivf_same(wide, twin, kind, d, metric, opt, xq, what):
             assert torch.equal(x, y) if torch.is_tensor(x) else np.array_equal(x, y), "%s: %s" % (what, name)
 
     same(wide.search(xq_d, k), twin.search(xq_d, k), "search")
-    probes, cdis = _probes(xq, wide.getCoarseCentroids(), IVF_NPROBE, metric)
+    probes, cdis = oc.probes(xq, wide.getCoarseCentroids(), IVF_NPROBE, metric)
     D, I = wide.search_preassigned(xq, k, probes, cdis)
     same((D, I), twin.search_preassigned(xq, k, probes, cdis), "search_preassigned")
     _ivf_truth_check(wide, kind, d, metric, opt, xq, D, I, probes)
