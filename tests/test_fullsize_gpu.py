@@ -4,7 +4,8 @@ The oracle cannot answer 10M x 10k in test time, so these use size-independent p
 equality of the tensor-core path with the exact fp32 kernel (bit for bit) on a query sample, self-queries,
 sortedness / uniqueness, shard-and-merge == unsharded, search == search_preassigned
 (faiss/gpu/test/test_gpu_index.py:190-194), batch-size invariance and run-to-run determinism.
-Synthetic data, generated on the device in seeded chunks."""
+Synthetic data, generated on the device in seeded chunks.  The last test holds bench.py's Flat search, every query,
+to float64 truth computed on the device (oracle/oracle_bound_torch.py)."""
 import numpy as np
 import pytest
 
@@ -271,3 +272,75 @@ def test_ivfpq_100m_vs_reference(res, ref):
     # distances agree to fp32 summation order (the reference test's own tolerance is 0.035 / 0.1 / 0.06)
     o.compare_lists(rD, rI, gD, gI, eps=2e-4, pct_max_diff1=0.03, pct_max_diffN=0.015)
     assert np.max(np.abs(rD - gD) / np.maximum(rD, 1e-20)) <= 2e-4
+
+
+# ------------------------------------------------------------------------------------------------
+# bench.py's flagship search, every query certified against float64 truth over all 10M rows
+# (oracle/oracle_bound_torch.certify_knn).
+# The inputs restate bench.gen_rows (1M-row chunks seeded 1234 + c) and bench.gen_queries (seed 1235).
+# ------------------------------------------------------------------------------------------------
+BENCH_N, BENCH_D, BENCH_NQ = 10_000_000, 128, 10_000
+# name: (metric, integer data, k, operand bits the search must take)
+BENCH_SEARCHES = {
+    "l2_k100": (1, False, 100, 8),  # the benchmarked search: int8 scoring on this database
+    "l2_k1": (1, False, 1, 16),  # streaming mode (IVF add, k-means assignment)
+    "l2_k1024": (1, False, 1024, 16),  # sorted base lists, five query batches of 2048
+    "ip_k100": (0, False, 100, 16),
+    "int_k100": (1, True, 100, 8),  # floor(16 x): every sum exact, the exact top-k including the rank-k tie group
+}
+
+
+@pytest.fixture(scope="module")
+def bench_flat(res):
+    """bench.py's rows and queries and one index over them at a time, built once per module.  The integer searches
+    floor the same 5 GB of rows in place: one copy of the database is on the device at any time."""
+    import torch
+
+    import faiss_b200 as fb
+
+    state = {}
+
+    def get(metric, integer):
+        key = (metric, integer)
+        if state.get("key") != key:
+            state.pop("idx", None)
+            if "xb" not in state or (state["integer"] and not integer):
+                state.pop("xb", None)
+                state["xb"] = _rows(torch, BENCH_N, BENCH_D, 1234)
+                state["xq"] = _sample_queries(torch, BENCH_NQ, BENCH_D, 1235)[0]
+                state["integer"] = False
+            if integer and not state["integer"]:
+                state["xb"].mul_(16).floor_()
+                state["xq"].mul_(16).floor_()
+                state["integer"] = True
+            idx = fb.GpuIndexFlat(res, BENCH_D, metric)
+            idx.add(state["xb"])
+            state["idx"], state["key"] = idx, key
+        return state["idx"], state["xq"], state["xb"]
+
+    yield get
+    state.clear()
+
+
+@pytest.mark.parametrize("name", list(BENCH_SEARCHES))
+def test_bench_search_certified(bench_flat, name, record_property):
+    import torch
+
+    from oracle import oracle_bound_torch as obt
+
+    metric, integer, k, bits = BENCH_SEARCHES[name]
+    idx, xq, xb = bench_flat(metric, integer)
+    D, I = idx.search(xq, k)
+    info = idx.lastSearchInfo()
+    assert info["tensor_cores"] == 1, info
+    assert idx.lastSearchOperandBits() == bits, "%s took %d-bit operands (the int8 fitness test decides)" % (
+        name, idx.lastSearchOperandBits())
+    record_property("fallback_queries", info["fallback_queries"])
+    torch.cuda.synchronize()
+    base = torch.cuda.memory_allocated()
+    torch.cuda.reset_peak_memory_stats()
+    obt.certify_knn(D, I, xq, xb, k, metric, exact=integer, what=name)
+    peak = torch.cuda.max_memory_allocated() - base
+    record_property("certifier_peak_bytes", peak)
+    # the GPUs are shared: the certifier's transient matrices stay a few GB whatever the database size
+    assert peak < 8 << 30, "certifier peak %.2f GB" % (peak / 2**30)
