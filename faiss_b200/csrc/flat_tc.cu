@@ -973,44 +973,25 @@ PFN_encodeTiled getEncodeTiled() {
     return fn;
 }
 
-// fp16 matrix [rows][dpad] viewed as (64, rows, dpad/64); one box = (64, 128, dpad/64) = a full
-// K-extent tile laid out [kblock][row][64] with the 128-byte swizzle the UMMA descriptors expect.
-// boxK = 0: the box spans every K-block (a whole tile); boxK = 1: one K-block per copy (K-split database stages).
-CUtensorMap makeTileMap(const __half* base, int64_t rows, int dpad, int boxRows, int boxK = 0) {
-    CUtensorMap m;
-    cuuint64_t dims[3] = {(cuuint64_t)kKBlock, (cuuint64_t)rows, (cuuint64_t)(dpad / kKBlock)};
-    cuuint64_t strides[2] = {(cuuint64_t)dpad * 2, (cuuint64_t)kKBlock * 2};
-    cuuint32_t box[3] = {(cuuint32_t)kKBlock, (cuuint32_t)boxRows, (cuuint32_t)(boxK > 0 ? boxK : dpad / kKBlock)};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = getEncodeTiled()(
-            &m,
-            CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
-            3,
-            const_cast<__half*>(base),
-            dims,
-            strides,
-            box,
-            estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B,
-            CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    FB_THROW_IF_NOT_FMT(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with %d", (int)r);
-    return m;
-}
+constexpr int kKBlockBytes = 128; // one K-block of a row: kKBlock fp16 or kDpad8 int8 operands, one swizzle row
 
-// int8 matrix [rows][128] viewed as (128, rows, 1); one box = 128 bytes x boxRows rows, 128-byte swizzle
-CUtensorMap makeTileMap8(const int8_t* base, int64_t rows, int boxRows) {
+// operand matrix [rows][kBlocks x 128 bytes] of fp16 (bits = 16) or int8 (bits = 8) viewed as (128-byte K-block, rows,
+// kBlocks); one box = (K-block, boxRows, boxKBlocks) laid out [kblock][row][128 bytes] with the 128-byte swizzle the
+// wgmma descriptors expect.  boxKBlocks = kBlocks: a whole K-extent per copy; 1: K-split database stages.
+CUtensorMap makeTileMap(const void* base, int bits, int64_t rows, int kBlocks, int boxRows, int boxKBlocks) {
     CUtensorMap m;
-    cuuint64_t dims[3] = {(cuuint64_t)kDpad8, (cuuint64_t)rows, 1};
-    cuuint64_t strides[2] = {(cuuint64_t)kDpad8, (cuuint64_t)rows * kDpad8};
-    cuuint32_t box[3] = {(cuuint32_t)kDpad8, (cuuint32_t)boxRows, 1};
+    const cuuint64_t rowBytes = (cuuint64_t)kBlocks * kKBlockBytes;
+    const cuuint32_t blockElems = kKBlockBytes * 8 / bits;
+    cuuint64_t dims[3] = {blockElems, (cuuint64_t)rows, (cuuint64_t)kBlocks};
+    // int8 rows are one K-block: that extent-1 dimension takes the stride of the whole matrix
+    cuuint64_t strides[2] = {rowBytes, bits == 8 ? (cuuint64_t)rows * rowBytes : kKBlockBytes};
+    cuuint32_t box[3] = {blockElems, (cuuint32_t)boxRows, (cuuint32_t)boxKBlocks};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = getEncodeTiled()(
             &m,
-            CU_TENSOR_MAP_DATA_TYPE_UINT8,
+            bits == 8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
             3,
-            const_cast<int8_t*>(base),
+            const_cast<void*>(base),
             dims,
             strides,
             box,
@@ -1124,30 +1105,33 @@ bool flatTcSupported(int d, int k, int64_t n) {
     return dpad <= kMaxKB * kKBlock && k >= 1 && k <= 2048 && n >= (k == 1 ? 2048 : 32768) && n < (int64_t(1) << 31) - 512;
 }
 
+FlatTcDatabase::Layout::Layout(GpuResources* res, int device, int bits, int kBlocks)
+        : bits(bits),
+          kBlocks(kBlocks),
+          rows(res, device, AllocType::FlatData),
+          bias(res, device, AllocType::FlatData),
+          tileBias(res, device, AllocType::FlatData),
+          perm(res, device, AllocType::FlatData) {}
+
+void FlatTcDatabase::Layout::clear() {
+    rows.clear();
+    bias.clear();
+    tileBias.clear();
+    perm.clear();
+}
+
 FlatTcDatabase::FlatTcDatabase(GpuResources* res, int device, int d)
         : res_(res),
           device_(device),
           d_(d),
           dpad_((int)round_up(d, kKBlock)),
-          y16_(res, device, AllocType::FlatData),
-          bias_(res, device, AllocType::FlatData),
-          perm_(res, device, AllocType::FlatData),
-          tileBias_(res, device, AllocType::FlatData),
-          y8_(res, device, AllocType::FlatData),
-          bias8_(res, device, AllocType::FlatData),
-          perm8_(res, device, AllocType::FlatData),
-          tileBias8_(res, device, AllocType::FlatData),
+          fp16_(res, device, 16, dpad_ / kKBlock),
+          int8_(res, device, 8, 1),
           center_(res, device, AllocType::FlatData) {}
 
 void FlatTcDatabase::clear() {
-    y16_.clear();
-    bias_.clear();
-    perm_.clear();
-    tileBias_.clear();
-    y8_.clear();
-    bias8_.clear();
-    perm8_.clear();
-    tileBias8_.clear();
+    fp16_.clear();
+    int8_.clear();
     center_.clear();
     dirty_ = true;
 }
@@ -1159,30 +1143,46 @@ void FlatTcDatabase::prepare(const void* rows, int64_t n, MetricType metric, int
     n_ = n;
     metric_ = metric;
     yHalf_ = yHalf;
-    fp16Ready_ = false;
-    int8Ready_ = false;
+    fp16_.ready = false;
+    int8_.ready = false;
     dirty_ = false;
 }
 
+// a layout sized for n rows, its bias -inf throughout: whole 256-row tiles plus one, -inf beyond n
+void FlatTcDatabase::resetLayout_(Layout& L, int64_t n, cudaStream_t stream) {
+    const int64_t padRows = round_up(n, 256) + 256;
+    L.rows.resize((size_t)n * L.kBlocks * kKBlockBytes, stream);
+    L.bias.resize((size_t)padRows, stream);
+    L.tileBias.resize((size_t)(padRows / 256) * 2, stream); // [T+1] max bias per tile, then [T+1] min bias per tile
+    fill_float_kernel<<<(unsigned)ceil_div(padRows, 256), 256, 0, stream>>>(L.bias.data(), padRows, -INFINITY);
+    CUDA_CHECK_LAST();
+}
+
+// perm [n] = the row ids in increasing order of keys [n]: the stored order of a layout
+void FlatTcDatabase::sortedPerm_(const float* keys, int64_t n, DeviceVector<int>& perm, cudaStream_t stream) {
+    perm.resize((size_t)n, stream);
+    auto keysOut = res_->temp(device_, sizeof(float) * n);
+    auto valsIn = res_->temp(device_, sizeof(int) * n);
+    tc_iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, stream>>>(valsIn.as<int>(), n);
+    CUDA_CHECK_LAST();
+    size_t tmpBytes = 0;
+    CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
+            nullptr, tmpBytes, keys, keysOut.as<float>(), valsIn.as<int>(), perm.data(), (int)n, 0, 32, stream));
+    auto tmp = res_->temp(device_, tmpBytes);
+    CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
+            tmp.data, tmpBytes, keys, keysOut.as<float>(), valsIn.as<int>(), perm.data(), (int)n, 0, 32, stream));
+}
+
 void FlatTcDatabase::prepareFp16(cudaStream_t stream) {
-    const void* rows = rows_;
     const int64_t n = n_;
-    const MetricType metric = metric_;
-    const int yHalf = yHalf_;
     const int d = d_, dpad = dpad_;
-    const int64_t padRows = round_up(n, 256) + 256; // whole 256-row tiles, -inf beyond n
-    y16_.resize((size_t)n * dpad, stream);
-    bias_.resize((size_t)padRows, stream);
-    tileBias_.resize((size_t)(padRows / 256) * 2, stream); // [T+1] max bias per tile, then [T+1] min bias per tile
-    const bool sorted = metric == METRIC_L2; // IP has no bias: row order is kept
-    if (sorted)
-        perm_.resize((size_t)n, stream);
-    else
-        perm_.clear();
+    Layout& L = fp16_;
+    resetLayout_(L, n, stream);
+    const bool sorted = metric_ == METRIC_L2; // IP has no bias: row order is kept
     auto scal = res_->temp(device_, sizeof(float) * 2);
     auto norms = res_->temp(device_, sizeof(float) * n);
     CUDA_VERIFY(cudaMemsetAsync(scal.data, 0, sizeof(float) * 2, stream));
-    runAbsMax(rows, n * (int64_t)d, scal.as<float>(), stream, yHalf);
+    runAbsMax(rows_, n * (int64_t)d, scal.as<float>(), stream, yHalf_);
     float h[2] = {0.f, 0.f};
     CUDA_VERIFY(cudaMemcpyAsync(h, scal.data, sizeof(float), cudaMemcpyDeviceToHost, stream));
     CUDA_VERIFY(cudaStreamSynchronize(stream));
@@ -1192,39 +1192,29 @@ void FlatTcDatabase::prepareFp16(cudaStream_t stream) {
         std::frexp(h[0], &e);
         scale = std::ldexp(1.f, 14 - e); // max |y| * scale in [2^13, 2^14)
     }
-    fill_float_kernel<<<(unsigned)ceil_div(padRows, 256), 256, 0, stream>>>(bias_.data(), padRows, -INFINITY);
-    CUDA_CHECK_LAST();
     const int warps = 8;
     const unsigned rowBlocks = (unsigned)ceil_div(n, warps);
-    int* perm = sorted ? perm_.data() : nullptr;
     // squared norms in row order (also feed the max-norm reduction)
     tc_prepare_rows_kernel<<<rowBlocks, warps * 32, 0, stream>>>(
-            rows, yHalf, n, d, dpad, scale, sorted, nullptr, nullptr, nullptr, norms.as<float>());
+            rows_, yHalf_, n, d, dpad, scale, sorted, nullptr, nullptr, nullptr, norms.as<float>());
     CUDA_CHECK_LAST();
-    if (perm) {
-        // stored order = rows sorted by squared norm: the biases of a 256-row tile are then nearly
-        // equal, which is what makes the kernel's per-tile score bound tight (flat_tc_kernel.cuh)
-        auto keysOut = res_->temp(device_, sizeof(float) * n);
-        auto valsIn = res_->temp(device_, sizeof(int) * n);
-        tc_iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, stream>>>(valsIn.as<int>(), n);
-        CUDA_CHECK_LAST();
-        size_t tmpBytes = 0;
-        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
-                nullptr, tmpBytes, norms.as<float>(), keysOut.as<float>(), valsIn.as<int>(), perm, (int)n, 0, 32, stream));
-        auto tmp = res_->temp(device_, tmpBytes);
-        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
-                tmp.data, tmpBytes, norms.as<float>(), keysOut.as<float>(), valsIn.as<int>(), perm, (int)n, 0, 32, stream));
-    }
+    // stored order = rows sorted by squared norm: the biases of a 256-row tile are then nearly
+    // equal, which is what makes the kernel's per-tile score bound tight (flat_tc_kernel.cuh)
+    if (sorted)
+        sortedPerm_(norms.as<float>(), n, L.perm, stream);
+    else
+        L.perm.clear();
     tc_prepare_rows_kernel<<<rowBlocks, warps * 32, 0, stream>>>(
-            rows, yHalf, n, d, dpad, scale, sorted, perm, y16_.data(), bias_.data(), nullptr);
+            rows_, yHalf_, n, d, dpad, scale, sorted, L.perm.data(), reinterpret_cast<__half*>(L.rows.data()),
+            L.bias.data(), nullptr);
     CUDA_CHECK_LAST();
-    runTileBias(bias_.data(), n, tileBias_.data(), stream);
+    runTileBias(L.bias.data(), n, L.tileBias.data(), stream);
     runAbsMax(norms.as<float>(), n, scal.as<float>() + 1, stream);
     CUDA_VERIFY(cudaMemcpyAsync(h, scal.data, sizeof(float) * 2, cudaMemcpyDeviceToHost, stream));
     CUDA_VERIFY(cudaStreamSynchronize(stream));
     scale_ = scale;
     maxNorm_ = std::sqrt(h[1]) * 1.0001f;
-    fp16Ready_ = true;
+    L.ready = true;
 }
 
 // Fitness of the int8 layout.  The int8 certificate's database term for a query q is about |q|*max|r_y|, the fp16
@@ -1236,11 +1226,8 @@ constexpr float kInt8Fitness = 4.f;
 void FlatTcDatabase::prepareInt8(cudaStream_t stream) {
     const int64_t n = n_;
     const int d = d_;
-    const int64_t padRows = round_up(n, 256) + 256;
-    y8_.resize((size_t)n * kDpad8, stream);
-    bias8_.resize((size_t)padRows, stream);
-    tileBias8_.resize((size_t)(padRows / 256) * 2, stream);
-    perm8_.resize((size_t)n, stream);
+    Layout& L = int8_;
+    resetLayout_(L, n, stream);
     center_.resize((size_t)d, stream);
     // [0, 2d): column range keys; then s_y, the three stats maxima and the sum of row norms
     auto scratch = res_->temp(device_, sizeof(unsigned) * 2 * d + sizeof(float) * 8);
@@ -1259,27 +1246,17 @@ void FlatTcDatabase::prepareInt8(cudaStream_t stream) {
     tc_prepare_rows8_kernel<<<rowBlocks, warps * 32, 0, stream>>>(
             rows_, yHalf_, n, d, center_.data(), sc, nullptr, nullptr, nullptr, keys.as<float>(), norms.as<float>(), nullptr);
     CUDA_CHECK_LAST();
-    {
-        // stored order = rows sorted by the centred norm, which enters the bias
-        auto keysOut = res_->temp(device_, sizeof(float) * n);
-        auto valsIn = res_->temp(device_, sizeof(int) * n);
-        tc_iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, stream>>>(valsIn.as<int>(), n);
-        CUDA_CHECK_LAST();
-        size_t sortBytes = 0, sumBytes = 0;
-        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
-                nullptr, sortBytes, keys.as<float>(), keysOut.as<float>(), valsIn.as<int>(), perm8_.data(), (int)n, 0, 32, stream));
-        CUDA_VERIFY(cub::DeviceReduce::Sum(nullptr, sumBytes, norms.as<float>(), sc + 4, (int)n, stream));
-        auto tmp = res_->temp(device_, std::max(sortBytes, sumBytes));
-        CUDA_VERIFY(cub::DeviceRadixSort::SortPairs(
-                tmp.data, sortBytes, keys.as<float>(), keysOut.as<float>(), valsIn.as<int>(), perm8_.data(), (int)n, 0, 32, stream));
-        CUDA_VERIFY(cub::DeviceReduce::Sum(tmp.data, sumBytes, norms.as<float>(), sc + 4, (int)n, stream));
-    }
-    fill_float_kernel<<<(unsigned)ceil_div(padRows, 256), 256, 0, stream>>>(bias8_.data(), padRows, -INFINITY);
-    CUDA_CHECK_LAST();
+    // stored order = rows sorted by the centred norm, which enters the bias
+    sortedPerm_(keys.as<float>(), n, L.perm, stream);
+    size_t sumBytes = 0;
+    CUDA_VERIFY(cub::DeviceReduce::Sum(nullptr, sumBytes, norms.as<float>(), sc + 4, (int)n, stream));
+    auto sumTmp = res_->temp(device_, sumBytes);
+    CUDA_VERIFY(cub::DeviceReduce::Sum(sumTmp.data, sumBytes, norms.as<float>(), sc + 4, (int)n, stream));
     tc_prepare_rows8_kernel<<<rowBlocks, warps * 32, 0, stream>>>(
-            rows_, yHalf_, n, d, center_.data(), sc, perm8_.data(), y8_.data(), bias8_.data(), nullptr, nullptr, sc + 1);
+            rows_, yHalf_, n, d, center_.data(), sc, L.perm.data(), reinterpret_cast<int8_t*>(L.rows.data()),
+            L.bias.data(), nullptr, nullptr, sc + 1);
     CUDA_CHECK_LAST();
-    runTileBias(bias8_.data(), n, tileBias8_.data(), stream);
+    runTileBias(L.bias.data(), n, L.tileBias.data(), stream);
     float h[5];
     CUDA_VERIFY(cudaMemcpyAsync(h, sc, sizeof(h), cudaMemcpyDeviceToHost, stream));
     CUDA_VERIFY(cudaStreamSynchronize(stream));
@@ -1290,13 +1267,9 @@ void FlatTcDatabase::prepareInt8(cudaStream_t stream) {
     const float c1 = 1.01f * (ldexpf(1.f, -10) + (float)kDpad8 * ldexpf(1.f, -22));
     const float meanNorm = h[4] / (float)n;
     int8Fit_ = maxRy_ <= kInt8Fitness * c1 * meanNorm && std::isfinite(maxYc_) && std::isfinite(maxYhat_);
-    int8Ready_ = true;
-    if (!int8Fit_) { // the fp16 layout serves this database: give the memory back
-        y8_.clear();
-        bias8_.clear();
-        perm8_.clear();
-        tileBias8_.clear();
-    }
+    L.ready = true;
+    if (!int8Fit_) // the fp16 layout serves this database: give the memory back
+        L.clear();
 }
 
 bool FlatTcDatabase::int8Eligible(int k, const FlatTcShard* shard) const {
@@ -1305,18 +1278,18 @@ bool FlatTcDatabase::int8Eligible(int k, const FlatTcShard* shard) const {
     return metric_ == METRIC_L2 && d_ > 112 && d_ <= kDpad8 && k >= 2 && k <= 128 && shard == nullptr;
 }
 
-// one search call: the schedule, the launch configuration and the bias arrays (the masked copies under a row mask)
+// one search call: the schedule, the launch configuration, the layout it scans and that layout's bias arrays (the
+// masked copies under a row mask)
 struct FlatTcDatabase::Call {
     cudaStream_t stream;
     const FlatTcSchedule& s;
     int KB, kSteps;
     SmemPlan sp;
+    const Layout& L;
     const float* bias;
     const float* tileBias;
     CUtensorMap mapY;
     const FlatTcShard* shard;
-    bool int8;       // the int8 layout
-    const int* perm; // the layout's stored position -> row id (null: identity)
 };
 
 // device state of one query batch
@@ -1332,7 +1305,7 @@ struct FlatTcDatabase::Batch {
 void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
     const int64_t nq = b.nq, qPairs = b.qPairs;
     cudaStream_t stream = c.stream;
-    b.q16 = res_->temp(device_, c.int8 ? (size_t)qPairs * kUnitM * kDpad8 : sizeof(__half) * qPairs * kUnitM * dpad_);
+    b.q16 = res_->temp(device_, (size_t)qPairs * kUnitM * c.L.kBlocks * kKBlockBytes); // query rows as wide as the layout's
     b.scal = res_->temp(device_, sizeof(float) * 4); // [absmax, qScale, inv, -]
     b.eps = res_->temp(device_, sizeof(float) * nq);
     b.thr = res_->temp(device_, sizeof(float) * nq);
@@ -1347,7 +1320,7 @@ void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
     CUDA_VERIFY(cudaMemsetAsync(b.scal.data, 0, sizeof(float) * 4, stream));
     CUDA_VERIFY(cudaMemsetAsync(b.flags.data, 0, sizeof(int) * (nq + 1), stream));
     CUDA_VERIFY(cudaMemsetAsync(b.q16.data, 0, b.q16.size, stream));
-    if (c.int8) {
+    if (c.L.bits == 8) {
         b.invQ = res_->temp(device_, sizeof(float) * nq);
         CUDA_VERIFY(cudaMemcpyAsync(b.scal.data, &scale8_, sizeof(float), cudaMemcpyHostToDevice, stream));
         tc_prepare_queries8_kernel<<<(unsigned)ceil_div(nq, 8), 256, 0, stream>>>(
@@ -1369,8 +1342,7 @@ void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
         tc_init_base_kernel<<<(unsigned)ceil_div(cnt, 256), 256, 0, stream>>>(b.baseKey.as<float>(), b.baseId.as<int>(), cnt);
         CUDA_CHECK_LAST();
     }
-    b.mapQ = c.int8 ? makeTileMap8(b.q16.as<int8_t>(), qPairs * kUnitM, kTileM)
-                    : makeTileMap(b.q16.as<__half>(), qPairs * kUnitM, dpad_, kTileM);
+    b.mapQ = makeTileMap(b.q16.data, c.L.bits, qPairs * kUnitM, c.L.kBlocks, kTileM, c.L.kBlocks);
 }
 
 // One round: score its tiles and emit candidates, then fold them into the base lists and thresholds (and, sharded,
@@ -1386,7 +1358,7 @@ void FlatTcDatabase::runRound(const Call& c, const Batch& b, const FlatTcRound& 
     p.tileMinBias = c.tileBias + s.T + 1; // second half of the array (see tc_tile_max_bias_kernel)
     p.thr = b.thr.as<float>();
     p.eps = b.eps.as<float>();
-    p.invQ = c.int8 ? b.invQ.as<float>() : nullptr;
+    p.invQ = b.invQ.as<float>(); // null unless int8
     p.cand = arena;
     p.candCount = counts;
     if (p.tileBegin < p.tileEnd) {
@@ -1400,7 +1372,7 @@ void FlatTcDatabase::runRound(const Call& c, const Batch& b, const FlatTcRound& 
         withBool(metric_ == METRIC_L2, [&](auto l2) {
             withBool(yHalf_ != 0, [&](auto yh) {
                 tc_argmin_finish_kernel<l2, yh><<<(unsigned)ceil_div(nq, fw), fw * 32, 0, stream>>>(
-                        nq, d_, r.slices, kParts, arena, r.cap, counts, b.eps.as<float>(), b.Q, rows_, perm_.data(), outD, outI,
+                        nq, d_, r.slices, kParts, arena, r.cap, counts, b.eps.as<float>(), b.Q, rows_, c.L.perm.data(), outD, outI,
                         b.flags.as<int>());
             });
         });
@@ -1443,7 +1415,7 @@ void FlatTcDatabase::rerank(const Call& c, const Batch& b, float* outD, idx_t* o
             auto kern = tc_rerank_kernel<l2, yh>;
             CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rrSmem));
             kern<<<(unsigned)ceil_div(b.nq, rrWarps), rrWarps * 32, rrSmem, stream>>>(
-                    (int)b.nq, d_, s.k, s.LIST, s.KL, b.Q, rows_, c.perm, b.baseId.as<int>(), b.baseKey.as<float>(),
+                    (int)b.nq, d_, s.k, s.LIST, s.KL, b.Q, rows_, c.L.perm.data(), b.baseId.as<int>(), b.baseKey.as<float>(),
                     c.shard ? b.thr.as<float>() : nullptr, outD, outI);
         });
     });
@@ -1486,26 +1458,24 @@ int64_t FlatTcDatabase::search(const float* Q, int64_t nqAll, int k, float* outD
         return 0;
     FB_THROW_IF_NOT(flatTcSupported(d_, k, n_));
     bool int8 = int8Eligible(k, shard);
-    if (int8 && !int8Ready_)
+    if (int8 && !int8_.ready)
         prepareInt8(stream);
     int8 = int8 && int8Fit_;
-    if (!int8 && !fp16Ready_)
+    if (!int8 && !fp16_.ready)
         prepareFp16(stream);
-    lastBits_ = int8 ? 8 : 16;
-    const DeviceVector<float>& biasL = int8 ? bias8_ : bias_;
-    const DeviceVector<float>& tileBiasL = int8 ? tileBias8_ : tileBias_;
-    const int* perm = int8 ? perm8_.data() : perm_.data();
-    const float* bias = biasL.data();
-    const float* tileBias = tileBiasL.data();
+    const Layout& L = int8 ? int8_ : fp16_;
+    last_ = &L;
+    const float* bias = L.bias.data();
+    const float* tileBias = L.tileBias.data();
     GpuMemoryReservation maskedBias, maskedTileBias;
     if (rowMask) {
         // an excluded row gets a -inf bias: its score can then never pass a round's threshold, exactly as the
         // padding rows past n.  The certificate's maxima over all rows stay valid bounds.
-        maskedBias = res_->temp(device_, sizeof(float) * biasL.size());
-        maskedTileBias = res_->temp(device_, sizeof(float) * tileBiasL.size());
-        const int64_t padRows = (int64_t)biasL.size();
+        maskedBias = res_->temp(device_, sizeof(float) * L.bias.size());
+        maskedTileBias = res_->temp(device_, sizeof(float) * L.tileBias.size());
+        const int64_t padRows = (int64_t)L.bias.size();
         mask_bias_kernel<<<(unsigned)ceil_div(padRows, (int64_t)256), 256, 0, stream>>>(
-                bias, perm, rowMask, n_, padRows, maskedBias.as<float>());
+                bias, L.perm.data(), rowMask, n_, padRows, maskedBias.as<float>());
         CUDA_CHECK_LAST();
         runTileBias(maskedBias.as<float>(), n_, maskedTileBias.as<float>(), stream);
         bias = maskedBias.as<float>();
@@ -1516,9 +1486,8 @@ int64_t FlatTcDatabase::search(const float* Q, int64_t nqAll, int k, float* outD
     const FlatTcSchedule s = planFlatTcSchedule(
             n_, k, res_->numSMs(device_), shard ? shard->comm->size() : 0, shard ? shard->maxTiles : 0, int8);
     const SmemPlan sp = planSmem(KB, kSteps, int8);
-    const CUtensorMap mapY = int8 ? makeTileMap8(y8_.data(), n_, sp.boxRows)
-                                  : makeTileMap(y16_.data(), n_, dpad_, sp.boxRows, sp.ksplit);
-    const Call c{stream, s, KB, kSteps, sp, bias, tileBias, mapY, shard, int8, perm};
+    const CUtensorMap mapY = makeTileMap(L.rows.data(), L.bits, n_, L.kBlocks, sp.boxRows, sp.ksplit ? 1 : L.kBlocks);
+    const Call c{stream, s, KB, kSteps, sp, L, bias, tileBias, mapY, shard};
     int64_t fallbacks = 0;
     for (int64_t qb = 0; qb < nqAll; qb += s.qBatch) {
         Batch b;
@@ -1550,9 +1519,9 @@ void runFlatTcScoresDebug(const void* Q, int64_t nq, const void* Y, int64_t n, i
     const int KB = dpad / kKBlock;
     const int kSteps = dpad / 16; // debug seam: operands arrive padded
     SmemPlan sp = planSmem(KB, kSteps, s8);
-    const size_t rowBytes = s8 ? (size_t)kDpad8 : sizeof(__half) * dpad;
-    CUtensorMap my = s8 ? makeTileMap8((const int8_t*)Y, n, sp.boxRows)
-                        : makeTileMap((const __half*)Y, n, dpad, sp.boxRows, sp.ksplit);
+    const int bits = s8 ? 8 : 16, kBlocks = s8 ? 1 : KB;
+    const size_t rowBytes = (size_t)kBlocks * kKBlockBytes;
+    CUtensorMap my = makeTileMap(Y, bits, n, kBlocks, sp.boxRows, sp.ksplit ? 1 : kBlocks);
     const int64_t numTiles = ceil_div(n, kTileN);
     const int64_t qPairs = ceil_div(nq, kUnitM);
     // the kernel reads whole 128-row query tiles: zero-padded private copy
@@ -1568,8 +1537,7 @@ void runFlatTcScoresDebug(const void* Q, int64_t nq, const void* Y, int64_t n, i
     // every tile in one slice, unpermuted
     const FlatTcRound all{0, (int)numTiles, 1, (int)numTiles, 0};
     TcParams p = roundParams(sp, KB, kSteps, nq, qPairs, all, numTiles, 1, 0, one);
-    CUtensorMap mq = s8 ? makeTileMap8((const int8_t*)qpad, qPairs * kUnitM, kTileM)
-                        : makeTileMap((const __half*)qpad, qPairs * kUnitM, dpad, kTileM);
+    CUtensorMap mq = makeTileMap(qpad, bits, qPairs * kUnitM, kBlocks, kTileM, kBlocks);
     p.dump = S;
     p.dumpLd = numTiles * kTileN; // S must be [nq][numTiles*128]
     int dev = 0, sms = 0;

@@ -21,12 +21,9 @@ struct FlatTcShard {
     int64_t maxTiles;         // max over ranks of ceil(n_r / 256): the common round schedule
 };
 
-// The database as the tensor-core search scans it (DESIGN.md 2), in one or both of two layouts:
-//   fp16: the scaled fp16 rows, under L2 sorted by norm (perm: stored position -> row id), the bias per stored row, the
-//         max / min bias per 256-row tile, the scale and the max norm;
-//   int8 (L2, 112 < d <= 128): the rows centred on the per-dimension midrange c and quantised with one scale s_y,
-//         128 s8 per row, sorted by the centred norm, with their own perm, bias = -|y - c|^2 / 2 and tile bias, and
-//         the database constants of the int8 certificate.
+// The database as the tensor-core search scans it (DESIGN.md 2): one layout type, two instances.  The fp16 layout
+// serves every search; the int8 layout serves the searches that score on the int8 tensor cores (see search()).  Each
+// certificate keeps its own database constants beside its layout.
 // Each layout is built on the first search that needs it after invalidate(); DeviceVector::resize keeps the
 // allocations, so an index whose rows are replaced in place (the k-means loop) re-prepares without reallocating.
 class FlatTcDatabase {
@@ -51,10 +48,23 @@ class FlatTcDatabase {
                    const FlatTcShard* shard = nullptr, const uint32_t* rowMask = nullptr);
     // operand width of the last search's scoring: 8 or 16
     int lastOperandBits() const {
-        return lastBits_;
+        return last_->bits;
     }
 
    private:
+    // one layout, in stored order: rows [n][kBlocks * 128 bytes], bias [round_up(n, 256) + 256] (-inf past n),
+    // tileBias [T + 1] max then [T + 1] min bias per 256-row tile, perm [n] stored position -> row id (empty: the row
+    // order is kept)
+    struct Layout {
+        Layout(GpuResources* res, int device, int bits, int kBlocks);
+        void clear(); // gives the memory back
+        const int bits;    // operand width: 16 (fp16) or 8 (int8)
+        const int kBlocks; // 128-byte K-blocks per stored row
+        DeviceVector<uint8_t> rows;
+        DeviceVector<float> bias, tileBias;
+        DeviceVector<int> perm;
+        bool ready = false; // built from the rows of the last prepare()
+    };
     // the launch steps of search(), in order
     struct Call;  // one search call
     struct Batch; // one query batch of it
@@ -65,23 +75,19 @@ class FlatTcDatabase {
     int recomputeFallbacks(const Call& c, const Batch& b, const uint32_t* rowMask, float* outD, idx_t* outI) const;
     void prepareFp16(cudaStream_t stream);
     void prepareInt8(cudaStream_t stream);
+    void resetLayout_(Layout& L, int64_t n, cudaStream_t stream);
+    void sortedPerm_(const float* keys, int64_t n, DeviceVector<int>& perm, cudaStream_t stream);
     bool int8Eligible(int k, const FlatTcShard* shard) const;
 
     GpuResources* res_;
     int device_;
     int d_, dpad_;
-    // fp16 layout
-    DeviceVector<__half> y16_;
-    DeviceVector<float> bias_;
-    DeviceVector<int> perm_; // L2 only
-    DeviceVector<float> tileBias_;
+    Layout fp16_, int8_;
+    const Layout* last_ = &fp16_; // the last search's layout
+    // fp16 certificate
     float scale_ = 1.f;
     float maxNorm_ = 0.f;
-    // int8 layout
-    DeviceVector<int8_t> y8_;
-    DeviceVector<float> bias8_;
-    DeviceVector<int> perm8_;
-    DeviceVector<float> tileBias8_;
+    // int8 certificate
     DeviceVector<float> center_; // [d]
     float scale8_ = 1.f;         // s_y
     float maxYhat_ = 0.f;        // max |Y8 / s_y|, x 1.0001
@@ -89,8 +95,6 @@ class FlatTcDatabase {
     float maxYc_ = 0.f;          // max |y - c|, x 1.0001
     bool int8Fit_ = false;       // the int8 certificate is tight enough on this database (prepareInt8)
     bool dirty_ = true;
-    bool fp16Ready_ = false, int8Ready_ = false;
-    int lastBits_ = 16;
     // what the last prepare() was built from
     const void* rows_ = nullptr;
     int64_t n_ = 0;

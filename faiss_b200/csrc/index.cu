@@ -572,31 +572,40 @@ void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, i
         fillEmpty_(n, k, dDev, iDev);
         return;
     }
-    // metrics without a product form (L1, Linf, Lp, Canberra, ...) always run the exact kernel
-    const bool tc = useTensorCores_(k, n);
+    // metrics without a product form (L1, Linf, Lp, Canberra, ...) always run the exact kernel; a selector that keeps
+    // no row, or few enough for the compacted search, never reaches the tensor cores either
+    const uint32_t* mask = call.mask;
+    const bool compact = mask && call.selected * kCompactRatio <= this->ntotal;
+    if (useTensorCores_(k, n) && !compact) {
+        searchTc_(n, xDev, k, dDev, iDev, nullptr, mask, call.row0);
+        return;
+    }
     GpuMemoryReservation qHold;
     xDev = roundedQueries_(n, xDev, qHold);
-    const uint32_t* mask = call.mask;
-    if (mask) {
-        if (call.selected == 0) {
-            fillEmpty_(n, k, dDev, iDev);
-            return;
-        }
-        if (call.selected * kCompactRatio <= this->ntotal) {
-            searchCompacted_(n, xDev, k, dDev, iDev, mask, call.selected);
-            return;
-        }
+    if (mask && call.selected == 0) {
+        fillEmpty_(n, k, dDev, iDev);
+        return;
     }
-    if (tc) {
-        tc_.prepare(rows_(), this->ntotal, searchMetric_(), yHalf_(), stream);
-        lastSearchFallbackQueries += (int)tc_.search(xDev, n, k, dDev, iDev, stream, nullptr, mask);
-        lastSearchUsedTensorCores = 1;
-        lastSearchOperandBits = tc_.lastOperandBits();
-    } else {
-        runFlatExact(
-                resources_.get(), config_.device, xDev, n, rows_(), this->ntotal, d, k, searchMetric_(), 0, dDev, iDev,
-                stream, yHalf_(), metric_arg, mask);
+    if (compact) {
+        searchCompacted_(n, xDev, k, dDev, iDev, mask, call.selected);
+        return;
     }
+    runFlatExact(
+            resources_.get(), config_.device, xDev, n, rows_(), this->ntotal, d, k, searchMetric_(), 0, dDev, iDev, stream,
+            yHalf_(), metric_arg, mask);
+}
+
+void GpuIndexFlat::searchTc_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* shard,
+                             const uint32_t* mask, idx_t row0) const {
+    auto stream = stream_();
+    tc_.prepare(rows_(), this->ntotal, searchMetric_(), yHalf_(), stream);
+    GpuMemoryReservation qHold;
+    xDev = roundedQueries_(n, xDev, qHold);
+    if (row0 == 0)
+        lastSearchFallbackQueries = 0;
+    lastSearchFallbackQueries += (int)tc_.search(xDev, n, k, dDev, iDev, stream, shard, mask);
+    lastSearchUsedTensorCores = 1;
+    lastSearchOperandBits = tc_.lastOperandBits();
 }
 
 bool GpuIndexFlat::shardPoolingEligible(int k, idx_t n) const {
@@ -611,15 +620,7 @@ void GpuIndexFlat::searchShardDevice(
         return;
     }
     FB_THROW_IF_NOT_MSG(shardPoolingEligible(k, n), "pooled sharded search requested on a shard that cannot take the tensor-core path");
-    auto stream = stream_();
-    tc_.prepare(rows_(), this->ntotal, searchMetric_(), yHalf_(), stream);
-    GpuMemoryReservation qHold;
-    xDev = roundedQueries_(n, xDev, qHold);
-    if (call.row0 == 0)
-        lastSearchFallbackQueries = 0;
-    lastSearchFallbackQueries += (int)tc_.search(xDev, n, k, dDev, iDev, stream, flatShard);
-    lastSearchUsedTensorCores = 1;
-    lastSearchOperandBits = tc_.lastOperandBits();
+    searchTc_(n, xDev, k, dDev, iDev, flatShard, nullptr, call.row0);
 }
 
 void GpuIndexFlat::search_and_reconstruct(

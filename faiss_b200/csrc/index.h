@@ -252,6 +252,10 @@ class GpuIndexFlat : public GpuIndex {
     // the `selected` rows of mask only: gathered (fp32) and searched with the exact kernel, labels mapped back
     void searchCompacted_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const uint32_t* mask, idx_t selected) const;
     void fillEmpty_(idx_t n, int k, float* dDev, idx_t* iDev) const;
+    // the tensor-core search of the stored rows (shard: pooled across the ranks, or null; mask: null, or the rows it
+    // may return), with the diagnostics of the last search; row0 as call.row0
+    void searchTc_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const FlatTcShard* shard,
+                   const uint32_t* mask, idx_t row0) const;
     // the metric the kernels run, read at search time: METRIC_Lp with metric_arg 1 is L1 and with 2 is L2
     // (faiss/gpu/impl/Distance.cuh:223-239); only L2 and inner product can take the tensor-core path
     MetricType searchMetric_() const;
