@@ -6,7 +6,9 @@ flat_tc_kernel launch each; later rounds filter against tighter thresholds.  Thi
 index (N=10M, d=128, nq=10k, k=100; BENCH_N / BENCH_D / BENCH_NQ / BENCH_K override), warms it, then profiles
 --searches searches with torch.profiler (CUDA activities only) while nvidia-smi samples the SM clock.  For each round
 it prints the median kernel time, the largest number of tiles one CTA walks in it (from the schedule, compiled here
-with the host C++ compiler) and so the clocks per tile at the median SM clock.  The last line is one JSON object.
+with the host C++ compiler) and so the clocks per tile at the median SM clock, and how many queries were searched again
+because their estimated thresholds overshot (those repairs add launches outside the table).  The last line is one
+JSON object.
 
   python bench_flat_rounds.py [--searches 5] [--warmup 3]
 
@@ -121,6 +123,7 @@ def main():
         index.search(xq, bench.K)
     torch.cuda.synchronize()
     bits = index.lastSearchOperandBits()
+    repaired = index.lastSearchRepairedQueries()
     sched = schedule(bench.N_TOTAL, bench.K, sms, bench.NQ, bits == 8)
 
     sampler.mark_begin()
@@ -134,8 +137,8 @@ def main():
     kern = sorted((e for e in prof.events() if "flat_tc_kernel" in e.name), key=lambda e: e.time_range.start)
     per_search = len(sched)
     if len(kern) != per_search * args.searches:
-        raise RuntimeError("profiled %d flat_tc_kernel launches, the schedule has %d per search x %d searches"
-                           % (len(kern), per_search, args.searches))
+        raise RuntimeError("profiled %d flat_tc_kernel launches, the schedule has %d per search x %d searches "
+                           "(%d queries repaired per search)" % (len(kern), per_search, args.searches, repaired))
     ms = np.array([e.time_range.elapsed_us() * 1e-3 for e in kern]).reshape(args.searches, per_search)
     mhz = clocks.get("sm_mhz")
     rows = []
@@ -149,8 +152,8 @@ def main():
     total_tiles = sum(r["tiles_per_cta"] for r in rows)
     gpu = bench.gpu_identity(0)
 
-    print("%s, power limit %s W, median SM clock %s MHz (%s), operand bits %d"
-          % (gpu.get("name"), gpu.get("power_limit_w"), mhz, clocks.get("window", clocks.get("reasons")), bits))
+    print("%s, power limit %s W, median SM clock %s MHz (%s), operand bits %d, repaired queries %d"
+          % (gpu.get("name"), gpu.get("power_limit_w"), mhz, clocks.get("window", clocks.get("reasons")), bits, repaired))
     print("%5s %15s %6s %5s %6s %10s %9s %12s" % ("round", "tiles", "slices", "grid", "tps", "tiles/CTA", "ms", "clocks/tile"))
     for r in rows:
         cpt = "%12.0f" % r["clocks_per_tile"] if r["clocks_per_tile"] else "%12s" % "-"
@@ -159,7 +162,8 @@ def main():
     cpt_all = total_ms * 1e-3 * mhz * 1e6 / total_tiles if mhz else None
     print("%5s %15s %6s %5s %6s %10d %9.3f %s" % ("all", "", "", "", "", total_tiles, total_ms,
                                                   ("%12.0f" % cpt_all) if cpt_all else "-"))
-    print(json.dumps({"gpu": gpu, "clocks": clocks, "operand_bits": bits, "searches": args.searches,
+    print(json.dumps({"gpu": gpu, "clocks": clocks, "operand_bits": bits, "repaired_queries": repaired,
+                      "searches": args.searches,
                       "flat_tc_ms": total_ms, "tiles_per_cta": total_tiles, "clocks_per_tile": cpt_all, "rounds": rows}),
           flush=True)
 

@@ -538,6 +538,13 @@ class GpuIndexFlat(Index):
         check(lib.faiss_GpuIndexFlat_lastSearchOperandBits(self._h, ctypes.byref(out)))
         return int(out.value)
 
+    def lastSearchRepairedQueries(self):
+        """Queries of the last search searched again with provable thresholds because their estimated thresholds
+        overshot; they are not among lastSearchInfo()'s fallback (exact-kernel) queries."""
+        out = ctypes.c_int(0)
+        check(lib.faiss_GpuIndexFlat_lastSearchRepairedQueries(self._h, ctypes.byref(out)))
+        return int(out.value)
+
 
 class GpuIndexFlatL2(GpuIndexFlat):
     def __init__(self, res, d, device=0, use_tensor_cores=True, use_float16=False):

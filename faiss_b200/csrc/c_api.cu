@@ -361,6 +361,12 @@ int faiss_GpuIndexFlat_lastSearchOperandBits(const FaissGpuIndex* p, int* bits) 
     }
     CATCH_AND_HANDLE
 }
+int faiss_GpuIndexFlat_lastSearchRepairedQueries(const FaissGpuIndex* p, int* count) {
+    try {
+        *count = AS<GpuIndexFlat>(p, "GpuIndexFlat")->lastSearchRepairedQueries;
+    }
+    CATCH_AND_HANDLE
+}
 
 // ---------------------------------------------------------------- GpuIndexIVF
 int faiss_GpuIndexIVF_set_nprobe(FaissGpuIndex* p, size_t nprobe) {

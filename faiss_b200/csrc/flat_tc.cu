@@ -21,7 +21,9 @@
 //   * Thresholds come from geometric rounds over a pseudo-randomly permuted tile order: round 0
 //     scans ~40 k rows, round r 3x the rows seen so far; after each round a small kernel folds the new candidates into
 //     a per-query sorted base list and sets threshold = (k-th best approx score) - 2*eps_q, which
-//     provably keeps every true top-k member.
+//     provably keeps every true top-k member.  Before the last round it may instead take a lower rank's score
+//     (an estimate of the final k-th); the last round checks every estimate, and a query one overshot is
+//     searched again with provable thresholds.
 //   * Certified exact result.  The final kernel re-ranks the base list with the library's canonical
 //     fp32 arithmetic (same expression and order as flat_exact.cu) and sorts by (distance, id).
 //     Queries whose certificate fails (candidate segment or base list overflow) are recomputed by
@@ -407,6 +409,10 @@ __global__ void tc_prepare_queries8_kernel(
     }
 }
 
+// a query's flag after its batch's rounds: its certificate failed (a candidate segment or list overflowed), so the exact
+// kernel recomputes it; or the estimated thresholds overshot its final one, so it is searched again with provable ones
+constexpr int kFlagExact = 1, kFlagRepair = 2;
+
 // pending-candidate buffer of the select kernel: a round brings ~(growth-1)*k candidates per query, and
 // the cost of a flush is dominated by the merge into the 2k-entry list -- fewer, larger flushes
 constexpr int kSelectBuf = 128;
@@ -428,7 +434,9 @@ __global__ void tc_select_kernel(
         float* __restrict__ thr,
         int* __restrict__ flags,
         float* __restrict__ contrib, // sharded search: [2][nq] certified lower bounds for the cross-rank threshold (or null)
-        int kFrac) {                 // ceil(k / number of shards)
+        int kFrac,                   // ceil(k / number of shards)
+        int estRank,                 // > 0: raise the threshold to the estRank-th best score - 2 eps as well
+        int check) {                 // the last round after estimated thresholds: flag the queries they overshot
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5;
     const int lane = lane_id();
@@ -496,6 +504,9 @@ __global__ void tc_select_kernel(
         float s = -kthKey - 2.f * eps[q];
         t = nextafterf(s, -CUDART_INF_F);
     }
+    float tEst = -CUDART_INF_F; // list position estRank - 1 holds the estRank-th best score
+    if (estRank > 0 && w.q.ids[estRank - 1] != IdLimits<int>::max())
+        tEst = nextafterf(-w.q.keys[estRank - 1] - 2.f * eps[q], -CUDART_INF_F);
     // saturated list: an entry we could not keep might have been >= t
     float lastKey = w.q.keys[LIST - 1];
     int lastId = w.q.ids[LIST - 1];
@@ -511,9 +522,11 @@ __global__ void tc_select_kernel(
         oi[j] = keep ? id : IdLimits<int>::max();
     }
     if (lane == 0) {
-        thr[q] = fmaxf(t, thrNow);
-        if (overflow)
-            flags[q] = 1;
+        thr[q] = fmaxf(fmaxf(t, tEst), thrNow);
+        if (check && t < thrNow)
+            flags[q] = kFlagRepair;
+        else if (overflow)
+            flags[q] = kFlagExact;
         if (contrib) {
             // certified lower bounds of true scores: >= k rows of this shard score at least c0, >= kFrac rows at
             // least c1.  Across S shards: max_r c0 and min_r c1 (S * kFrac >= k rows) both bound the global k-th.
@@ -552,7 +565,9 @@ __global__ void __launch_bounds__(kSelWarps * 32) tc_select_bisect_kernel(
         float* __restrict__ thr,
         int* __restrict__ flags,
         float* __restrict__ contrib,
-        int kFrac) {
+        int kFrac,
+        int estRank,
+        int check) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5;
     const int lane = lane_id();
@@ -663,7 +678,13 @@ __global__ void __launch_bounds__(kSelWarps * 32) tc_select_bisect_kernel(
         kthScore = ordered_to_float(Tk);
         t = nextafterf(kthScore - 2.f * e2, -CUDART_INF_F);
     }
-    const float tNew = fmaxf(t, thrNow);
+    float tEst = -CUDART_INF_F;
+    if (estRank > 0) {
+        const unsigned Tj = kthLargest(estRank);
+        if (Tj != 0u)
+            tEst = nextafterf(ordered_to_float(Tj) - 2.f * e2, -CUDART_INF_F);
+    }
+    const float tNew = fmaxf(fmaxf(t, tEst), thrNow);
     // (4) survivors -> base list (compacted, unsorted), sentinels behind them
     int W = 0;
 #pragma unroll 1
@@ -696,8 +717,10 @@ __global__ void __launch_bounds__(kSelWarps * 32) tc_select_bisect_kernel(
     }
     if (lane == 0) {
         thr[q] = tNew;
-        if (overflow)
-            flags[q] = 1;
+        if (check && t < thrNow)
+            flags[q] = kFlagRepair;
+        else if (overflow)
+            flags[q] = kFlagExact;
     }
 }
 
@@ -909,14 +932,14 @@ __global__ void tc_argmin_finish_kernel(
         outD[q] = ok ? (IS_L2 ? bestD : -bestD) : (IS_L2 ? FLT_MAX : -FLT_MAX);
         outI[q] = ok ? (idx_t)bestI : -1;
         if (overflow || !ok)
-            flags[q] = 1;
+            flags[q] = kFlagExact;
     }
 }
 
-// compact flagged query indices: list[0..count)
-__global__ void tc_collect_flags_kernel(const int* flags, int nq, int* list, int* count) {
+// compact the indices of the queries flagged `flag`: list[0..count)
+__global__ void tc_collect_flags_kernel(const int* flags, int nq, int flag, int* list, int* count) {
     int q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q < nq && flags[q]) {
+    if (q < nq && flags[q] == flag) {
         int pos = atomicAdd(count, 1);
         list[pos] = q;
     }
@@ -1309,7 +1332,7 @@ void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
     b.scal = res_->temp(device_, sizeof(float) * 4); // [absmax, qScale, inv, -]
     b.eps = res_->temp(device_, sizeof(float) * nq);
     b.thr = res_->temp(device_, sizeof(float) * nq);
-    b.flags = res_->temp(device_, sizeof(int) * (nq + 1));
+    b.flags = res_->temp(device_, sizeof(int) * (nq + 3)); // [nq] flags, then a counter per flag value
     b.baseKey = res_->temp(device_, c.s.streaming ? sizeof(float) : sizeof(float) * nq * c.s.LIST);
     b.baseId = res_->temp(device_, c.s.streaming ? sizeof(int) : sizeof(int) * nq * c.s.LIST);
 
@@ -1318,7 +1341,7 @@ void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
     const float c2 = (float)(dpad_ + 16) * ldexpf(1.f, -24);
 
     CUDA_VERIFY(cudaMemsetAsync(b.scal.data, 0, sizeof(float) * 4, stream));
-    CUDA_VERIFY(cudaMemsetAsync(b.flags.data, 0, sizeof(int) * (nq + 1), stream));
+    CUDA_VERIFY(cudaMemsetAsync(b.flags.data, 0, sizeof(int) * (nq + 3), stream));
     CUDA_VERIFY(cudaMemsetAsync(b.q16.data, 0, b.q16.size, stream));
     if (c.L.bits == 8) {
         b.invQ = res_->temp(device_, sizeof(float) * nq);
@@ -1347,8 +1370,8 @@ void FlatTcDatabase::prepareQueries(const Call& c, Batch& b) const {
 
 // One round: score its tiles and emit candidates, then fold them into the base lists and thresholds (and, sharded,
 // pool the thresholds across the ranks) -- or, streaming, select and re-rank in one pass into outD / outI.
-void FlatTcDatabase::runRound(const Call& c, const Batch& b, const FlatTcRound& r, uint2* arena, int* counts, float* contrib,
-                              float* outD, idx_t* outI) const {
+void FlatTcDatabase::runRound(const Call& c, const Batch& b, const FlatTcRound& r, int estRank, bool check, uint2* arena,
+                              int* counts, float* contrib, float* outD, idx_t* outI) const {
     const FlatTcSchedule& s = c.s;
     cudaStream_t stream = c.stream;
     const int nq = (int)b.nq;
@@ -1389,7 +1412,7 @@ void FlatTcDatabase::runRound(const Call& c, const Batch& b, const FlatTcRound& 
     KernelTiming::begin("tc_select", stream);
     sel<<<(unsigned)ceil_div(nq, selWarps), selWarps * 32, selSmem, stream>>>(
             nq, s.k, s.LIST, r.slices, kParts, arena, r.cap, counts, b.eps.as<float>(), b.baseKey.as<float>(),
-            b.baseId.as<int>(), b.thr.as<float>(), b.flags.as<int>(), contrib, s.kFrac);
+            b.baseId.as<int>(), b.thr.as<float>(), b.flags.as<int>(), contrib, s.kFrac, estRank, (int)check);
     KernelTiming::end("tc_select", stream);
     CUDA_CHECK_LAST();
     if (c.shard) {
@@ -1423,18 +1446,50 @@ void FlatTcDatabase::rerank(const Call& c, const Batch& b, float* outD, idx_t* o
     CUDA_CHECK_LAST();
 }
 
+// the indices of the batch's queries flagged `flag` -> list; returns their number
+int FlatTcDatabase::collectFlagged(const Call& c, const Batch& b, int flag, GpuMemoryReservation& list) const {
+    const int64_t nq = b.nq;
+    list = res_->temp(device_, sizeof(int) * nq);
+    int* countDev = b.flags.as<int>() + nq + flag;
+    tc_collect_flags_kernel<<<(unsigned)ceil_div(nq, 256), 256, 0, c.stream>>>(b.flags.as<int>(), (int)nq, flag, list.as<int>(),
+                                                                               countDev);
+    CUDA_CHECK_LAST();
+    int nflag = 0;
+    CUDA_VERIFY(cudaMemcpyAsync(&nflag, countDev, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    CUDA_VERIFY(cudaStreamSynchronize(c.stream));
+    return nflag;
+}
+
+// queries whose estimated thresholds overshot their final one -> the same search with provable thresholds, into
+// outD / outI.  Returns their number and that search's exact recomputes.
+FlatTcDatabase::Counts FlatTcDatabase::repairEstimates(const Call& c, const Batch& b, const uint32_t* rowMask, float* outD,
+                                                       idx_t* outI) const {
+    const int k = c.s.k;
+    cudaStream_t stream = c.stream;
+    GpuMemoryReservation list;
+    Counts n;
+    n.repairs = collectFlagged(c, b, kFlagRepair, list);
+    if (n.repairs > 0) {
+        const int nr = (int)n.repairs;
+        auto rq = res_->temp(device_, sizeof(float) * (size_t)nr * d_);
+        auto rD = res_->temp(device_, sizeof(float) * (size_t)nr * k);
+        auto rI = res_->temp(device_, sizeof(idx_t) * (size_t)nr * k);
+        tc_gather_queries_kernel<<<nr, 128, 0, stream>>>(b.Q, list.as<int>(), d_, rq.as<float>());
+        CUDA_CHECK_LAST();
+        n.fallbacks = runBatch(c, rq.as<float>(), nr, false, rowMask, rD.as<float>(), rI.as<idx_t>()).fallbacks;
+        tc_scatter_results_kernel<<<nr, 128, 0, stream>>>(rD.as<float>(), rI.as<idx_t>(), list.as<int>(), k, outD, outI);
+        CUDA_CHECK_LAST();
+        CUDA_VERIFY(cudaStreamSynchronize(stream));
+    }
+    return n;
+}
+
 // certificate failures -> exact SIMT recompute into outD / outI; returns their number
 int FlatTcDatabase::recomputeFallbacks(const Call& c, const Batch& b, const uint32_t* rowMask, float* outD, idx_t* outI) const {
     const int k = c.s.k;
-    const int64_t nq = b.nq;
     cudaStream_t stream = c.stream;
-    auto list = res_->temp(device_, sizeof(int) * nq);
-    int* countDev = b.flags.as<int>() + nq;
-    tc_collect_flags_kernel<<<(unsigned)ceil_div(nq, 256), 256, 0, stream>>>(b.flags.as<int>(), (int)nq, list.as<int>(), countDev);
-    CUDA_CHECK_LAST();
-    int nflag = 0;
-    CUDA_VERIFY(cudaMemcpyAsync(&nflag, countDev, sizeof(int), cudaMemcpyDeviceToHost, stream));
-    CUDA_VERIFY(cudaStreamSynchronize(stream));
+    GpuMemoryReservation list;
+    const int nflag = collectFlagged(c, b, kFlagExact, list);
     if (nflag > 0) {
         auto fq = res_->temp(device_, sizeof(float) * (size_t)nflag * d_);
         auto fD = res_->temp(device_, sizeof(float) * (size_t)nflag * k);
@@ -1451,9 +1506,44 @@ int FlatTcDatabase::recomputeFallbacks(const Call& c, const Batch& b, const uint
     return nflag;
 }
 
+FlatTcDatabase::Counts FlatTcDatabase::runBatch(const Call& c, const float* Q, int64_t nq, bool estimate,
+                                                const uint32_t* rowMask, float* outD, idx_t* outI) const {
+    Batch b;
+    b.Q = Q;
+    b.nq = nq;
+    b.qPairs = ceil_div(nq, kUnitM);
+    prepareQueries(c, b);
+    const FlatTcRounds plan = c.s.rounds(b.qPairs);
+    auto arena = res_->temp(device_, plan.arenaBytes);
+    auto counts = res_->temp(device_, plan.countBytes);
+    GpuMemoryReservation contrib;
+    if (c.shard)
+        contrib = res_->temp(device_, sizeof(float) * 2 * nq);
+    bool estimated = false; // an earlier round's threshold was estimated: the last round's selection checks it
+    for (size_t i = 0; i < plan.rounds.size(); i++) {
+        const FlatTcRound& r = plan.rounds[i];
+        const int estRank = estimate ? r.estRank : 0;
+        runRound(c, b, r, estRank, estimated && i + 1 == plan.rounds.size(), arena.as<uint2>(), counts.as<int>(),
+                 contrib.as<float>(), outD, outI);
+        estimated = estimated || estRank > 0;
+    }
+    if (!c.s.streaming)
+        rerank(c, b, outD, outI);
+    Counts n;
+    if (estimated)
+        n = repairEstimates(c, b, rowMask, outD, outI);
+    n.fallbacks += recomputeFallbacks(c, b, rowMask, outD, outI);
+    return n;
+}
+
+// a batch that repairs more than 1 / kRepairShare of its queries (a database whose nearest rows crowd into few tiles)
+// leaves the call's later batches to provable thresholds
+constexpr int64_t kRepairShare = 32;
+
 int64_t FlatTcDatabase::search(const float* Q, int64_t nqAll, int k, float* outD, idx_t* outI, cudaStream_t stream,
                                const FlatTcShard* shard, const uint32_t* rowMask) {
     FB_THROW_IF_NOT_MSG(!dirty_, "FlatTcDatabase::search before prepare");
+    lastRepairs_ = 0;
     if (nqAll == 0)
         return 0;
     FB_THROW_IF_NOT(flatTcSupported(d_, k, n_));
@@ -1489,25 +1579,14 @@ int64_t FlatTcDatabase::search(const float* Q, int64_t nqAll, int k, float* outD
     const CUtensorMap mapY = makeTileMap(L.rows.data(), L.bits, n_, L.kBlocks, sp.boxRows, sp.ksplit ? 1 : L.kBlocks);
     const Call c{stream, s, KB, kSteps, sp, L, bias, tileBias, mapY, shard};
     int64_t fallbacks = 0;
+    bool estimate = true;
     for (int64_t qb = 0; qb < nqAll; qb += s.qBatch) {
-        Batch b;
-        b.Q = Q + qb * d_;
-        b.nq = std::min(s.qBatch, nqAll - qb);
-        b.qPairs = ceil_div(b.nq, kUnitM);
-        prepareQueries(c, b);
-        const FlatTcRounds plan = s.rounds(b.qPairs);
-        auto arena = res_->temp(device_, plan.arenaBytes);
-        auto counts = res_->temp(device_, plan.countBytes);
-        GpuMemoryReservation contrib;
-        if (shard)
-            contrib = res_->temp(device_, sizeof(float) * 2 * b.nq);
-        float* oD = outD + qb * k;
-        idx_t* oI = outI + qb * k;
-        for (const FlatTcRound& r : plan.rounds)
-            runRound(c, b, r, arena.as<uint2>(), counts.as<int>(), contrib.as<float>(), oD, oI);
-        if (!s.streaming)
-            rerank(c, b, oD, oI);
-        fallbacks += recomputeFallbacks(c, b, rowMask, oD, oI);
+        const int64_t nq = std::min(s.qBatch, nqAll - qb);
+        const Counts n = runBatch(c, Q + qb * d_, nq, estimate, rowMask, outD + qb * k, outI + qb * k);
+        fallbacks += n.fallbacks;
+        lastRepairs_ += n.repairs;
+        if (n.repairs * kRepairShare > nq)
+            estimate = false;
     }
     return fallbacks;
 }

@@ -50,6 +50,11 @@ class FlatTcDatabase {
     int lastOperandBits() const {
         return last_->bits;
     }
+    // queries of the last search searched again with provable thresholds because the estimated ones overshot
+    // (DESIGN.md 3.1); they are not among the queries search() returns as recomputed exactly
+    int64_t lastRepairedQueries() const {
+        return lastRepairs_;
+    }
 
    private:
     // one layout, in stored order: rows [n][kBlocks * 128 bytes], bias [round_up(n, 256) + 256] (-inf past n),
@@ -68,10 +73,19 @@ class FlatTcDatabase {
     // the launch steps of search(), in order
     struct Call;  // one search call
     struct Batch; // one query batch of it
+    struct Counts {
+        int64_t fallbacks = 0, repairs = 0;
+    };
+    // one batch of nq queries: its rounds (with estimated thresholds when `estimate`), the re-rank, the repairs and
+    // the exact recomputes
+    Counts runBatch(const Call& c, const float* Q, int64_t nq, bool estimate, const uint32_t* rowMask, float* outD,
+                    idx_t* outI) const;
     void prepareQueries(const Call& c, Batch& b) const;
-    void runRound(const Call& c, const Batch& b, const tc::FlatTcRound& r, uint2* arena, int* counts, float* contrib,
-                  float* outD, idx_t* outI) const;
+    void runRound(const Call& c, const Batch& b, const tc::FlatTcRound& r, int estRank, bool check, uint2* arena,
+                  int* counts, float* contrib, float* outD, idx_t* outI) const;
     void rerank(const Call& c, const Batch& b, float* outD, idx_t* outI) const;
+    int collectFlagged(const Call& c, const Batch& b, int flag, GpuMemoryReservation& list) const;
+    Counts repairEstimates(const Call& c, const Batch& b, const uint32_t* rowMask, float* outD, idx_t* outI) const;
     int recomputeFallbacks(const Call& c, const Batch& b, const uint32_t* rowMask, float* outD, idx_t* outI) const;
     void prepareFp16(cudaStream_t stream);
     void prepareInt8(cudaStream_t stream);
@@ -84,6 +98,7 @@ class FlatTcDatabase {
     int d_, dpad_;
     Layout fp16_, int8_;
     const Layout* last_ = &fp16_; // the last search's layout
+    int64_t lastRepairs_ = 0;
     // fp16 certificate
     float scale_ = 1.f;
     float maxNorm_ = 0.f;

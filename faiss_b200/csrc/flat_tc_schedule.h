@@ -5,6 +5,7 @@
 #pragma once
 
 #include <algorithm>
+#include <cmath>
 #include <cstddef>
 #include <cstdint>
 #include <numeric>
@@ -21,10 +22,48 @@ constexpr int kSegsPerUnit = kUnitM * kParts; // candidate segments of a work un
 constexpr int kSelCap = 1536;
 
 // one round of the geometric schedule: positions [begin, end) of the permuted tile order, split into `slices`
-// slices of `tilesPerSlice` tiles; `cap` candidates per segment
+// slices of `tilesPerSlice` tiles; `cap` candidates per segment.  estRank: the selection that closes the round sets
+// the next round's threshold from the estRank-th best approximate score seen so far as well as from the k-th (0: the
+// k-th alone, the provable threshold; see flatTcEstRank)
 struct FlatTcRound {
     int begin, end, slices, tilesPerSlice, cap;
+    int estRank = 0;
 };
+
+// Estimated thresholds (DESIGN.md 3.1).  After the tiles at positions [0, seen) a threshold s_j(seen) - 2 eps with
+// j < k is at most the final s_k - 2 eps unless the seen tiles hold >= j of the query's top-k rows.  The tile
+// permutation does not depend on the query, so the seen tiles are modelled as `seen` tiles drawn uniformly from T.
+// Rows of a norm-sorted tile are alike in norm, so a query's top-k rows can share tiles: the rule takes them in pairs,
+// k/2 tiles of two rows each, which doubles the variance of the count against rows in distinct tiles.  The count is
+// then X = 2 Y with Y ~ Hypergeometric(T, ceil(k / 2), seen), and j is the smallest rank with P(X >= j) <= delta.
+// A query whose estimate overshoots anyway (its top-k rows clustered more tightly) fails the check of the last round
+// and is searched again with provable thresholds: the estimate decides the time a query takes, never its result.
+constexpr double kEstMissBudget = 1e-4; // per query and search, split evenly over the rounds that estimate
+constexpr int kEstClump = 2;            // top-k rows per shared tile in the rule's model
+
+// the rank j of the estimated threshold after `seen` of T tiles, for a per-round miss probability delta; 0 when no
+// j < k meets it
+inline int flatTcEstRank(int64_t T, int k, int64_t seen, double delta) {
+    const int64_t K = (k + kEstClump - 1) / kEstClump, n = std::min(seen, T);
+    if (K >= T) // a pair in every tile: any sample holds top-k rows
+        return 0;
+    auto lchoose = [](int64_t a, int64_t b) {
+        return std::lgamma((double)a + 1) - std::lgamma((double)b + 1) - std::lgamma((double)(a - b) + 1);
+    };
+    // P(Y = y) = C(K, y) C(T - K, n - y) / C(T, n); walk the tail down from its far end until it exceeds delta:
+    // P(Y >= y + 1) <= delta < P(Y >= y)
+    const double lden = lchoose(T, n);
+    double tail = 0;
+    int64_t y = std::min(K, n);
+    for (; y >= 1; y--) {
+        if (n - y <= T - K)
+            tail += std::exp(lchoose(K, y) + lchoose(T - K, n - y) - lden);
+        if (tail > delta)
+            break;
+    }
+    const int64_t j = (int64_t)kEstClump * y + 1; // X = 2 Y >= j  <=>  Y >= y + 1
+    return j < k ? (int)j : 0;
+}
 
 // the rounds of one query batch and the scratch they need
 struct FlatTcRounds {
@@ -103,6 +142,12 @@ struct FlatTcSchedule {
             out.countBytes = std::max(out.countBytes, segs * sizeof(int));
             seen = end;
         }
+        // estimated thresholds: unsharded (pooled thresholds are certified across ranks) and in rounds; the last round's
+        // selection sets the final, provable threshold and checks the estimates against it
+        const int nEst = (int)out.rounds.size() - 1;
+        if (nShards == 1 && !streaming)
+            for (int i = 0; i < nEst; i++)
+                out.rounds[i].estRank = flatTcEstRank(T, k, out.rounds[i].end, kEstMissBudget / nEst);
         return out;
     }
 };

@@ -564,8 +564,10 @@ void GpuIndexFlat::searchCompacted_(
 
 void GpuIndexFlat::searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const SearchCall& call) const {
     auto stream = stream_();
-    if (call.row0 == 0)
+    if (call.row0 == 0) {
         lastSearchFallbackQueries = 0;
+        lastSearchRepairedQueries = 0;
+    }
     lastSearchUsedTensorCores = 0;
     lastSearchOperandBits = 0;
     if (this->ntotal == 0) {
@@ -601,9 +603,12 @@ void GpuIndexFlat::searchTc_(idx_t n, const float* xDev, int k, float* dDev, idx
     tc_.prepare(rows_(), this->ntotal, searchMetric_(), yHalf_(), stream);
     GpuMemoryReservation qHold;
     xDev = roundedQueries_(n, xDev, qHold);
-    if (row0 == 0)
+    if (row0 == 0) {
         lastSearchFallbackQueries = 0;
+        lastSearchRepairedQueries = 0;
+    }
     lastSearchFallbackQueries += (int)tc_.search(xDev, n, k, dDev, iDev, stream, shard, mask);
+    lastSearchRepairedQueries += (int)tc_.lastRepairedQueries();
     lastSearchUsedTensorCores = 1;
     lastSearchOperandBits = tc_.lastOperandBits();
 }

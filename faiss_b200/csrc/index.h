@@ -240,6 +240,8 @@ class GpuIndexFlat : public GpuIndex {
     mutable int lastSearchUsedTensorCores = 0;
     mutable int lastSearchFallbackQueries = 0;
     mutable int lastSearchOperandBits = 0; // tensor-core operand width of the last search: 8 or 16; 0: exact kernel
+    // queries searched again with provable thresholds because their estimated ones overshot (summed over the call)
+    mutable int lastSearchRepairedQueries = 0;
 
    protected:
     bool addImplRequiresIDs_() const override {

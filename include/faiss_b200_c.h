@@ -126,6 +126,9 @@ FB200_API int faiss_GpuIndexFlat_setUseTensorCores(FaissGpuIndex* index, int ena
 FB200_API int faiss_GpuIndexFlat_lastSearchInfo(const FaissGpuIndex* index, int* out2);
 /* operand width of the last search's tensor-core scoring: 8 (int8), 16 (fp16), or 0 when it ran the exact kernel */
 FB200_API int faiss_GpuIndexFlat_lastSearchOperandBits(const FaissGpuIndex* index, int* bits);
+/* queries of the last search searched again with provable thresholds because their estimated thresholds overshot
+   (not exact-kernel recomputes: lastSearchInfo does not count them) */
+FB200_API int faiss_GpuIndexFlat_lastSearchRepairedQueries(const FaissGpuIndex* index, int* count);
 
 /* ---- GpuIndexIVF (faiss/gpu/GpuIndexIVF.h:40-167) ---- */
 FB200_API int faiss_GpuIndexIVF_set_nprobe(FaissGpuIndex* index, size_t nprobe);
