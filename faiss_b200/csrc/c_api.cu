@@ -1686,7 +1686,16 @@ int b200_ivfflat_scan(
         auto res = RES(r);
         DeviceScope s(device);
         FB_THROW_IF_NOT(k >= 1 && k <= kMaxK && nprobe >= 1 && nprobe <= kMaxNprobe);
-        runIvfFlatScan(res.get(), device, Q, nq, d, probes, nprobe, list_start, list_len, arena_vecs, arena_ids, arena_elems, k, MT_L2IP(metric), D, I, res->getDefaultStream(device));
+        IvfScanLayout a;
+        a.kind = IVF_STORED_FLAT;
+        a.d = d;
+        a.listStart = list_start;
+        a.listLen = list_len;
+        a.arenaElems = arena_elems;
+        a.codes = reinterpret_cast<const uint8_t*>(arena_vecs);
+        a.ids = arena_ids;
+        const IvfScanCall c{Q, nq, probes, nullptr, nprobe, k, MT_L2IP(metric), D, I, res->getDefaultStream(device)};
+        runIvfScan(res.get(), device, a, c);
     }
     CATCH_AND_HANDLE
 }
@@ -1716,7 +1725,19 @@ int b200_ivfpq_scan(
         auto res = RES(r);
         DeviceScope s(device);
         FB_THROW_IF_NOT(k >= 1 && k <= kMaxK && nprobe >= 1 && nprobe <= kMaxNprobe);
-        runIvfPqScan(res.get(), device, Q, nq, d, probes, coarse_dis, nprobe, coarse_centroids, pq_centroids, M, 8, list_start, list_len, arena_codes, arena_ids, k, MT_L2IP(metric), D, I, res->getDefaultStream(device));
+        IvfScanLayout a;
+        a.kind = IVF_STORED_PQ;
+        a.d = d;
+        a.listStart = list_start;
+        a.listLen = list_len;
+        a.codes = arena_codes;
+        a.ids = arena_ids;
+        a.centroids = coarse_centroids;
+        a.M = M;
+        a.nbits = 8;
+        a.pq = pq_centroids;
+        const IvfScanCall c{Q, nq, probes, coarse_dis, nprobe, k, MT_L2IP(metric), D, I, res->getDefaultStream(device)};
+        runIvfScan(res.get(), device, a, c);
     }
     CATCH_AND_HANDLE
 }

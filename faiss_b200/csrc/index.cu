@@ -1047,6 +1047,20 @@ IvfLists::~IvfLists() {
         res_->deallocMemory(device_, ids_);
 }
 
+IvfScanLayout IvfLists::layout(int d) const {
+    IvfScanLayout a;
+    a.d = d;
+    a.codeSize = codeSize_;
+    a.interleaved = interleaved_;
+    a.listStart = dStart_;
+    a.listLen = dLen_;
+    a.nlist = nlist_;
+    a.arenaElems = arenaElems_;
+    a.codes = codes_;
+    a.ids = ids_;
+    return a;
+}
+
 void IvfLists::uploadMeta_(cudaStream_t stream) {
     CUDA_VERIFY(cudaMemcpyAsync(dStart_, hStart_.data(), sizeof(int64_t) * nlist_, cudaMemcpyHostToDevice, stream));
     CUDA_VERIFY(cudaMemcpyAsync(dLen_, hLen_.data(), sizeof(int) * nlist_, cudaMemcpyHostToDevice, stream));
@@ -1476,21 +1490,21 @@ void GpuIndexIVF::search_preassigned(
     CUDA_VERIFY(cudaStreamSynchronize(stream));
 }
 
-// ---- retrieval: ids -> arena slots -> decoded entries (ivf_reconstruct.cu)
-IvfStoredLayout GpuIndexIVF::listLayout_() const {
-    IvfStoredLayout a;
-    a.d = d;
-    a.codeSize = lists_->codeSize();
-    a.interleaved = lists_->interleaved();
-    a.listStart = lists_->dStart();
-    a.listLen = lists_->dLen();
-    a.nlist = nlist;
-    a.arenaElems = lists_->arenaElems();
-    a.codes = lists_->codes();
-    a.ids = lists_->ids();
-    return a;
+void GpuIndexIVF::scanImpl_(
+        idx_t n,
+        const float* xDev,
+        const idx_t* probes,
+        const float* coarseDis,
+        int np,
+        int k,
+        float* dDev,
+        idx_t* iDev,
+        const SearchCall& call) const {
+    const IvfScanCall c{xDev, n, probes, coarseDis, np, k, metric_type, dDev, iDev, stream_(), call.mask, call.slots};
+    runIvfScan(resources_.get(), config_.device, scanLayout_(), c);
 }
 
+// ---- retrieval: ids -> arena slots -> decoded entries (ivf_reconstruct.cu)
 int GpuIndexIVF::coarse_code_size() const {
     int nbyte = 0;
     for (idx_t nl = nlist - 1; nl > 0; nl >>= 8)
@@ -1585,7 +1599,7 @@ void GpuIndexIVF::search_and_return_codes(
         idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, uint8_t* codes, bool include_listno,
         const SearchParameters* params) const {
     FB_THROW_IF_NOT_MSG(n == 0 || codes, "null pointer passed to search_and_return_codes");
-    const IvfStoredLayout a = listLayout_();
+    const IvfStoredLayout a = lists_->layout(d);
     const int listnoBytes = include_listno ? coarse_code_size() : 0;
     const size_t rowBytes = (size_t)listnoBytes + a.codeSize;
     searchWithSlots_(n, x, k, distances, labels, params, rowBytes, [&](idx_t i0, idx_t nb, const idx_t* slots) {
@@ -1623,24 +1637,8 @@ const uint8_t* GpuIndexIVFFlat::encode_(idx_t, const float* xDev, const idx_t*, 
     return reinterpret_cast<const uint8_t*>(xDev);
 }
 
-void GpuIndexIVFFlat::scanImpl_(
-        idx_t n,
-        const float* xDev,
-        const idx_t* probes,
-        const float*,
-        int np,
-        int k,
-        float* dDev,
-        idx_t* iDev,
-        const SearchCall& call) const {
-    runIvfFlatScan(
-            resources_.get(), config_.device, xDev, n, d, probes, np, lists_->dStart(), lists_->dLen(),
-            reinterpret_cast<const float*>(lists_->codes()), scanIds_(call), lists_->arenaElems(), k, metric_type, dDev,
-            iDev, stream_(), call.mask, call.slots);
-}
-
-IvfStoredLayout GpuIndexIVFFlat::storedLayout_() const {
-    IvfStoredLayout a = listLayout_();
+IvfScanLayout GpuIndexIVFFlat::storedLayout_() const {
+    IvfScanLayout a = lists_->layout(d);
     a.kind = IVF_STORED_FLAT;
     return a;
 }
@@ -1853,40 +1851,26 @@ const uint8_t* GpuIndexIVFPQ::encode_(idx_t n, const float* xDev, const idx_t* a
     return hold.as<uint8_t>();
 }
 
-void GpuIndexIVFPQ::scanImpl_(
-        idx_t n,
-        const float* xDev,
-        const idx_t* probes,
-        const float* coarseDis,
-        int np,
-        int k,
-        float* dDev,
-        idx_t* iDev,
-        const SearchCall& call) const {
-    FB_THROW_IF_NOT_MSG(pqCentroids_.size() > 0, "PQ not trained");
-    if (lists_->interleaved()) {
-        runIvfPqScanInterleaved(
-                resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np, quantizer->vectorsDevice(),
-                pqCentroidsT_.data(), precomputedActive_() ? (ensureTerm2_(), term2_.data()) : nullptr,
-                lists_->codeSize(), nibbleLayout_(), lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(call),
-                lists_->arenaElems(), k, metric_type, dDev, iDev, stream_(), call.mask, call.slots);
-        return;
-    }
-    runIvfPqScan(
-            resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np, quantizer->vectorsDevice(),
-            pqCentroids_.data(), M_, nbits_, lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(call), k,
-            metric_type, dDev, iDev, stream_(), call.mask, call.slots);
-}
-
 // IndexIVFPQ::reconstruct_from_offset (faiss/IndexIVFPQ.cpp:358-372): pq.decode, then + the list's centroid
-IvfStoredLayout GpuIndexIVFPQ::storedLayout_() const {
+IvfScanLayout GpuIndexIVFPQ::storedLayout_() const {
     FB_THROW_IF_NOT_MSG(pqCentroids_.size() > 0, "PQ not trained");
-    IvfStoredLayout a = listLayout_();
+    IvfScanLayout a = lists_->layout(d);
     a.kind = IVF_STORED_PQ;
     a.M = M_;
     a.nbits = nbits_;
     a.pq = pqCentroids_.data();
     a.centroids = quantizer->vectorsDevice();
+    a.pqT = pqCentroidsT_.data();
+    return a;
+}
+
+// the term-2 table is built by the scans alone: decoding never allocates it
+IvfScanLayout GpuIndexIVFPQ::scanLayout_() const {
+    IvfScanLayout a = storedLayout_();
+    if (precomputedActive_()) {
+        ensureTerm2_();
+        a.term2 = term2_.data();
+    }
     return a;
 }
 
@@ -1898,6 +1882,35 @@ static bool sqTypeSupported(int qtype) { // faiss/gpu/impl/GpuScalarQuantizer.cu
 }
 static bool sqUniform(int qtype) {
     return qtype == SQ_QT_8bit_uniform || qtype == SQ_QT_4bit_uniform;
+}
+// the code layout (codec of ivf_layout.cuh) of a quantiser type
+static int sqCodec(int qtype) {
+    switch (qtype) {
+        case SQ_QT_4bit:
+        case SQ_QT_4bit_uniform:
+            return SQC_NIBBLE;
+        case SQ_QT_6bit:
+            return SQC_SIX;
+        case SQ_QT_fp16:
+            return SQC_HALF;
+        default:
+            return SQC_BYTE;
+    }
+}
+// the decode's divisor s in x = vmin + (c + 0.5) / s * vdiff; 0 for the types whose code is the value (fp16, direct)
+static float sqLevels(int qtype) {
+    switch (qtype) {
+        case SQ_QT_fp16:
+        case SQ_QT_8bit_direct:
+            return 0.f;
+        case SQ_QT_4bit:
+        case SQ_QT_4bit_uniform:
+            return 15.f;
+        case SQ_QT_6bit:
+            return 63.f;
+        default:
+            return 255.f;
+    }
 }
 
 int GpuIndexIVFScalarQuantizer::codeSizeFor(int qtype, int d) {
@@ -1976,7 +1989,7 @@ void GpuIndexIVFScalarQuantizer::setTrained(const float* t, size_t n) {
     float* vdiff = vmin + d;
     float* m = vdiff + d;
     float* b = m + d;
-    const float levels = (qtype_ == SQ_QT_4bit || qtype_ == SQ_QT_4bit_uniform) ? 15.f : qtype_ == SQ_QT_6bit ? 63.f : 255.f;
+    const float levels = sqLevels(qtype_);
     for (int i = 0; i < d; i++) {
         if (n == 0) { // fp16, 8bit_direct: the code is the value
             vmin[i] = 0.f;
@@ -2066,36 +2079,17 @@ const uint8_t* GpuIndexIVFScalarQuantizer::encode_(
     return hold.as<uint8_t>();
 }
 
-void GpuIndexIVFScalarQuantizer::scanImpl_(
-        idx_t n,
-        const float* xDev,
-        const idx_t* probes,
-        const float* coarseDis,
-        int np,
-        int k,
-        float* dDev,
-        idx_t* iDev,
-        const SearchCall& call) const {
-    FB_THROW_IF_NOT_MSG(params_.size() == (size_t)4 * d, "scalar quantizer not trained");
-    const bool needCentroids = by_residual && metric_type == METRIC_L2;
-    runIvfSqScan(
-            resources_.get(), config_.device, xDev, n, d, probes, coarseDis, np,
-            needCentroids ? quantizer->vectorsDevice() : nullptr, by_residual, qtype_, params_.data() + 2 * d,
-            lists_->dStart(), lists_->dLen(), lists_->codes(), scanIds_(call), lists_->arenaElems(), lists_->codeSize(), k,
-            metric_type, dDev, iDev, stream_(), call.mask, call.slots);
-}
-
 // IndexIVFScalarQuantizer::reconstruct_from_offset (faiss/IndexScalarQuantizer.cpp:400-425): sq.decode, then + the
 // list's centroid when by_residual
-IvfStoredLayout GpuIndexIVFScalarQuantizer::storedLayout_() const {
+IvfScanLayout GpuIndexIVFScalarQuantizer::storedLayout_() const {
     FB_THROW_IF_NOT_MSG(params_.size() == (size_t)4 * d, "scalar quantizer not trained");
-    IvfStoredLayout a = listLayout_();
+    IvfScanLayout a = lists_->layout(d);
     a.kind = IVF_STORED_SQ;
-    const bool nibble = qtype_ == SQ_QT_4bit || qtype_ == SQ_QT_4bit_uniform;
-    a.sqCodec = nibble ? SQC_NIBBLE : qtype_ == SQ_QT_6bit ? SQC_SIX : qtype_ == SQ_QT_fp16 ? SQC_HALF : SQC_BYTE;
-    a.levels = qtype_ == SQ_QT_fp16 || qtype_ == SQ_QT_8bit_direct ? 0.f : nibble ? 15.f : qtype_ == SQ_QT_6bit ? 63.f : 255.f;
+    a.sqCodec = sqCodec(qtype_);
+    a.levels = sqLevels(qtype_);
     a.vmin = params_.data();
     a.vdiff = params_.data() + d;
+    a.sqDecodeMB = params_.data() + 2 * d;
     a.centroids = by_residual ? quantizer->vectorsDevice() : nullptr;
     return a;
 }

@@ -415,6 +415,8 @@ class IvfLists {
     bool interleaved() const {
         return interleaved_;
     }
+    // the lists of d-dimensional entries as the decoders and scans see them, before the index adds its format
+    IvfScanLayout layout(int d) const;
 
    private:
     void relayout_(const std::vector<int64_t>& newCap, cudaStream_t stream);
@@ -523,9 +525,12 @@ class GpuIndexIVF : public GpuIndex {
     }
 
    protected:
-    // the decoder's view of this index's lists
-    virtual IvfStoredLayout storedLayout_() const = 0;
-    IvfStoredLayout listLayout_() const;
+    // this index's lists as the decoders (the IvfStoredLayout part) and the scans read them; builds nothing
+    virtual IvfScanLayout storedLayout_() const = 0;
+    // the scans' view: storedLayout_() and the scan tables that are built on first use
+    virtual IvfScanLayout scanLayout_() const {
+        return storedLayout_();
+    }
     idx_t retrievalPageRows_(const float* out, idx_t n) const;
     // search with the slot of every result: per page of queries, `page(i0, nb, slotsDev)` runs after D / I of the
     // page are on the device (slotsDev [nb][k], -1 with a missing result); resultBytes (the page's output per result)
@@ -533,11 +538,6 @@ class GpuIndexIVF : public GpuIndex {
     void searchWithSlots_(
             idx_t n, const float* x, idx_t k, float* distances, idx_t* labels, const SearchParameters* params,
             size_t resultBytes, const std::function<void(idx_t, idx_t, const idx_t*)>& page) const;
-    // the id table the scans read: the slot search's identity table, else the list ids
-    const idx_t* scanIds_(const SearchCall& call) const {
-        return call.slots ? call.slots->identity : lists_->ids();
-    }
-
     bool addImplRequiresIDs_() const override {
         return true;
     }
@@ -558,7 +558,8 @@ class GpuIndexIVF : public GpuIndex {
     GpuMemoryReservation coarseResiduals_(idx_t n, const float* xDev, const idx_t* assignDev) const;
     void searchImpl_(idx_t n, const float* xDev, int k, float* dDev, idx_t* iDev, const SearchCall& call) const override;
     GpuMemoryReservation selMask_(const IDSelector& sel, idx_t& selected) const override; // slot = arena position, id = stored id
-    virtual void scanImpl_(
+    // runIvfScan over scanLayout_() with the call's selector mask and slots
+    void scanImpl_(
             idx_t n,
             const float* xDev,
             const idx_t* probesDev,
@@ -567,7 +568,7 @@ class GpuIndexIVF : public GpuIndex {
             int k,
             float* dDev,
             idx_t* iDev,
-            const SearchCall& call) const = 0;
+            const SearchCall& call) const;
 
     GpuIndexIVFConfig ivfConfig_;
     std::unique_ptr<IvfLists> lists_;
@@ -592,8 +593,7 @@ class GpuIndexIVFFlat : public GpuIndexIVF {
 
    protected:
     const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
-    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*, const SearchCall&) const override;
-    IvfStoredLayout storedLayout_() const override;
+    IvfScanLayout storedLayout_() const override;
 };
 
 struct GpuIndexIVFPQConfig : GpuIndexIVFConfig { // faiss/gpu/GpuIndexIVFPQ.h:25-49
@@ -663,16 +663,12 @@ class GpuIndexIVFPQ : public GpuIndexIVF {
     }
     void trainEncoder_(idx_t n, const float* xDev) override; // the PQ, on residuals
     const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
-    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*, const SearchCall&) const override;
-    IvfStoredLayout storedLayout_() const override;
+    IvfScanLayout storedLayout_() const override;
+    IvfScanLayout scanLayout_() const override; // + the precomputed term-2 table when precomputedActive_()
 
     int M_, nbits_;
     int ksub_() const {
         return 1 << nbits_;
-    }
-    // 4-bit codes stored as M/2 nibble-pair bytes in the interleaved layout
-    bool nibbleLayout_() const {
-        return nbits_ == 4 && lists_->interleaved();
     }
     bool precomputedActive_() const;
     void ensureTerm2_() const;
@@ -736,8 +732,7 @@ class GpuIndexIVFScalarQuantizer : public GpuIndexIVF {
     }
     void trainEncoder_(idx_t n, const float* xDev) override; // the RS_minmax ranges
     const uint8_t* encode_(idx_t n, const float* xDev, const idx_t* assignDev, GpuMemoryReservation& hold) override;
-    void scanImpl_(idx_t, const float*, const idx_t*, const float*, int, int, float*, idx_t*, const SearchCall&) const override;
-    IvfStoredLayout storedLayout_() const override;
+    IvfScanLayout storedLayout_() const override;
 
     int qtype_;
     std::vector<float> trained_;

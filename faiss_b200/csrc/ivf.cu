@@ -471,21 +471,16 @@ int ivfScanChunks(int device, int64_t nq, int nprobe, int* probesPerCta) {
 void runIvfScanBatches(
         GpuResources* res,
         int device,
-        int64_t nq,
-        int nprobe,
-        int k,
-        MetricType metric,
+        const IvfScanCall& call,
         bool oneProbePerCta,
         const char* timingName,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const std::function<void(const IvfScanBatch&)>& launch,
-        const IvfSlotOutput* slots) {
+        const std::function<void(const IvfScanBatch&)>& launch) {
+    const int64_t nq = call.nq;
+    const int k = call.k;
     if (nq == 0)
         return;
     int probesPerCta = 1;
-    const int ctasPerQuery = oneProbePerCta ? nprobe : ivfScanChunks(device, nq, nprobe, &probesPerCta);
+    const int ctasPerQuery = oneProbePerCta ? call.nprobe : ivfScanChunks(device, nq, call.nprobe, &probesPerCta);
     // query batches bound the partial-result scratch
     const int64_t maxQ =
             std::max<int64_t>(1, std::min<int64_t>(65535, (int64_t(1) << 30) / ((int64_t)ctasPerQuery * k * 12)));
@@ -495,61 +490,41 @@ void runIvfScanBatches(
         auto partI = res->temp(device, sizeof(idx_t) * nb * ctasPerQuery * k);
         const IvfScanBatch batch{
                 q0, nb, dim3((unsigned)ctasPerQuery, (unsigned)nb), probesPerCta, partD.as<float>(), partI.as<idx_t>()};
-        KernelTiming::begin(timingName, stream);
+        KernelTiming::begin(timingName, call.stream);
         launch(batch);
-        KernelTiming::end(timingName, stream);
+        KernelTiming::end(timingName, call.stream);
         CUDA_CHECK_LAST();
-        if (slots)
+        if (call.slots)
             runIvfMergeTopKSlots(
-                    partD.as<float>(), partI.as<idx_t>(), slots->arenaIds, nb, ctasPerQuery, k, k, metric, outD + q0 * k,
-                    outI + q0 * k, slots->outSlot + q0 * k, stream);
+                    partD.as<float>(), partI.as<idx_t>(), call.slots->arenaIds, nb, ctasPerQuery, k, k, call.metric,
+                    call.outD + q0 * k, call.outI + q0 * k, call.slots->outSlot + q0 * k, call.stream);
         else
             runMergeTopKKeyspace(
-                    partD.as<float>(), partI.as<idx_t>(), nb, ctasPerQuery, k, k, metric, 0, outD + q0 * k, outI + q0 * k,
-                    stream);
+                    partD.as<float>(), partI.as<idx_t>(), nb, ctasPerQuery, k, k, call.metric, 0, call.outD + q0 * k,
+                    call.outI + q0 * k, call.stream);
     }
 }
 
-void runIvfFlatScan(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nq,
-        int d,
-        const idx_t* probes,
-        int nprobe,
-        const int64_t* listStart,
-        const int* listLen,
-        const float* arenaVecs,
-        const idx_t* arenaIds,
-        int64_t arenaElems,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const uint32_t* slotMask,
-        const IvfSlotOutput* slots) {
-    if (nq == 0)
-        return;
+static void runIvfFlatScan(GpuResources* res, int device, const IvfScanLayout& a, const IvfScanCall& c) {
+    const int d = a.d, k = c.k, nprobe = c.nprobe;
     const int LIST = std::max(64, next_pow2(k));
-    const bool wide = arenaElems >= (int64_t(1) << 31) - 1;
+    const bool wide = ivfScanWideIds(a);
     const size_t listBytes = wide ? SmemTopK<long long>::bytes(LIST, kScanBuf) : SmemTopK<int>::bytes(LIST, kScanBuf);
     size_t smem = round_up(sizeof(float) * d, 16) + listBytes * kScanWarps;
     FB_THROW_IF_NOT_MSG(smem <= 200 * 1024, "k / d too large for the IVF-Flat scan kernel");
-    runIvfScanBatches(res, device, nq, nprobe, k, metric, false, "ivfflat_scan", outD, outI, stream, [&](const IvfScanBatch& b) {
-        withBool(metric == METRIC_L2, [&](auto l2) {
+    runIvfScanBatches(res, device, c, false, "ivfflat_scan", [&](const IvfScanBatch& b) {
+        withBool(c.metric == METRIC_L2, [&](auto l2) {
             withBool(wide, [&](auto wideIds) {
-                withBool(slotMask != nullptr, [&](auto masked) {
+                withBool(c.mask != nullptr, [&](auto masked) {
                     auto kern = ivfflat_scan_kernel<l2, ScanIdT<decltype(wideIds)>, masked>;
                     CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                    kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
-                            Q + b.q0 * d, d, probes + b.q0 * nprobe, nprobe, b.probesPerCta, listStart, listLen,
-                            arenaVecs, arenaIds, k, LIST, b.partD, b.partI, slotMask);
+                    kern<<<b.grid, kScanWarps * 32, smem, c.stream>>>(
+                            c.Q + b.q0 * d, d, c.probes + b.q0 * nprobe, nprobe, b.probesPerCta, a.listStart, a.listLen,
+                            reinterpret_cast<const float*>(a.codes), a.ids, k, LIST, b.partD, b.partI, c.mask);
                 });
             });
         });
-    }, slots);
+    });
 }
 
 // ------------------------------------------------------------------------------------------
@@ -677,32 +652,9 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfpq_scan_kernel(
     block_merge_and_write(w, warp, lists, perWarp, LIST, k, arenaIds + listStart[l], add, oD, oI);
 }
 
-void runIvfPqScan(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nq,
-        int d,
-        const idx_t* probes,
-        const float* coarseDis,
-        int nprobe,
-        const float* coarseCentroids,
-        const float* pqCentroids,
-        int M,
-        int nbits,
-        const int64_t* listStart,
-        const int* listLen,
-        const uint8_t* arenaCodes,
-        const idx_t* arenaIds,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const uint32_t* slotMask,
-        const IvfSlotOutput* slots) {
-    if (nq == 0)
-        return;
+// vector-major codes: 8-bit, or the CPU's packed bitstring below 8 bits
+static void runIvfPqScan(GpuResources* res, int device, const IvfScanLayout& a, const IvfScanCall& c) {
+    const int d = a.d, k = c.k, nprobe = c.nprobe, M = a.M, nbits = a.nbits;
     FB_THROW_IF_NOT(nbits >= 1 && nbits <= 8);
     const int ksub = 1 << nbits;
     const bool packed = nbits != 8;
@@ -711,20 +663,36 @@ void runIvfPqScan(
     size_t smem = sizeof(float) * M * ksub + round_up(sizeof(float) * d, 16) +
             SmemTopK<int>::bytes(LIST, kScanBuf) * kScanWarps;
     FB_THROW_IF_NOT_MSG(smem <= 220 * 1024, "LUT + top-k lists do not fit shared memory (IVFPQ.cu:596-617)");
-    runIvfScanBatches(res, device, nq, nprobe, k, metric, true, name, outD, outI, stream, [&](const IvfScanBatch& b) {
-        withBool(metric == METRIC_L2, [&](auto l2) {
+    runIvfScanBatches(res, device, c, true, name, [&](const IvfScanBatch& b) {
+        withBool(c.metric == METRIC_L2, [&](auto l2) {
             withBool(packed, [&](auto pk) {
-                withBool(slotMask != nullptr, [&](auto masked) {
+                withBool(c.mask != nullptr, [&](auto masked) {
                     auto kern = ivfpq_scan_kernel<l2, pk, masked>;
                     CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                    kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
-                            Q + b.q0 * d, d, probes + b.q0 * nprobe, coarseDis + b.q0 * nprobe, nprobe, coarseCentroids,
-                            pqCentroids, M, ksub, listStart, listLen, arenaCodes, arenaIds, k, LIST, b.partD, b.partI,
-                            slotMask);
+                    kern<<<b.grid, kScanWarps * 32, smem, c.stream>>>(
+                            c.Q + b.q0 * d, d, c.probes + b.q0 * nprobe, c.coarseDis + b.q0 * nprobe, nprobe,
+                            a.centroids, a.pq, M, ksub, a.listStart, a.listLen, a.codes, a.ids, k, LIST, b.partD,
+                            b.partI, c.mask);
                 });
             });
         });
-    }, slots);
+    });
+}
+
+void runIvfScan(GpuResources* res, int device, const IvfScanLayout& lists, const IvfScanCall& call) {
+    if (call.nq == 0)
+        return;
+    IvfScanLayout a = lists;
+    if (call.slots) // the scan returns arena positions; the batch merge turns them into the stored ids
+        a.ids = call.slots->identity;
+    if (a.kind == IVF_STORED_FLAT)
+        runIvfFlatScan(res, device, a, call);
+    else if (a.kind == IVF_STORED_SQ)
+        runIvfSqScan(res, device, a, call);
+    else if (a.interleaved)
+        runIvfPqScanInterleaved(res, device, a, call);
+    else
+        runIvfPqScan(res, device, a, call);
 }
 
 } // namespace fb200

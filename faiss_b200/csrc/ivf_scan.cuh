@@ -26,25 +26,22 @@ struct IvfScanBatch {
     idx_t* partI;
 };
 
-// With `slots`, the launch writes arena positions (the scan reads slots->identity as its id table), merged by
-// runIvfMergeTopKSlots into outI and slots->outSlot.
-// Splits nq queries into batches that bound the partial-result scratch, calls `launch` once per batch (the
+// Splits call.nq queries into batches that bound the partial-result scratch, calls `launch` once per batch (the
 // scan kernel launch, bracketed by KernelTiming `timingName`) and merges each batch's partial results into
-// outD / outI [nq][k].  oneProbePerCta: one CTA per (query, probe); else the probes are split by ivfScanChunks.
+// call.outD / call.outI.  oneProbePerCta: one CTA per (query, probe); else the probes are split by ivfScanChunks.
+// With call.slots, the launch writes arena positions (the scan reads slots->identity as its id table), merged by
+// runIvfMergeTopKSlots into outI and slots->outSlot.
 void runIvfScanBatches(
         GpuResources* res,
         int device,
-        int64_t nq,
-        int nprobe,
-        int k,
-        MetricType metric,
+        const IvfScanCall& call,
         bool oneProbePerCta,
         const char* timingName,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const std::function<void(const IvfScanBatch&)>& launch,
-        const IvfSlotOutput* slots = nullptr);
+        const std::function<void(const IvfScanBatch&)>& launch);
+
+// the scans of runIvfScan that live in their own files; `lists.ids` is the id table the scan reads
+void runIvfPqScanInterleaved(GpuResources* res, int device, const IvfScanLayout& lists, const IvfScanCall& call);
+void runIvfSqScan(GpuResources* res, int device, const IvfScanLayout& lists, const IvfScanCall& call);
 
 // runtime value -> compile-time constant (see withBool): f(std::integral_constant<int, V>{}) for the V of Vs equal to v
 template <int... Vs, typename F>
@@ -65,6 +62,9 @@ __device__ __forceinline__ bool slotSelected(const uint32_t* __restrict__ mask, 
 // list ids of the scans' top-k lists: arena positions, 64-bit once they do not fit an int
 template <typename Wide>
 using ScanIdT = std::conditional_t<Wide::value, long long, int>;
+inline bool ivfScanWideIds(const IvfStoredLayout& lists) {
+    return lists.arenaElems >= (int64_t(1) << 31) - 1;
+}
 
 // ------------------------------------------------------------------------------------------
 // block-level helper: merge the per-warp lists of a block into warp 0's list, write k results

@@ -535,52 +535,30 @@ static int probedSmemBase(int device, cudaStream_t stream) {
     return (int)h;
 }
 
-void runIvfPqScanInterleaved(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nq,
-        int d,
-        const idx_t* probes,
-        const float* coarseDis,
-        int nprobe,
-        const float* coarseCentroids,
-        const float* pqCentroidsT,
-        const float* term2,
-        int M,
-        bool nibble,
-        const int64_t* listStart,
-        const int* listLen,
-        const uint8_t* arenaCodes,
-        const idx_t* arenaIds,
-        int64_t arenaElems,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const uint32_t* slotMask,
-        const IvfSlotOutput* slots) {
-    if (nq == 0)
-        return;
+// the interleaved layout's M template argument is the code's byte count: nibble-pair codes (4-bit PQ, M sub-quantisers
+// stored as M/2 bytes, byte j = code 2j | code 2j+1 << 4) are scanned as M/2 "8-bit" codes over the pair table
+// T'[j][b] = T[2j][b & 15] + T[2j+1][b >> 4], with pqT [16][M][dsub] and no precomputed tables
+void runIvfPqScanInterleaved(GpuResources* res, int device, const IvfScanLayout& a, const IvfScanCall& c) {
+    const int d = a.d, k = c.k, nprobe = c.nprobe, M = a.codeSize;
+    const bool nibble = a.nbits == 4;
     FB_THROW_IF_NOT(ivfPqInterleavedSupported(M));
-    FB_THROW_IF_NOT(!nibble || term2 == nullptr);
+    FB_THROW_IF_NOT(!nibble || a.term2 == nullptr);
     const int LIST = std::max(CtaTopK<int>::BUF, next_pow2(k)); // a sorted buffer (<= BUF entries) is merged into the list
-    const bool wide = arenaElems >= (int64_t(1) << 31) - 1; // arena positions need 64-bit list ids
-    const int smemBase = probedSmemBase(device, stream);
+    const bool wide = ivfScanWideIds(a); // arena positions need 64-bit list ids
+    const int smemBase = probedSmemBase(device, c.stream);
     const size_t listBytes = wide ? CtaTopK<long long>::bytes(LIST, kIlvScanWarps) : CtaTopK<int>::bytes(LIST, kIlvScanWarps);
     size_t smem = sizeof(float) * 256 * kLutSlots + round_up(sizeof(float) * 2 * d, 16) + 16 + listBytes +
             (nibble ? sizeof(float) * 2 * 16 * 2 * M : 0);
     FB_THROW_IF_NOT_MSG(smem <= 220 * 1024, "LUT + top-k lists do not fit shared memory");
-    const bool l2 = metric == METRIC_L2;
-    const bool pre = l2 && term2 != nullptr;
-    runIvfScanBatches(res, device, nq, nprobe, k, metric, false, "ivfpq_scan", outD, outI, stream, [&](const IvfScanBatch& b) {
+    const bool l2 = c.metric == METRIC_L2;
+    const bool pre = l2 && a.term2 != nullptr;
+    runIvfScanBatches(res, device, c, false, "ivfpq_scan", [&](const IvfScanBatch& b) {
         withInt<16, 32>(M, [&](auto m) {
             withBool(nibble, [&](auto nib) {
                 withBool(l2, [&](auto isL2) {
                     withBool(pre, [&](auto precomp) {
                         withBool(wide, [&](auto wideIds) {
-                            withBool(slotMask != nullptr, [&](auto masked) {
+                            withBool(c.mask != nullptr, [&](auto masked) {
                                 // precomputed tables are an L2 decomposition of 8-bit codes (pre implies l2 and !nibble)
                                 if constexpr (!precomp || (isL2 && !nib)) {
                                     using IdT = ScanIdT<decltype(wideIds)>;
@@ -589,10 +567,10 @@ void runIvfPqScanInterleaved(
                                             ? ivfpq_scan_interleaved_kernel<m, isL2, precomp, IdT, kExpectedSmemBase, nib, masked>
                                             : ivfpq_scan_interleaved_kernel<m, isL2, precomp, IdT, -1, nib, masked>;
                                     CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                                    kern<<<b.grid, kIlvScanWarps * 32, smem, stream>>>(
-                                            Q + b.q0 * d, d, probes + b.q0 * nprobe, coarseDis + b.q0 * nprobe, nprobe,
-                                            b.probesPerCta, coarseCentroids, pqCentroidsT, term2, listStart, listLen,
-                                            arenaCodes, arenaIds, k, LIST, b.partD, b.partI, slotMask);
+                                    kern<<<b.grid, kIlvScanWarps * 32, smem, c.stream>>>(
+                                            c.Q + b.q0 * d, d, c.probes + b.q0 * nprobe, c.coarseDis + b.q0 * nprobe,
+                                            nprobe, b.probesPerCta, a.centroids, a.pqT, a.term2, a.listStart, a.listLen,
+                                            a.codes, a.ids, k, LIST, b.partD, b.partI, c.mask);
                                 }
                             });
                         });
@@ -600,7 +578,7 @@ void runIvfPqScanInterleaved(
                 });
             });
         });
-    }, slots);
+    });
 }
 
 } // namespace fb200

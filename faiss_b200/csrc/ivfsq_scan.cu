@@ -359,81 +359,41 @@ __global__ void __launch_bounds__(kScanWarps * 32) ivfsq_scan_kernel(
     block_merge_and_write<IdT>(w, warp, lists, perWarp, LIST, k, arenaIds, 0.f, oD, oI);
 }
 
-static int sqCodec(int qtype) {
-    switch (qtype) {
-        case SQ_QT_4bit:
-        case SQ_QT_4bit_uniform:
-            return SQC_NIBBLE;
-        case SQ_QT_6bit:
-            return SQC_SIX;
-        case SQ_QT_fp16:
-            return SQC_HALF;
-        default:
-            return SQC_BYTE;
-    }
-}
-
 size_t ivfSqScanTableBytes(int d) {
     return round_up(sizeof(float) * (2 * d + kScanWarps), 16);
 }
 
-void runIvfSqScan(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nq,
-        int d,
-        const idx_t* probes,
-        const float* coarseDis,
-        int nprobe,
-        const float* coarseCentroids,
-        bool byResidual,
-        int qtype,
-        const float* decodeMB,
-        const int64_t* listStart,
-        const int* listLen,
-        const uint8_t* arenaCodes,
-        const idx_t* arenaIds,
-        int64_t arenaElems,
-        int codeSize,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const uint32_t* slotMask,
-        const IvfSlotOutput* slots) {
-    if (nq == 0)
-        return;
-    const int codec = sqCodec(qtype);
+void runIvfSqScan(GpuResources* res, int device, const IvfScanLayout& a, const IvfScanCall& c) {
+    const int d = a.d, k = c.k, nprobe = c.nprobe, codeSize = a.codeSize, codec = a.sqCodec;
     const int bits = codec == SQC_BYTE ? 8 : codec == SQC_NIBBLE ? 4 : codec == SQC_SIX ? 6 : 16;
     const int maxch = codec == SQC_HALF ? SqFast<SQC_HALF>::MAXCH : SqFast<SQC_BYTE>::MAXCH;
     const int fast = codec != SQC_SIX && (codeSize & 127) == 0 && (int64_t)d * bits == (int64_t)codeSize * 8 &&
             (codeSize >> 7) <= maxch;
     const int LIST = std::max(64, next_pow2(k));
-    const bool wide = arenaElems >= (int64_t(1) << 31) - 1;
+    const bool wide = ivfScanWideIds(a);
     const size_t listBytes = wide ? SmemTopK<long long>::bytes(LIST, kScanBuf) : SmemTopK<int>::bytes(LIST, kScanBuf);
     const size_t smem = ivfSqScanTableBytes(d) + listBytes * kScanWarps;
     FB_THROW_IF_NOT_MSG(smem <= 220 * 1024, "k / d too large for the IVF-SQ scan kernel");
-    const bool l2 = metric == METRIC_L2;
-    const float* coarse = (l2 && byResidual) ? coarseCentroids : nullptr;
-    const float* cdis = (!l2 && byResidual) ? coarseDis : nullptr;
-    runIvfScanBatches(res, device, nq, nprobe, k, metric, false, "ivfsq_scan", outD, outI, stream, [&](const IvfScanBatch& b) {
-        withInt<SQC_BYTE, SQC_NIBBLE, SQC_SIX, SQC_HALF>(codec, [&](auto c) {
+    // lists of residuals (centroids set): L2 scans q - c_list, IP adds the coarse distance
+    const bool l2 = c.metric == METRIC_L2;
+    const float* coarse = l2 ? a.centroids : nullptr;
+    const float* cdis = (!l2 && a.centroids) ? c.coarseDis : nullptr;
+    runIvfScanBatches(res, device, c, false, "ivfsq_scan", [&](const IvfScanBatch& b) {
+        withInt<SQC_BYTE, SQC_NIBBLE, SQC_SIX, SQC_HALF>(codec, [&](auto cc) {
             withBool(l2, [&](auto isL2) {
                 withBool(wide, [&](auto wideIds) {
-                    withBool(slotMask != nullptr, [&](auto masked) {
-                        auto kern = ivfsq_scan_kernel<c, isL2, ScanIdT<decltype(wideIds)>, masked>;
+                    withBool(c.mask != nullptr, [&](auto masked) {
+                        auto kern = ivfsq_scan_kernel<cc, isL2, ScanIdT<decltype(wideIds)>, masked>;
                         CUDA_VERIFY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                        kern<<<b.grid, kScanWarps * 32, smem, stream>>>(
-                                Q + b.q0 * d, d, probes + b.q0 * nprobe, cdis ? cdis + b.q0 * nprobe : nullptr, nprobe,
-                                b.probesPerCta, coarse, decodeMB, listStart, listLen, arenaCodes, arenaIds, codeSize,
-                                fast, k, LIST, b.partD, b.partI, slotMask);
+                        kern<<<b.grid, kScanWarps * 32, smem, c.stream>>>(
+                                c.Q + b.q0 * d, d, c.probes + b.q0 * nprobe, cdis ? cdis + b.q0 * nprobe : nullptr,
+                                nprobe, b.probesPerCta, coarse, a.sqDecodeMB, a.listStart, a.listLen, a.codes, a.ids,
+                                codeSize, fast, k, LIST, b.partD, b.partI, c.mask);
                     });
                 });
             });
         });
-    }, slots);
+    });
 }
 
 } // namespace fb200

@@ -9,8 +9,6 @@
 
 namespace fb200 {
 
-struct IvfSlotOutput; // ivf_reconstruct.cu section below
-
 // ---------------------------------------------------------------- flat_exact.cu
 // ||x||^2 per row (role of runL2Norm, faiss/gpu/impl/L2Norm.cu:176)
 void runL2Norms(const float* x, int64_t n, int d, float* norms, cudaStream_t stream);
@@ -218,62 +216,6 @@ void runIvfScatter(
         idx_t* arenaIds,
         cudaStream_t stream);
 
-// IVF-Flat list scan (role of runIVFInterleavedScan, faiss/gpu/impl/IVFInterleaved.cu:179).
-//   probes [nq,nprobe] list ids (-1 = skip), lists are row-major fp32 [len,d] inside the arena.
-void runIvfFlatScan(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nq,
-        int d,
-        const idx_t* probes,
-        int nprobe,
-        const int64_t* listStart,
-        const int* listLen,
-        const float* arenaVecs,
-        const idx_t* arenaIds,
-        int64_t arenaElems,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const uint32_t* slotMask = nullptr, // SearchParameters::sel over the arena, or null
-        const IvfSlotOutput* slots = nullptr); // the slot-keeping search, or null
-
-// IVF-PQ list scan (role of runPQScanMultiPassNoPrecomputed + pqCodeDistances,
-// faiss/gpu/impl/PQScanMultiPassNoPrecomputed-inl.cuh:527, PQCodeDistances-inl.cuh:591): the
-// per-(query,list) LUT is built in shared memory, codes are streamed with 128-bit loads, the
-// running top-k stays on chip.  Distance form follows the reference CPU scanner
-// (faiss/impl/pq_code_distance/IVFPQ_QueryTables.cpp:126-192): L2 by_residual:
-//   dis = sum_m || (q - c_list)_m - pq[m][code_m] ||^2 ; IP: q.c_list + sum_m q_m . pq[m][code_m]
-// nbits < 8: lists hold the CPU's packed bitstring, ceil(M*nbits/8) bytes per vector (kernel timing name
-// "ivfpq_scan_packed").
-void runIvfPqScan(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nq,
-        int d,
-        const idx_t* probes,
-        const float* coarseDis,
-        int nprobe,
-        const float* coarseCentroids /*[nlist,d]*/,
-        const float* pqCentroids /*[M][2^nbits][dsub]*/,
-        int M,
-        int nbits,
-        const int64_t* listStart,
-        const int* listLen,
-        const uint8_t* arenaCodes,
-        const idx_t* arenaIds,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const uint32_t* slotMask = nullptr, // SearchParameters::sel over the arena, or null
-        const IvfSlotOutput* slots = nullptr); // the slot-keeping search, or null
-
 // ---------------------------------------------------------------- ivf_reconstruct.cu
 // What a decoder needs to know about an IVF index's stored lists (all pointers on the device).  Every entry is
 // addressed by its arena slot; lists start in ascending list order, so a slot's list is found by bisection.
@@ -298,6 +240,13 @@ struct IvfStoredLayout {
     // PQ: codebooks [M][2^nbits][d / M], codes LSB-first bitstrings
     int M = 0, nbits = 8;
     const float* pq = nullptr;
+};
+// What the list scans read: the stored layout and the tables only the scans use.  They stay out of IvfStoredLayout,
+// which the decoder kernels take by value.
+struct IvfScanLayout : IvfStoredLayout {
+    const float* pqT = nullptr;   // PQ: the codebooks transposed to [2^nbits][M][d / M] (interleaved scan)
+    const float* term2 = nullptr; // PQ: the precomputed L2 table [nlist][256][M] of the interleaved 8-bit scan, or null
+    const float* sqDecodeMB = nullptr; // SQ: the scan's folded decode x = m + b * c, m[d] | b[d]
 };
 
 // out[i] = i: a table of arena slots the list scans read as their id table, so that they return positions
@@ -335,6 +284,37 @@ struct IvfSlotOutput {
     idx_t* outSlot; // [nq][k], beside outD / outI
 };
 
+// ---------------------------------------------------------------- ivf.cu: the list scans
+// One scan call (device pointers): queries Q [nq][d], their probes [nq][nprobe] (list ids, -1 = skip) and coarse
+// distances [nq][nprobe], results outD / outI [nq][k].
+struct IvfScanCall {
+    const float* Q = nullptr;
+    int64_t nq = 0;
+    const idx_t* probes = nullptr;
+    const float* coarseDis = nullptr;
+    int nprobe = 0;
+    int k = 0;
+    MetricType metric = METRIC_L2;
+    float* outD = nullptr;
+    idx_t* outI = nullptr;
+    cudaStream_t stream = nullptr;
+    const uint32_t* mask = nullptr;       // SearchParameters::sel over the arena, or null
+    const IvfSlotOutput* slots = nullptr; // the slot-keeping search, or null
+};
+
+// Scans the probed lists of `lists` and keeps the top k per query, with the scan of the lists' format:
+//   IVF-Flat: fp32 rows (role of runIVFInterleavedScan, faiss/gpu/impl/IVFInterleaved.cu:179);
+//   IVF-SQ: the decode folded into per-(query, probe) tables (role of the reference GPU IVFFlatScan with a
+//     scalar-quantiser codec); distance forms of faiss/impl/scalar_quantizer/scanners.h:44-135: L2 on the residual
+//     q - c_list when the lists hold residuals (centroids set), IP adds the coarse distance then;
+//   IVF-PQ: the per-(query, list) LUT built in shared memory, codes streamed, the running top-k on chip (role of
+//     runPQScanMultiPassNoPrecomputed + pqCodeDistances, PQScanMultiPassNoPrecomputed-inl.cuh:527,
+//     PQCodeDistances-inl.cuh:591), distance form of the CPU scanner (IVFPQ_QueryTables.cpp:126-192): L2
+//     sum_m || (q - c_list)_m - pq[m][code_m] ||^2, IP q.c_list + sum_m q_m . pq[m][code_m].  The interleaved layout
+//     has its own scan (ivfpq_scan.cu), vector-major codes (8-bit, or packed below 8 bits) the other.
+// Kernel timing names: ivfflat_scan, ivfsq_scan, ivfpq_scan, ivfpq_scan_packed (vector-major, nbits < 8).
+void runIvfScan(GpuResources* res, int device, const IvfScanLayout& lists, const IvfScanCall& call);
+
 // ---------------------------------------------------------------- ivfsq_scan.cu
 // ScalarQuantizer::QuantizerType values (faiss/impl/ScalarQuantizer.h:27-34) the GPU index accepts
 enum SqQuantizerType {
@@ -367,37 +347,6 @@ void runSqEncode(
 // shared-memory bytes of the per-(query, probe) decode tables of the IVF-SQ scan
 size_t ivfSqScanTableBytes(int d);
 
-// IVF-SQ list scan (role of the reference GPU IVFFlatScan with a scalar-quantiser codec): decode folded into
-// per-(query, probe) tables, lists in the CPU's [len][codeSize] layout.  decodeMB = m[d] | b[d] with the
-// decode x_i = m_i + b_i * code_i.  Distance forms follow faiss/impl/scalar_quantizer/scanners.h:44-135:
-// L2 on the residual q - c_list when byResidual; IP adds the coarse distance to every distance when byResidual.
-void runIvfSqScan(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nq,
-        int d,
-        const idx_t* probes,
-        const float* coarseDis,
-        int nprobe,
-        const float* coarseCentroids,
-        bool byResidual,
-        int qtype,
-        const float* decodeMB,
-        const int64_t* listStart,
-        const int* listLen,
-        const uint8_t* arenaCodes,
-        const idx_t* arenaIds,
-        int64_t arenaElems,
-        int codeSize,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const uint32_t* slotMask = nullptr, // SearchParameters::sel over the arena, or null
-        const IvfSlotOutput* slots = nullptr); // the slot-keeping search, or null
-
 // ---- "rotated, interleaved-by-32" PQ code layout (native storage for M % 16 == 0, M <= 32) ----
 // List-relative vector v = 32*g + t is stored in group g; byte position j of the vector holds
 // code[(j + t) % M] and lives at  g*32*M + (j/16)*512 + t*16 + (j%16).  A warp therefore loads a
@@ -428,37 +377,6 @@ void runIvfPqListFromInterleaved(const uint8_t* listCodes, int64_t len, int M, u
 // T2[l][c][m] = ||y_{m,c}||^2 + 2 <centroid_l restricted to sub-space m, y_{m,c}>   (pqT = [256][M][dsub])
 void runIvfPqPrecomputeTerm2(
         const float* coarse, const float* pqT, int64_t nlist, int d, int M, float* term2, cudaStream_t stream);
-
-// scan over the interleaved layout; pqCentroidsT is the [ksub][M][dsub] transpose of pqCentroids.
-// nibble: 4-bit PQ with M sub-quantisers stored as M/2 code bytes (nibble pairs, byte j = code 2j | code 2j+1
-// << 4), scanned as M/2 "8-bit" codes over the pair table T'[j][b] = T[2j][b & 15] + T[2j+1][b >> 4];
-// pqCentroidsT is then [16][M][dsub] and M/2 must be 16 or 32.  No precomputed tables.
-void runIvfPqScanInterleaved(
-        GpuResources* res,
-        int device,
-        const float* Q,
-        int64_t nq,
-        int d,
-        const idx_t* probes,
-        const float* coarseDis,
-        int nprobe,
-        const float* coarseCentroids,
-        const float* pqCentroidsT,
-        const float* term2, // precomputed [nlist][256][M] table (L2) or null
-        int M,
-        bool nibble,
-        const int64_t* listStart,
-        const int* listLen,
-        const uint8_t* arenaCodes,
-        const idx_t* arenaIds,
-        int64_t arenaElems,
-        int k,
-        MetricType metric,
-        float* outD,
-        idx_t* outI,
-        cudaStream_t stream,
-        const uint32_t* slotMask = nullptr, // SearchParameters::sel over the arena, or null
-        const IvfSlotOutput* slots = nullptr); // the slot-keeping search, or null
 
 // ---------------------------------------------------------------- cagra_build.cu
 // G0[rows[i]] for a batch of rows: the exact fp32 distances of each row's cand [nb][nc] (IVF-PQ ids; -1 skipped), the
